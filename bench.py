@@ -1,7 +1,8 @@
 #!/usr/bin/env python3
-"""bench.py -- registrations/sec of the VGICP hot path on B200 (BASELINE.json metric), one JSON line on stdout.
+"""bench.py -- registrations/sec of the VGICP hot path on H100 (BASELINE.json metric), one JSON line on stdout.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload c2|c2_direct1|c3|c4|c4_direct1|c5]
+                    [--dump-outputs DIR]
 
 Workload (N=1 default, BASELINE configs[1]): the reference's benchmark pair (tests/golden/pair_0p1.npz = data/251370668.pcd
 vs 251371071.pcd after align.cpp's filter + ApproximateVoxelGrid(0.1): 17047 / 17334 points), FastVGICPCuda, DIRECT27,
@@ -10,8 +11,7 @@ voxel_res 1.0, k=20, PLANE, LM defaults, identity initial guess.
 One registration follows the reference's "100times" protocol (src/align.cpp:72-81): clearTarget, clearSource,
 setInputTarget (upload, kNN, covariances, voxel map), setInputSource (upload, kNN, covariances), align.
 One *step* = one registration on each of S concurrent streams of the GPU (--streams, default 8 at every N: one host thread and one
-handle per stream; a 17k-pt registration is a chain of small latency-bound kernels, so one stream cannot fill 148 SMs; the rate
-saturates at 8 streams).  Host threads are pinned to the cores of the GPU's NUMA node, an own slice per rank.
+handle per stream; a 17k-pt registration is a chain of small latency-bound kernels, so one stream cannot fill 132 SMs).  Host threads are pinned to the cores of the GPU's NUMA node, an own slice per rank.
 
   value  : registrations/s with the clouds already resident in HBM when the timed region starts (device pointers
            through the C ABI); device time from a common start event to the last stream's end event; every registration
@@ -19,8 +19,8 @@ saturates at 8 streams).  Host threads are pinned to the cores of the GPU's NUMA
   e2e    : the same through the reference-facing class FastVGICPCuda with HOST (pinned) buffers: H2D of both clouds and D2H
            of the aligned cloud + pose inside the timed region.
   single_stream: the sequential protocol on one stream (latency), L2 flushed between registrations.
-  roofline: dominant kernel group of the step, algorithmic bytes (SURVEY.md 8d) / CUDA-event time, against MEASURED_PEAKS.json;
-           traffic = ncu DRAM bytes (profiles/traffic.json, quoted only while it matches the CUDA sources being run).
+  roofline: dominant kernel group of the step, algorithmic bytes (SURVEY.md 8d) / CUDA-event time, against MEASURED_PEAKS.json
+           when present, else the H100 SXM data-sheet HBM3 bandwidth.
   cpu_baseline: the reference's own CPU implementation of the path (OpenMP FastVGICP, restated in oracle/ because the
            reference cannot be compiled here) on 32 pinned host cores, median of >= 30 registrations; plus the FastGICP single-thread
            row of BASELINE config 1.
@@ -31,6 +31,11 @@ saturates at 8 streams).  Host threads are pinned to the cores of the GPU's NUMA
 
 N>1 (torchrun): the 17k-pt path does not shard usefully (SURVEY 8e) -> replicas, S registration streams per GPU, no
 data-path collective; value = N*S*K registrations / max-over-ranks time ("weak" scaling).  The c4 record is the sharded path.
+
+--dump-outputs DIR: after the timed steps, what the timed path returned in its last step, as DIR/<name>.npy (rank 0): per stream
+the pose, Hessian, iteration count and convergence flag of the resident arm (`value`), and the pose and aligned source cloud of
+the end-to-end arm (`e2e`); the reference arm writes the pose and Hessian of its last registration.  Inputs are seeded, so two
+builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -45,7 +50,7 @@ import numpy as np
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 # 8 handles x 2 streams alias onto the default 8 hardware work queues and wait on each other; 32 queues (read by the driver when the context is
-# created) give +5..9 % registrations/s at 8 handles, +20 % at 16 (profiles/r02_connections_sweep.txt).  fast_gicp_b200.core sets the same default.
+# created) let them run concurrently.  fast_gicp_b200.core sets the same default.
 os.environ.setdefault("CUDA_DEVICE_MAX_CONNECTIONS", "32")
 
 _REAL_STDOUT = sys.stdout
@@ -191,8 +196,10 @@ def run_reference_arm(args, w, rank, world):
     times = []
     for _ in range(args.steps * per_step):
         t0 = time.perf_counter()
-        cpu_one_registration(w, offs, threads)
+        last = cpu_one_registration(w, offs, threads)
         times.append(time.perf_counter() - t0)
+    if args.dump_outputs and times:
+        write_dump(args.dump_outputs, {"reference_pose": np.asarray(last.T, dtype=np.float64), "reference_hessian": np.asarray(last.H, dtype=np.float64)})
     med = float(np.median(times))
     value = 1.0 / med
     # BASELINE config 1: FastGICP, single thread (fast_gicp_impl.hpp:117-301 restated), same pair; a reported row, not the arm's value
@@ -237,7 +244,7 @@ def gpu_numa_node(torch, local_rank):
 
 def pin_rank_threads(torch, local_rank, world):
     """Keep this rank's host threads (one per registration stream) on cores of its GPU's NUMA node, an own slice per rank: with 8
-    ranks x 8 spinning threads on two sockets the scheduler otherwise migrates them across nodes (SCALE_r01: e2e efficiency 0.81)."""
+    ranks x 8 spinning threads on two sockets the scheduler otherwise migrates them across nodes."""
     node = gpu_numa_node(torch, local_rank)
     if node is None:
         return None
@@ -264,16 +271,21 @@ def pin_rank_threads(torch, local_rank, world):
         return None
 
 
-def source_hash():
-    """Hash of the CUDA sources: profiles/traffic.json (ncu DRAM bytes per launch) is only quoted while it matches."""
-    import hashlib
+DUMP_MAX_BYTES = 64 << 20
 
-    h = hashlib.sha256()
-    d = os.path.join(ROOT, "fast_gicp_b200", "csrc")
-    for f in sorted(os.listdir(d)):
-        if f.endswith((".cu", ".cuh", ".hpp")):
-            h.update(open(os.path.join(d, f), "rb").read())
-    return h.hexdigest()[:16]
+
+def write_dump(dirname, arrays, sampled=()):
+    """--dump-outputs: DIR/<name>.npy per array (float32 / float64).  When the total would exceed DUMP_MAX_BYTES, the arrays named in
+    `sampled` (point clouds, points along axis -2) keep a fixed, seeded sample of their points, in order."""
+    os.makedirs(dirname, exist_ok=True)
+    fixed = sum(a.nbytes for n, a in arrays.items() if n not in sampled)
+    big = sum(a.nbytes for n, a in arrays.items() if n in sampled)
+    for name, a in arrays.items():
+        if name in sampled and fixed + big > DUMP_MAX_BYTES:
+            keep = max(1, int(a.shape[-2] * (DUMP_MAX_BYTES - fixed) / big))
+            rows = np.sort(np.random.default_rng(0).choice(a.shape[-2], size=keep, replace=False))
+            a = np.take(a, rows, axis=-2)
+        np.save(os.path.join(dirname, name + ".npy"), a)
 
 
 # --------------------------------------------------------------------------------------------- C4 (1M-point pair)
@@ -419,13 +431,14 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--workload", default="c2")
     ap.add_argument("--streams", type=int, default=8,
-                    help="concurrent registration streams per GPU (host thread + handle each); the same at every N (8 reach 98 %% of the 16-stream rate and "
-                         "leave the host cores of a NUMA node to the ranks that share it)")
+                    help="concurrent registration streams per GPU (host thread + handle each); the same at every N (leaves the host cores of a NUMA node to "
+                         "the ranks that share it)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-c4", action="store_true", help="skip the 1M-point sub-record (config 4: evaluation roofline at N=1, sharded registration at N>1)")
     ap.add_argument("--e2e-impl", default="class", choices=["class", "batch"],
                     help="end-to-end arm: the FastVGICPCuda class from S Python threads (default, verified), or one vgicp_batch_register C call per timed region "
-                         "(include/vgicp_batch_b200.h; not yet verified on hardware)")
+                         "(include/vgicp_batch_b200.h)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write what the timed path returned in its last step as DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
 
@@ -467,7 +480,7 @@ def main():
         if rank == 0:
             print("[bench %7.1fs] %s" % (time.perf_counter() - _t0, msg), file=sys.stderr, flush=True)
 
-    # ---- input pool: P distinct pairs (the workload pair under random rigid motions), P * pair bytes > L2 (126 MB), so a
+    # ---- input pool: P distinct pairs (the workload pair under random rigid motions), P * pair bytes > 3 x L2 (50 MB), so a
     # pair has left the L2 by the time a stream comes back to it.  Resident copy for `value`, pinned host copy for `e2e`.
     pair_bytes = (n_t + n_s) * 12
     P = max(2 * S, int(np.ceil(160e6 / pair_bytes)))
@@ -488,7 +501,7 @@ def main():
     pool_s_h.copy_(pool_s)
     pool_t_np, pool_s_np = pool_t_h.numpy(), pool_s_h.numpy()
     aligned_h = [torch.empty((n_s, 3), dtype=torch.float32).pin_memory() for _ in range(S)]
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 126 MB L2 (single-stream latency pass)
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 50 MB L2 (single-stream latency pass)
     torch.cuda.synchronize()
 
     import threading
@@ -544,7 +557,7 @@ def main():
 
     def run_streams(step_fn, stream_list, steps):
         """`steps` registrations on each of the S streams (one host thread + one handle per stream), distinct pairs from the
-        pool; returns (device time from the common start event to the last stream's end event [ms], last result)."""
+        pool; returns (device time from the common start event to the last stream's end event [ms], the S results of the last step)."""
         start = torch.cuda.Event(enable_timing=True)
         ends = [torch.cuda.Event(enable_timing=True) for _ in range(S)]
         out = [None] * S
@@ -566,7 +579,7 @@ def main():
         for t_ in th:
             t_.join()
         torch.cuda.synchronize()
-        return max(start.elapsed_time(e) for e in ends), out[0]
+        return max(start.elapsed_time(e) for e in ends), out
 
     # ---- value: resident inputs, S concurrent streams
     note("handles ready")
@@ -576,10 +589,17 @@ def main():
     sampler = ClockSampler(local_rank) if rank == 0 else None
     l0 = sum(c.launch_count() for c in cores)
     t_wall0 = time.perf_counter()
-    total_ms, res = run_streams(step_resident, streams, K)
+    total_ms, res_all = run_streams(step_resident, streams, K)
     barrier()
     wall_s = time.perf_counter() - t_wall0
     launches = sum(c.launch_count() for c in cores) - l0
+    res = res_all[0]
+    dump = {}
+    if args.dump_outputs:
+        dump["value_pose"] = np.stack([pose_from_c(r.T) for r in res_all])
+        dump["value_hessian"] = np.stack([np.array(r.H, dtype=np.float64).reshape(6, 6).T for r in res_all])
+        dump["value_iterations"] = np.array([r.nr_iterations for r in res_all], dtype=np.float64)
+        dump["value_converged"] = np.array([r.converged for r in res_all], dtype=np.float64)
 
     # ---- e2e: host buffers through the reference-facing class, S concurrent streams
     note("value arm done")
@@ -602,11 +622,11 @@ def main():
             res_b = call(20, REG_PLANE)
             ev1.record()
             torch.cuda.synchronize()
-            return ev0.elapsed_time(ev1), pose_from_c(res_b[0].T)
+            return ev0.elapsed_time(ev1), [pose_from_c(r.T) for r in res_b[len(idx) - S:]], aligned_all[len(idx) - S: len(idx)]
 
         run_batch(W)
         barrier()
-        total_ms_e2e, T_e2e = run_batch(K)
+        total_ms_e2e, T_e2e_all, aligned_last = run_batch(K)
         barrier()
         launches_e2e = int(launches)  # the pool's handles are internal: same launches per registration as the resident arm
         e2e_api = "vgicp_batch_register (one C call for all registrations of the timed region; pinned host buffers, aligned clouds + poses read back)"
@@ -614,9 +634,14 @@ def main():
         run_streams(step_e2e, e2e_streams, W)
         barrier()
         l1 = sum(r.vgicp_cuda_.launch_count() for r in regs)
-        total_ms_e2e, T_e2e = run_streams(step_e2e, e2e_streams, K)
+        total_ms_e2e, T_e2e_all = run_streams(step_e2e, e2e_streams, K)
         barrier()
         launches_e2e = sum(r.vgicp_cuda_.launch_count() for r in regs) - l1
+        aligned_last = [a.numpy() for a in aligned_h]
+    T_e2e = T_e2e_all[0]
+    if args.dump_outputs:  # copied now: the single-stream pass below reuses the buffers
+        dump["e2e_pose"] = np.stack([np.asarray(T, dtype=np.float64) for T in T_e2e_all])
+        dump["e2e_aligned"] = np.stack([np.array(a, dtype=np.float32) for a in aligned_last])
     clocks = sampler.stop() if sampler else None
 
     # ---- single-stream latency (the reference's sequential protocol), L2 flushed between registrations
@@ -713,7 +738,7 @@ def main():
     if os.path.exists(peaks_path):
         peak_gbs, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     else:
-        peak_gbs, peak_src = 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        peak_gbs, peak_src = 3350.0, "data sheet (H100 SXM HBM3 3.35 TB/s; not measured)"
     V, B = core.num_voxels(), core.num_buckets()
     # ---- config 4 (all ranks take part: sharded over the ranks when there are several)
     c4 = None
@@ -756,23 +781,16 @@ def main():
         avg_ms = ms / max(launches_g, 1e-9)
         ab = alg_bytes[cats[0]]
         ach = ab / (avg_ms * 1e-3) / 1e9
-        traffic = None  # ncu dram__bytes per launch, written by scripts/make_traffic.sh; quoted only while the kernels are the ones it measured
-        tpath = os.path.join(ROOT, "profiles", "traffic.json")
-        if os.path.exists(tpath):
-            tj = json.load(open(tpath))
-            vals = [tj[c] for c in cats if c in tj]
-            if tj.get("source_hash") == source_hash() and vals:
-                traffic = float(np.mean(vals))
-        return {"bound": "hbm", "kernel": gname, "achieved": ach, "peak": peak_gbs, "unit": "GB/s", "frac": ach / peak_gbs, "traffic": traffic, "peak_source": peak_src,
+        return {"bound": "hbm", "kernel": gname, "achieved": ach, "peak": peak_gbs, "unit": "GB/s", "frac": ach / peak_gbs, "peak_source": peak_src,
                 "avg_launch_ms": avg_ms, "algorithmic_bytes_per_launch": ab, "kernel_share_of_step": ms / total_kernel_ms}
 
     present = [g for g in groups if any(c in per_kernel for c in groups[g])]
     rl = {g: group_roofline(g) for g in present}
     dom = max(present, key=lambda g: rl[g]["kernel_share_of_step"])
     roofline = rl[dom]
-    roofline["note"] = ("at ~17k points every kernel is latency/issue-bound (one evaluation moves ~1 MB = 0.17 us at the HBM peak); the fraction is reported as the "
-                        "contract asks, the 1M-point numbers are in profiles/README.md")
-    roofline_other = {g: {k: rl[g][k] for k in ("achieved", "frac", "avg_launch_ms", "kernel_share_of_step", "algorithmic_bytes_per_launch", "traffic")} for g in present if g != dom}
+    roofline["note"] = ("at ~17k points every kernel is latency/issue-bound (one evaluation moves ~1 MB = 0.33 us at the data-sheet HBM bandwidth); the fraction is reported as the "
+                        "contract asks, the 1M-point numbers are in the c4 record")
+    roofline_other = {g: {k: rl[g][k] for k in ("achieved", "frac", "avg_launch_ms", "kernel_share_of_step", "algorithmic_bytes_per_launch")} for g in present if g != dom}
 
     note("profile pass done")
     cpu_baseline = None
@@ -809,6 +827,8 @@ def main():
         "wall_ms_per_step": 1e3 * wall_s / K, "host_placement": placement, "c4": c4, "published_configurations": extras,
         "pose_check": {"translation": [float(x) for x in T_val[:3, 3]], "e2e_vs_resident_max_abs": float(np.abs(np.asarray(T_e2e, dtype=np.float64) - T_val).max())},
     }
+    if args.dump_outputs:
+        write_dump(args.dump_outputs, dump, sampled=("e2e_aligned",))
     print(json.dumps(line), file=_REAL_STDOUT, flush=True)
     D.finalize()
 

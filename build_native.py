@@ -1,4 +1,4 @@
-"""Build the native library in-tree: fast_gicp_b200/lib/libvgicp_b200.so (sm_100a only, -lineinfo).
+"""Build the native library in-tree: fast_gicp_b200/lib/libvgicp_b200.so (sm_90a only, -lineinfo).
 
     python build_native.py [--force] [-v]
 
@@ -16,8 +16,8 @@ CSRC = os.path.join(HERE, "csrc")
 LIB_DIR = os.path.join(HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libvgicp_b200.so")
 
-NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]  # H100 (Hopper); the image carries no other architecture and no PTX
+NVCC_FLAGS = GENCODE + [
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC,-fvisibility=hidden,-O3",
 ]
@@ -63,7 +63,7 @@ def build_native(force=False, verbose=False):
         cmd = [_nvcc()] + NVCC_FLAGS + extra + (["-Xptxas", "-v"] if verbose else []) + ccbin + ["-c", "-o", obj, os.path.join(CSRC, src)]
         subprocess.check_call(cmd, env=env)
         objs.append(obj)
-    subprocess.check_call([_nvcc(), "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", LIB_PATH] + ccbin + objs, env=env)
+    subprocess.check_call([_nvcc()] + GENCODE + ["-shared", "-o", LIB_PATH] + ccbin + objs, env=env)
     return LIB_PATH
 
 

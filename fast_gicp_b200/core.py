@@ -1,7 +1,7 @@
 """ctypes binding of the C ABI (include/vgicp_b200.h): `Core` mirrors fast_gicp::cuda::FastVGICPCudaCore
 (reference include/fast_gicp/cuda/fast_vgicp_cuda.cuh:28-92) method for method.
 
-There is no CPU fallback: importing this module without the built library, or creating a Core without a B200, raises.
+There is no CPU fallback: importing this module without the built library, or creating a Core without an H100, raises.
 """
 import ctypes as C
 import os
@@ -10,8 +10,7 @@ import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 # Several handles in one process (each owns two streams) alias onto the default 8 hardware work queues and wait on each other; the driver reads
-# this when the context is created.  Measured: +5..9 % registrations/s at 8 handles, +20 % at 16 (profiles/r02_connections_sweep.txt).  A value
-# the caller has set wins.  C/C++ callers export it themselves (INTEGRATION.md 7).
+# this when the context is created.  A value the caller has set wins.  C/C++ callers export it themselves (INTEGRATION.md 7).
 os.environ.setdefault("CUDA_DEVICE_MAX_CONNECTIONS", "32")
 LIB_PATH = os.environ.get("VGICP_B200_LIB") or os.path.join(_HERE, "lib", "libvgicp_b200.so")  # override only for A/B experiments
 
@@ -196,7 +195,7 @@ class Core:
         rc = self._lib.vgicp_create(int(device), C.byref(self._h))
         if rc != OK:
             self._h = None
-            raise VgicpError(rc, "vgicp_create failed (needs a CUDA device with an sm_100a image; no CPU fallback)")
+            raise VgicpError(rc, "vgicp_create failed (needs a CUDA device with an sm_90a image; no CPU fallback)")
 
     def close(self):
         if getattr(self, "_h", None):

@@ -33,7 +33,7 @@ public:
     regularization_method_ = RegularizationMethod::PLANE;
     neighbor_search_method_ = NearestNeighborMethod::CPU_PARALLEL_KDTREE;
     int rc = vgicp_create(device, &vgicp_cuda_);
-    if (rc != VGICP_OK) throw std::runtime_error("FastVGICPCuda: vgicp_create failed (a CUDA device with an sm_100a image is required; there is no CPU fallback)");
+    if (rc != VGICP_OK) throw std::runtime_error("FastVGICPCuda: vgicp_create failed (a CUDA device with an sm_90a image is required; there is no CPU fallback)");
     check(vgicp_set_resolution(vgicp_cuda_, voxel_resolution_));
     check(vgicp_set_kernel_params(vgicp_cuda_, 0.5, 3.0));
   }

@@ -28,7 +28,7 @@ protected:
 public:
   explicit NDTCuda(int device = 0) : Base() {  // ndt_cuda_impl.hpp:11-14 + NDTCudaCore ctor ndt_cuda.cu:13-23
     this->reg_name_ = "NDTCuda";
-    if (vgicp_create(device, &ndt_cuda_) != VGICP_OK) throw std::runtime_error("NDTCuda: vgicp_create failed (a CUDA device with an sm_100a image is required)");
+    if (vgicp_create(device, &ndt_cuda_) != VGICP_OK) throw std::runtime_error("NDTCuda: vgicp_create failed (a CUDA device with an sm_90a image is required)");
     check(vgicp_set_problem(ndt_cuda_, 2));                                     // distance_mode = D2D
     check(vgicp_set_neighbor_search_method(ndt_cuda_, VGICP_DIRECT7, 0.0));     // DIRECT7
   }

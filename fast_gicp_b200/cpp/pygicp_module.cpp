@@ -48,7 +48,7 @@ static Cloud::Ptr eigen2pcl(const ArrD& points) {  // main.cpp:36-44 (double -> 
 // filter's output (points and order) bit for bit (tests/test_input_prep.py); no host implementation is kept in the product.
 static Cloud::Ptr approximate_voxel_grid(const Cloud& in, float leaf) {
   static vgicp_prep_handle prep = nullptr;  // one per process, device 0 like the registration objects' default
-  if (!prep && vgicp_prep_create(0, &prep) != 0) throw std::runtime_error("pygicp: the input-preparation library found no usable CUDA device (sm_100a required)");
+  if (!prep && vgicp_prep_create(0, &prep) != 0) throw std::runtime_error("pygicp: the input-preparation library found no usable CUDA device (sm_90a required)");
   auto out = pcl::make_shared<Cloud>();
   const size_t n = in.points.size();
   if (n == 0) return out;
@@ -116,7 +116,7 @@ static py::array_t<double> align_points(const ArrD& target, const ArrD& source, 
   }
   if (method != "VGICP_CUDA") {
     if (method == "GICP" || method == "VGICP")
-      std::cerr << "error: this build provides only VGICP_CUDA and NDT_CUDA (the B200 paths); " << method << " is outside it" << std::endl;
+      std::cerr << "error: this build provides only VGICP_CUDA and NDT_CUDA (the GPU paths); " << method << " is outside it" << std::endl;
     else
       std::cerr << "error: unknown registration method " << method << std::endl;
     return to_numpy(Eigen::Matrix4d::Identity());

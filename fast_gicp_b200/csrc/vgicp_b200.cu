@@ -295,7 +295,7 @@ int set_neighbors(vgicp_handle h, Cloud& c, int k, const int* idx, size_t nk) {
   // one pass over the table, the verdict comes back with the synchronisation the copy needs anyway
   int* bad = h->map.d_counters + 8;
   CU_TRY(h, cudaMemsetAsync(bad, 0, sizeof(int), c.st));
-  KLAUNCH_ST(h, c.st, VGICP_PROF_OTHER, k_validate_indices<<<blocks_for(nk, 256) < 1184 ? blocks_for(nk, 256) : 1184, 256, 0, c.st>>>(c.nbr.p, nk, c.n, bad));
+  KLAUNCH_ST(h, c.st, VGICP_PROF_OTHER, k_validate_indices<<<blocks_for(nk, 256) < 8 * kNumSMs ? blocks_for(nk, 256) : 8 * kNumSMs, 256, 0, c.st>>>(c.nbr.p, nk, c.n, bad));
   CU_TRY(h, cudaGetLastError());
   CU_TRY(h, cudaMemcpyAsync(h->map.h_counters + 8, bad, sizeof(int), cudaMemcpyDeviceToHost, c.st));
   CU_TRY(h, cudaStreamSynchronize(c.st));
@@ -565,7 +565,7 @@ int voxelmap_finish(vgicp_handle h, Cloud& t, VoxelMap& m) {
     CU_TRY(h, cudaMemsetAsync(m.sort_scratch.p, 0, sbytes, t.st));
     const int kb = blocks_for(n, kSortThreads);
     KLAUNCH_ST(h, t.st, VGICP_PROF_VOXELMAP,
-               k_voxel_sort_keys<<<kb < 1184 ? kb : 1184, kSortThreads, 0, t.st>>>(m.slot_of_point.p, m.buckets.p, n, invalid, passes, m.sort_keys[0].p, reinterpret_cast<unsigned*>(m.sort_scratch.p)));
+               k_voxel_sort_keys<<<kb < 8 * kNumSMs ? kb : 8 * kNumSMs, kSortThreads, 0, t.st>>>(m.slot_of_point.p, m.buckets.p, n, invalid, passes, m.sort_keys[0].p, reinterpret_cast<unsigned*>(m.sort_scratch.p)));
     int nl = 0;
     cudaError_t se = cudaSuccess;
     KLAUNCH_ST(h, t.st, VGICP_PROF_VOXELMAP,
@@ -653,8 +653,7 @@ LinLaunch make_lin_launch(vgicp_handle h) {
   const int n_off = a.n_off;
   const bool wide = a.n < 400000 && n_off > 1;
   // small clouds: split a point's cells over 3 (DIRECT27: whole z-columns), 4 (<= 7 offsets) or 8 lanes.  With the hits compacted
-  // before the arithmetic the split costs no lane efficiency, so it is used under both execution hints (measured: 7.1k vs 6.9k
-  // registrations/s at 16 streams, 0.42 vs 0.50 ms single-stream)
+  // before the arithmetic the split costs no lane efficiency, so it is used under both execution hints
   const bool cols = h->offset_mode == 27;
   L.G = !wide ? 1 : (cols ? 3 : (n_off <= 7 ? 4 : 8));
   {
@@ -874,7 +873,7 @@ int evaluate_spec(vgicp_handle h, const double* T, double* err_old, double* H36,
 // =====================================================================================================================
 extern "C" {
 
-const char* vgicp_version(void) { return "vgicp_b200 0.1 (sm_100a)"; }
+const char* vgicp_version(void) { return "vgicp_b200 0.1 (sm_90a)"; }
 
 int vgicp_create(int device, vgicp_handle* out) {
   if (!out) return VGICP_ERR_INVALID_ARGUMENT;
@@ -888,7 +887,7 @@ int vgicp_create(int device, vgicp_handle* out) {
   { const char* e = getenv("VGICP_LIN_G"); h->force_lin_g = e ? atoi(e) : 0; }
   { const char* e = getenv("VGICP_LIN_STREAM"); h->lin_stream = e ? atoi(e) : 1; }
   DeviceGuard g(device);
-  // the kernel image is sm_100a only: fail loudly on anything else instead of falling back
+  // the kernel image is sm_90a only: fail loudly on anything else instead of falling back
   cudaFuncAttributes fa;
   if (cudaFuncGetAttributes(&fa, k_linearize<1, true, 1>) != cudaSuccess) {
     cudaGetLastError();

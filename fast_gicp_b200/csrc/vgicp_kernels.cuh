@@ -1,4 +1,4 @@
-// vgicp_kernels.cuh -- hand-written sm_100a kernels of the VGICP hot path.
+// vgicp_kernels.cuh -- hand-written sm_90a (H100) kernels of the VGICP hot path.
 //
 // Stage 1  k-NN + covariance + regularisation   (reference: brute_force_knn.cu, covariance_estimation.cu,
 //                                                covariance_estimation_rbf.cu, covariance_regularization.cu)
@@ -27,7 +27,7 @@
 namespace vgicp {
 
 constexpr int kLinThreads = 128;     // block size of the linearize kernel
-constexpr int kLinMaxBlocks = 592;   // 4 x 148 SMs: upper bound on partial sums the last block has to fold (more resident warps only thrash L1: measured)
+constexpr int kLinMaxBlocks = 4 * kNumSMs;  // 4 blocks per SM: upper bound on partial sums the last block has to fold (more resident warps only thrash L1: measured)
 constexpr int kLinValues = 28;       // 21 unique H + 6 b + 1 err
 constexpr int kLinStride = 32;       // row length of the partial-sum arrays (the speculative evaluation carries 29 values)
 constexpr int kLinOutCommError = 44; // out[44]: 1.0 when a sharded evaluation timed out waiting for a peer (the sums are then incomplete)
@@ -357,7 +357,7 @@ __global__ void __launch_bounds__(128) k_voxel_reduce(const float4* __restrict__
     return (double)reinterpret_cast<const float*>(covB + i)[c - 7];
   };
   // 32 points per round: one coalesced load of their indices, then the gathers sixteen at a time in flight, added in point order
-  // (a dependent index -> gather -> add chain per point made the largest voxel -- 158 points at 17 k -- a 40 us tail)
+  // (a dependent index -> gather -> add chain per point made the largest voxel -- 158 points at 17 k -- a long tail)
   double sum = 0.0;
   for (int j0 = se.x; j0 < se.y; j0 += 32) {
     const int nb = min(32, se.y - j0);
@@ -724,9 +724,9 @@ __device__ __forceinline__ void lin_accumulate(const LinArgs& a, const Pose& Tl,
 
 // block reduction (warp shuffles in float -> shared in double -> per-block partial), ticket, fixed-order fold by the last
 // block.  Returns true in every thread of the last block; the folded sums are then in fin[0][0..NV).
-// (Tried in round 2 and dropped: a first-level reduction over distributed shared memory inside 8-block clusters, so that the last
-// block folds grid/8 partials.  It bought 0.4 us of the 22.6 us of an evaluation at 17 k points and cost 16 % at 1 M points, where the
-// cluster placement constraint left SMs idle at the tail of the single wave.)
+// (Tried and dropped: a first-level reduction over distributed shared memory inside 8-block clusters, so that the last block folds
+// grid/8 partials.  It gained little at 17 k points and lost at 1 M points, where the cluster placement constraint left SMs idle
+// at the tail of the single wave.)
 template <int NV>
 __device__ __forceinline__ bool lin_reduce(const LinArgs& a, const float* sum, double (*fin)[kLinStride]) {
   // ---- block reduction: warp shuffles (float) -> shared (double) -> per-block partial ----
@@ -761,7 +761,7 @@ __device__ __forceinline__ bool lin_reduce(const LinArgs& a, const float* sum, d
     const int v = threadIdx.x & 31, chain = threadIdx.x >> 5;  // kLinThreads == 128 -> 4 chains
     if (v < NV) {
       // ld.global.cg: coherent at L2 (the partials were written by other SMs), 16 independent loads in flight per
-      // round -- a dependent load->add chain over 148 blocks costs ~25 us of serialised L2 latency
+      // round -- a dependent load->add chain over hundreds of blocks serialises on L2 latency
       double s = 0.0;
       const double* part = a.partials + v;
       unsigned b = chain;
@@ -904,7 +904,7 @@ __global__ void __launch_bounds__(kLinThreads) k_linearize_spec(const LinArgs a)
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int kLinStreamTile = 128;     // points per tile (1 per thread)
 constexpr int kLinStreamStages = 4;
-constexpr int kLinStreamMaxBlocks = 1184;  // 8 x 148 SMs
+constexpr int kLinStreamMaxBlocks = 8 * kNumSMs;
 
 __device__ __forceinline__ unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(unsigned long long* bar, unsigned count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory"); }

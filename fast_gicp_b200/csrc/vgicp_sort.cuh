@@ -14,6 +14,8 @@
 
 namespace vgicp {
 
+constexpr int kNumSMs = 132;  // H100 SXM: the caps on grid-stride / persistent grids below are multiples of it
+
 constexpr int kSortRadixBits = 9;
 constexpr int kSortBins = 1 << kSortRadixBits;
 constexpr int kSortThreads = 256;
@@ -155,7 +157,7 @@ __device__ __forceinline__ void sort_pass_tile(SortTileSmem& sm, unsigned tile, 
   }
   if (tile > 0) {
     // walk back over the preceding tiles, kLook of them per round with all loads in flight (a dependent chain of single loads
-    // costs an L2 round trip per tile: 8 tiles x 2 digits were 11 us of the 13 us of a pass at 17 k points)
+    // costs an L2 round trip per tile, which dominated a pass at 17 k points)
     constexpr int kLook = 8;
 #pragma unroll
     for (int j = 0; j < J; j++) {
@@ -224,7 +226,7 @@ inline cudaError_t launch_sort_pairs(KeyT* k0, unsigned* v0, KeyT* k1, unsigned*
   const int tiles = sort_num_tiles(n);
   if (!hist_done) {
     int hb = (n + kSortThreads * 8 - 1) / (kSortThreads * 8);
-    k_sort_hist<KeyT><<<hb < 592 ? (hb > 0 ? hb : 1) : 592, kSortThreads, 0, stream>>>(k0, n, passes, hist);
+    k_sort_hist<KeyT><<<hb < 4 * kNumSMs ? (hb > 0 ? hb : 1) : 4 * kNumSMs, kSortThreads, 0, stream>>>(k0, n, passes, hist);
     if (launches) (*launches)++;
   }
   KeyT* kk[2] = {k0, k1};

@@ -699,13 +699,11 @@ __device__ __forceinline__ int level_for(float B, int l_min, int L, float s0, fl
 //      the bound are appended (ballot + prefix) to the warp's buffer in shared memory -- nothing is sorted while scanning;
 //   4. the buffer is tightened to at most 32 (64 for k > 32) keys by another bisection, the survivors are sorted once across the
 //      lanes (bitonic network on 64-bit keys) and the first k are the row, ascending in (d2, index).
-// Measured alternatives (round 2, 17 k-point fixture cloud, B200; all exact, all dropped):
-//   one thread per query, max-heap of the k best in shared memory   592 us  (1530 warp-instructions per query at 37 % lane efficiency,
-//                                                                            dependent shared-memory chains, a 3x tail)
-//   one thread per query, bisection + append buffer + rank sort      608 us
-//   this kernel with four consecutive queries per warp sharing the 27 table lookups      90 us  (fewer, longer warps)
-//   eight lanes per query, four queries per warp (segmented ballots / shuffles)          ~118 us (132 -> 207 us for the whole stage)
-//   this kernel                                                       43 us  (1200 warp-instructions per query, 69 % issue utilisation)
+// Alternatives tried and dropped (all exact, all slower on the 17 k-point fixture cloud):
+//   one thread per query, max-heap of the k best in shared memory  (low lane efficiency, dependent shared-memory chains, a long tail)
+//   one thread per query, bisection + append buffer + rank sort
+//   this kernel with four consecutive queries per warp sharing the 27 table lookups  (fewer, longer warps)
+//   eight lanes per query, four queries per warp (segmented ballots / shuffles)
 template <bool WIDE>
 __global__ void __launch_bounds__(kSearchWarps * 32) k_knn_search(GridArgs a, int force_whole_cloud) {
   __shared__ tkey sbuf[kSearchWarps][kWarpBuf];
@@ -1136,12 +1134,12 @@ cudaError_t launch_knn_grid(const float4* pts, int n, int k, int* nbr, unsigned 
   const int nb = (n + 255) / 256;
   if ((e = cudaMemsetAsync(ff_begin, 0xFF, ff_bytes, stream)) != cudaSuccess) return e;
   if ((e = cudaMemsetAsync(z_begin, 0, z_bytes, stream)) != cudaSuccess) return e;
-  k_grid_bbox<<<nb < 592 ? nb : 592, 256, 0, stream>>>(pts, n, a.bbox_min, a.bbox_max);
-  k_grid_codes<<<nb < 1184 ? nb : 1184, kSortThreads, 0, stream>>>(a, passes, reinterpret_cast<unsigned*>(sort_scratch));
+  k_grid_bbox<<<nb < 4 * kNumSMs ? nb : 4 * kNumSMs, 256, 0, stream>>>(pts, n, a.bbox_min, a.bbox_max);
+  k_grid_codes<<<nb < 8 * kNumSMs ? nb : 8 * kNumSMs, kSortThreads, 0, stream>>>(a, passes, reinterpret_cast<unsigned*>(sort_scratch));
   nl += 2;
   if ((e = launch_sort_pairs<unsigned long long>(codes0, vals0, codes1, vals1, n, key_bits, sort_scratch, true, pts, a.sorted, &nl, stream)) != cudaSuccess) return e;
   a.codes = (passes & 1) ? codes1 : codes0;
-  k_grid_levels<<<nb < 592 ? nb : 592, 256, 0, stream>>>(a);
+  k_grid_levels<<<nb < 4 * kNumSMs ? nb : 4 * kNumSMs, 256, 0, stream>>>(a);
   k_grid_table<<<dim3(nb, L), 256, 0, stream>>>(a);
   nl += 2;
   const int nq = q_end > q_begin ? q_end - q_begin : 0;
@@ -1150,7 +1148,7 @@ cudaError_t launch_knn_grid(const float4* pts, int n, int k, int* nbr, unsigned 
     if (k <= 32) k_knn_search<false><<<sblocks, kSearchWarps * 32, 0, stream>>>(a, force_bruteforce);
     else k_knn_search<true><<<sblocks, kSearchWarps * 32, 0, stream>>>(a, force_bruteforce);
     int hblocks = (nq + kKnnGridWarps - 1) / kKnnGridWarps;
-    if (hblocks > 148 * 4) hblocks = 148 * 4;  // persistent: items pulled from a counter
+    if (hblocks > 4 * kNumSMs) hblocks = 4 * kNumSMs;  // persistent: items pulled from a counter
     if (k <= 32) k_knn_deferred<false><<<hblocks, kKnnGridWarps * 32, 0, stream>>>(a);
     else k_knn_deferred<true><<<hblocks, kKnnGridWarps * 32, 0, stream>>>(a);
     nl += 2;

@@ -44,7 +44,7 @@ class InputPrep:
         rc = self._lib.vgicp_prep_create(int(device), C.byref(self._h))
         if rc:
             self._h = None
-            raise PrepError(rc, "vgicp_prep_create failed (no sm_100a device?)")
+            raise PrepError(rc, "vgicp_prep_create failed (no sm_90a device?)")
 
     def close(self):
         if getattr(self, "_h", None):

@@ -212,7 +212,7 @@ class NDTCuda(LsqRegistration):
 
 
 class FastVGICPCuda(LsqRegistration):
-    """Fast Voxelized GICP on a B200 behind the reference's FastVGICPCuda interface."""
+    """Fast Voxelized GICP on an H100 behind the reference's FastVGICPCuda interface."""
 
     def __init__(self, device=0):
         super().__init__()

@@ -1,5 +1,5 @@
 /*
- * vgicp_b200.h -- C ABI of libvgicp_b200.so, the Blackwell (sm_100a) VGICP registration core.
+ * vgicp_b200.h -- C ABI of libvgicp_b200.so, the H100 (sm_90a) VGICP registration core.
  *
  * This is the drop-in seam for fast_gicp's device core: every function below replaces one member of
  * fast_gicp::cuda::FastVGICPCudaCore (reference include/fast_gicp/cuda/fast_vgicp_cuda.cuh:28-92, implemented in
@@ -44,7 +44,7 @@ typedef enum {
   VGICP_ERR_BAD_STATE = 2,        /* a prerequisite call is missing (e.g. covariances before the cloud) */
   VGICP_ERR_CUDA = 3,             /* a CUDA runtime call failed; message has the cudaError string */
   VGICP_ERR_UNSUPPORTED = 4,      /* regularisation method not implemented on the GPU path (as in the reference) */
-  VGICP_ERR_NO_DEVICE = 5,        /* no CUDA device / kernel image not loadable on this GPU (needs sm_100a) */
+  VGICP_ERR_NO_DEVICE = 5,        /* no CUDA device / kernel image not loadable on this GPU (needs sm_90a) */
   VGICP_ERR_COMM = 6              /* multi-GPU exchange failed */
 } vgicp_status;
 
@@ -203,12 +203,12 @@ VGICP_API int vgicp_ndt_create_voxelmaps(vgicp_handle h);
 /* Execution hint: 0 = latency (default: the persistent k-NN kernel takes 4 blocks per SM; every evaluation writes its 43 doubles
  * straight into mapped host memory and the calling thread spins on a completion word), 1 = throughput / polite (2 k-NN blocks per SM;
  * evaluations are read back with a copy and a stream wait, so the host thread sleeps instead of spinning).  Results are identical.
- * On a B200 host with cores to spare the latency shape is also the faster one with 16 handles per GPU (bench.py uses it). */
+ * bench.py uses the latency shape. */
 VGICP_API int vgicp_set_execution_hint(vgicp_handle h, int hint);
 /* vgicp_align driver: 1 = host-driven loop over the evaluation kernels (default; one 344-byte readback per evaluation, like
  * the reference), 0 = device-resident loop (the LM state machine runs in the last block of each evaluation kernel, the host
- * reads one state block back per chunk of launches).  Both walk the same iterates; measured on B200 the serial double-precision
- * LM step on one GPU thread costs about what the host round trip costs, so the host-driven loop stays the default. */
+ * reads one state block back per chunk of launches).  Both walk the same iterates; the serial double-precision LM step
+ * on one GPU thread costs about what the host round trip saves, so the host-driven loop stays the default. */
 VGICP_API int vgicp_set_align_mode(vgicp_handle h, int mode);
 /* k-NN engine used by find_*_neighbors: 0 = multi-level hash grid (default), 1 = warp-cooperative scan of the whole cloud,
  * 2 = one-thread-per-query scan (the shape of the reference's brute_force_knn.cu).  All three return identical rows. */

@@ -1,13 +1,13 @@
 /* vgicp_batch_b200.h -- many registrations, one call: the reference's benchmark and odometry loops (src/align.cpp:72-81 "100times",
  * src/kitti.cpp:97-118) call clear + setInputTarget + setInputSource + align once per pair from one host thread.  A 17k-point
- * registration is a chain of ~30 small latency-bound launches and cannot fill a B200; the throughput configuration runs several
+ * registration is a chain of ~30 small latency-bound launches and cannot fill an H100; the throughput configuration runs several
  * registrations concurrently, one vgicp handle (own CUDA streams) and one host thread each (DESIGN.md 5).  This small host-side
  * library (lib/libvgicp_batch_b200.so, plain C++ over the public C ABI of vgicp_b200.h, no CUDA code of its own) packages that:
  * a pool of handles on one device, worker threads pulling pairs from a shared counter.  Every pair goes through vgicp_register
  * on one handle exactly as a sequential caller would run it, so the results are those of the sequential loop, bit for bit,
  * whatever the interleaving.  (SURVEY.md 8b lists it as the `vgicp_batch_align` extension.)
  *
- * Checked on a B200 by tests/test_batch.py (24 pairs over 6 handles against the sequential loop: same poses, counters and aligned clouds,
+ * Checked by tests/test_batch.py (24 pairs over 6 handles against the sequential loop: same poses, counters and aligned clouds,
  * bit for bit).  A device-batched execution path (one launch per stage over all pairs) is not built: DESIGN.md 8. */
 #ifndef VGICP_BATCH_B200_H
 #define VGICP_BATCH_B200_H

@@ -4,9 +4,8 @@
  *   src/align.cpp:136-147, src/kitti.cpp:80-82, src/python/main.cpp:46-62,81-91   pcl::ApproximateVoxelGrid<PointXYZ>
  * A separate small library (lib/libvgicp_prep_b200.so): the registration library does not depend on it.
  *
- * STATUS (round 1): the algorithm is pinned on the CPU side (oracle/vgicp_oracle.c: orc_approximate_voxel_grid reproduces the
- * point counts the reference prints, README.md:116, and the committed benchmark fixture bit for bit); the CUDA implementation is
- * compiled for sm_100a and covered by tests/test_gpu_input_prep.py, which has not run on hardware yet.
+ * The algorithm is pinned on the CPU side (oracle/vgicp_oracle.c: orc_approximate_voxel_grid reproduces the committed benchmark
+ * fixture bit for bit); the CUDA implementation is compiled for sm_90a and checked against it by tests/test_input_prep.py.
  *
  * pcl::ApproximateVoxelGrid is a streaming filter: each point goes to entry (ix*7171 + iy*3079 + iz*4231) & 511 of a 512-entry
  * history; an entry holding another voxel is flushed (its centroid emitted) first; what is left is flushed in entry order at the

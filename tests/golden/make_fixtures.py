@@ -1,11 +1,11 @@
 #!/usr/bin/env python3
 """Generate the committed golden input fixtures from the reference's own data files.
 
-Run in the build container only (needs /root/reference, which does not exist on the GPU box):
+Needs the data/ directory of a fast_gicp checkout:
 
-    python tests/golden/make_fixtures.py
+    python tests/golden/make_fixtures.py <fast_gicp>/data
 
-Reads  /root/reference/data/251370668.pcd (target), 251371071.pcd (source), relative.txt
+Reads  data/251370668.pcd (target), 251371071.pcd (source), relative.txt
 Writes tests/golden/pair_0p1.npz   -- the reference's benchmark inputs: near-origin filter
                                       (src/align.cpp:128-133) + ApproximateVoxelGrid(0.1) (src/align.cpp:136-147)
        tests/golden/pair_0p2.npz   -- the reference's test inputs: VoxelGrid(0.2) (src/test/gicp_test.cpp:55-65)
@@ -21,7 +21,6 @@ import os
 import sys
 import numpy as np
 
-REF = "/root/reference/data"
 OUT = os.path.dirname(os.path.abspath(__file__))
 
 
@@ -119,8 +118,9 @@ def voxel_grid(pts, leaf):
 
 
 def main():
-    if not os.path.isdir(REF):
-        sys.exit("needs /root/reference/data (build container only)")
+    if len(sys.argv) != 2 or not os.path.isdir(sys.argv[1]):
+        sys.exit("usage: make_fixtures.py <fast_gicp data/ directory>")
+    REF = sys.argv[1]
     tgt = read_pcd_xyz(os.path.join(REF, "251370668.pcd"))
     src = read_pcd_xyz(os.path.join(REF, "251371071.pcd"))
     assert tgt.shape == (69088, 3) and src.shape == (69792, 3)

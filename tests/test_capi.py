@@ -23,11 +23,11 @@ def test_header_symbols_all_exported():
     assert sorted(core.EXPORTED_SYMBOLS) == declared  # the binding knows exactly the header's surface
     for name in declared:
         assert hasattr(lib, name), name
-    assert b"sm_100a" in lib.vgicp_version()
+    assert b"sm_90a" in lib.vgicp_version()
 
 
-def test_library_is_sm100a_only():
-    """The fatbin carries exactly one image: sm_100a (no PTX fallback for other architectures)."""
+def test_library_is_sm90a_only():
+    """The fatbin carries exactly one image: sm_90a (no PTX fallback for other architectures)."""
     import subprocess
 
     from fast_gicp_b200 import core
@@ -36,7 +36,7 @@ def test_library_is_sm100a_only():
     if out.returncode != 0:
         pytest.skip("cuobjdump unavailable")
     archs = set(re.findall(r"sm_\d+a?", out.stdout))
-    assert archs == {"sm_100a"}, out.stdout
+    assert archs == {"sm_90a"}, out.stdout
 
 
 def test_no_cpu_fallback_without_gpu():

@@ -1,4 +1,4 @@
-"""Source sharding across GPUs (SURVEY.md 8e): needs >= 2 GPUs, skipped otherwise (run with `gpurun --gpus 2`)."""
+"""Source sharding across GPUs (SURVEY.md 8e): needs >= 2 GPUs, skipped otherwise."""
 import json
 import os
 import socket
