@@ -41,6 +41,7 @@ EXPORTED_SYMBOLS = [
     "vgicp_set_knn_mode", "vgicp_set_voxel_index", "vgicp_set_speculation", "vgicp_register", "vgicp_set_align_mode", "vgicp_get_fitness_score", "vgicp_set_execution_hint", "vgicp_set_problem", "vgicp_ndt_create_voxelmaps",
     "vgicp_comm_export", "vgicp_comm_init", "vgicp_comm_shutdown", "vgicp_comm_error", "vgicp_set_source_shard", "vgicp_clear_source_shard",
     "vgicp_comm_export_arena", "vgicp_comm_init_arena", "vgicp_set_stage1_sharding", "vgicp_set_source_covariances", "vgicp_set_target_covariances",
+    "vgicp_align_multi", "vgicp_evaluate_poses",
 ]
 PROF_NUM_CATEGORIES = 7
 
@@ -121,6 +122,8 @@ def load_library():
         "vgicp_compute_error": [hp, dp, dp, dp, dp],
         "vgicp_lsq_default_params": [C.POINTER(LsqParams)],
         "vgicp_align": [hp, dp, C.POINTER(LsqParams), C.POINTER(AlignResult)],
+        "vgicp_align_multi": [hp, dp, C.c_int, C.POINTER(LsqParams), C.POINTER(AlignResult)],
+        "vgicp_evaluate_poses": [hp, dp, C.c_int, dp, dp, dp, C.POINTER(C.c_int64)],
         "vgicp_transform_source": [hp, dp, C.c_void_p, C.c_size_t, C.c_size_t],
         "vgicp_get_launch_count": [hp, C.POINTER(C.c_uint64)],
         "vgicp_synchronize": [hp],
@@ -438,6 +441,38 @@ class Core:
         res = AlignResult()
         self._check(self._lib.vgicp_align(self._h, _dp(g), C.byref(params), C.byref(res)))
         return res
+
+    @staticmethod
+    def _poses_to_c(poses):
+        P = np.asarray(poses, dtype=np.float64)
+        if P.ndim != 3 or P.shape[1:] != (4, 4):
+            raise ValueError("poses must be (B, 4, 4)")
+        return np.ascontiguousarray(P.transpose(0, 2, 1)).reshape(-1)  # B x 16 doubles, column-major each
+
+    def align_multi(self, guesses, params=None):
+        """B registrations from the (B, 4, 4) initial guesses, evaluated together -> list of AlignResult;
+        result i equals align(guesses[i], params) bit for bit."""
+        g = self._poses_to_c(guesses)
+        B = len(g) // 16
+        params = params or default_params()
+        res = (AlignResult * max(B, 1))()
+        self._check(self._lib.vgicp_align_multi(self._h, _dp(g), B, C.byref(params), res))
+        return list(res)[:B]
+
+    def evaluate_poses(self, poses, want_H=False):
+        """-> (err (B,), H (B,6,6) | None, b (B,6) | None, n_corr (B,) int64): per pose what update_correspondences(T) +
+        compute_error(T, want_H) return, and the number of correspondences get_voxel_correspondences() would list."""
+        t = self._poses_to_c(poses)
+        B = len(t) // 16
+        err = np.zeros(B)
+        n_corr = np.zeros(B, dtype=np.int64)
+        H = np.zeros((B, 36)) if want_H else None
+        b = np.zeros((B, 6)) if want_H else None
+        self._check(self._lib.vgicp_evaluate_poses(self._h, _dp(t), B, _dp(err), _dp(H) if want_H else None, _dp(b) if want_H else None,
+                                                   n_corr.ctypes.data_as(C.POINTER(C.c_int64))))
+        if want_H:
+            H = H.reshape(B, 6, 6).transpose(0, 2, 1).copy()
+        return err, H, b, n_corr
 
     def register_raw(self, tgt_ptr, n_t, src_ptr, n_s, stride=12, on_device=False, k=20, reg=REG_PLANE, guess=None, params=None):
         """clear + setInputTarget + setInputSource + align in one C call (pointers: host, or device when on_device)."""

@@ -97,9 +97,11 @@ public:
 
 protected:
   virtual void computeTransformation(PointCloudSource& output, const Matrix4& guess) override {  // impl:144-148
-    check(vgicp_set_resolution(vgicp_cuda_, voxel_resolution_));
+    multiPrelude();
     Base::computeTransformation(output, guess);
   }
+  virtual vgicp_handle multiHandle() const override { return vgicp_cuda_; }
+  virtual void multiPrelude() override { check(vgicp_set_resolution(vgicp_cuda_, voxel_resolution_)); }
 
   virtual void transformSource(PointCloudSource& output, const Matrix4& T) override {  // pcl::transformPointCloud on the device
     output = *input_;

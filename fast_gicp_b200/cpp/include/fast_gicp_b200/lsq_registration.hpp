@@ -2,10 +2,15 @@
 // include/fast_gicp/gicp/lsq_registration.hpp:16-85 and impl/lsq_registration_impl.hpp:9-168 (same members, same LM /
 // Gauss-Newton logic in double); the 6x6 solve and SE(3) exponential come from csrc/lsq_math.hpp instead of Eigen.
 #pragma once
+#include <cstdint>
 #include <cstdio>
 #include <cstring>
 #include <iostream>
+#include <stdexcept>
+#include <string>
+#include <vector>
 
+#include "../../../../include/vgicp_b200.h"
 #include "../../../csrc/lsq_math.hpp"
 #include "compat.hpp"
 #include "gicp_settings.hpp"
@@ -69,7 +74,58 @@ public:
   virtual void clearSource() {}
   virtual void clearTarget() {}
 
+  // Multi-hypothesis alignment (not in the reference): one registration of the source per initial guess, the evaluations of all
+  // hypotheses sharing launches on the device (vgicp_align_multi).  T_out[i] and converged_out[i] are the final transformation and
+  // convergence flag of that registration; getFinalTransformation(), hasConverged() and the final Hessian are left alone.
+  void alignMulti(const std::vector<Matrix4>& guesses, std::vector<Matrix4>& T_out, std::vector<bool>& converged_out) {
+    T_out.clear();
+    converged_out.clear();
+    if (!input_ || !this->target_ || guesses.empty()) return;  // (pcl's align returns without inputs)
+    multiPrelude();
+    const int n = static_cast<int>(guesses.size());
+    std::vector<double> g(16 * guesses.size());
+    for (int i = 0; i < n; i++)
+      for (int k = 0; k < 16; k++) g[16 * i + k] = static_cast<double>(guesses[i].v[k]);
+    vgicp_lsq_params P;
+    vgicp_lsq_default_params(&P);
+    P.max_iterations = max_iterations_;
+    P.rotation_epsilon = rotation_epsilon_;
+    P.transformation_epsilon = transformation_epsilon_;
+    P.use_gauss_newton = lsq_optimizer_type_ == LSQ_OPTIMIZER_TYPE::GaussNewton ? 1 : 0;
+    P.lm_max_iterations = lm_max_iterations_;
+    P.lm_init_lambda_factor = lm_init_lambda_factor_;
+    std::vector<vgicp_align_result> r(guesses.size());
+    multiCheck(vgicp_align_multi(multiHandle(), g.data(), n, &P, r.data()));
+    T_out.resize(guesses.size());
+    converged_out.resize(guesses.size());
+    for (int i = 0; i < n; i++) {
+      for (int k = 0; k < 16; k++) T_out[i].v[k] = static_cast<float>(r[i].T[k]);
+      converged_out[i] = r[i].converged != 0;
+    }
+  }
+
+  // Scores poses in one launch: err[i] is the error of linearize(poses[i]) and n_corr[i] its number of (source point, voxel)
+  // correspondences (vgicp_evaluate_poses).  A pose without overlap scores 0 with no correspondences.
+  void evaluatePoses(const std::vector<Eigen::Matrix4d>& poses, std::vector<double>& err, std::vector<int64_t>& n_corr) {
+    err.clear();
+    n_corr.clear();
+    if (!input_ || !this->target_ || poses.empty()) return;
+    multiPrelude();
+    std::vector<double> T(16 * poses.size());
+    for (size_t i = 0; i < poses.size(); i++) std::memcpy(&T[16 * i], poses[i].data(), 16 * sizeof(double));
+    err.resize(poses.size());
+    n_corr.resize(poses.size());
+    multiCheck(vgicp_evaluate_poses(multiHandle(), T.data(), static_cast<int>(poses.size()), err.data(), nullptr, nullptr, n_corr.data()));
+  }
+
 protected:
+  // the device handle and the computeTransformation prelude of a subclass, for alignMulti / evaluatePoses
+  virtual vgicp_handle multiHandle() const = 0;
+  virtual void multiPrelude() {}
+  void multiCheck(int rc) const {
+    if (rc != VGICP_OK) throw std::runtime_error(this->reg_name_ + ": " + vgicp_last_error(multiHandle()));
+  }
+
   virtual void transformSource(PointCloudSource& output, const Matrix4& T) {  // pcl::transformPointCloud (:78)
     output = *input_;
     for (auto& p : output.points) {

@@ -61,9 +61,11 @@ public:
 
 protected:
   virtual void computeTransformation(PointCloudSource& output, const Matrix4& guess) override {  // ndt_cuda_impl.hpp:70-74
-    check(vgicp_ndt_create_voxelmaps(ndt_cuda_));
+    multiPrelude();
     Base::computeTransformation(output, guess);
   }
+  virtual vgicp_handle multiHandle() const override { return ndt_cuda_; }
+  virtual void multiPrelude() override { check(vgicp_ndt_create_voxelmaps(ndt_cuda_)); }
   virtual void transformSource(PointCloudSource& output, const Matrix4& T) override {
     output = *input_;
     if (output.empty()) return;

@@ -158,7 +158,58 @@ PYBIND11_MODULE(pygicp, m) {
            }
            return to_numpy(reg.getFinalTransformation());
          },
-         py::arg("initial_guess") = identity4f());
+         py::arg("initial_guess") = identity4f())
+    // multi-hypothesis alignment (not in the reference binding): (B,4,4) guesses -> (T (B,4,4) float32, converged (B,) bool)
+    .def("align_multi",
+         [](LsqReg& reg, const ArrF& initial_guesses) {
+           if (initial_guesses.ndim() != 3 || initial_guesses.shape(1) != 4 || initial_guesses.shape(2) != 4) throw std::invalid_argument("initial_guesses must be (B, 4, 4)");
+           const py::ssize_t B = initial_guesses.shape(0);
+           auto a = initial_guesses.unchecked<3>();
+           std::vector<Eigen::Matrix4f> guesses(B), T;
+           for (py::ssize_t i = 0; i < B; i++)
+             for (int r = 0; r < 4; r++) for (int c = 0; c < 4; c++) guesses[i](r, c) = a(i, r, c);
+           std::vector<bool> converged;
+           {
+             py::gil_scoped_release release;
+             reg.alignMulti(guesses, T, converged);
+           }
+           const py::ssize_t n = static_cast<py::ssize_t>(T.size());
+           py::array_t<float> T_out({n, static_cast<py::ssize_t>(4), static_cast<py::ssize_t>(4)});
+           py::array_t<bool> conv_out(n);
+           auto t = T_out.mutable_unchecked<3>();
+           auto cv = conv_out.mutable_unchecked<1>();
+           for (py::ssize_t i = 0; i < n; i++) {
+             for (int r = 0; r < 4; r++) for (int c = 0; c < 4; c++) t(i, r, c) = T[i](r, c);
+             cv(i) = converged[i];
+           }
+           return py::make_tuple(T_out, conv_out);
+         },
+         py::arg("initial_guesses"))
+    // (B,4,4) poses scored in one launch -> (err (B,), n_corr (B,) int64)
+    .def("evaluate_poses",
+         [](LsqReg& reg, const ArrD& poses) {
+           if (poses.ndim() != 3 || poses.shape(1) != 4 || poses.shape(2) != 4) throw std::invalid_argument("poses must be (B, 4, 4)");
+           const py::ssize_t B = poses.shape(0);
+           auto a = poses.unchecked<3>();
+           std::vector<Eigen::Matrix4d> P(B);
+           for (py::ssize_t i = 0; i < B; i++)
+             for (int r = 0; r < 4; r++) for (int c = 0; c < 4; c++) P[i](r, c) = a(i, r, c);
+           std::vector<double> err;
+           std::vector<int64_t> n_corr;
+           {
+             py::gil_scoped_release release;
+             reg.evaluatePoses(P, err, n_corr);
+           }
+           const py::ssize_t n = static_cast<py::ssize_t>(err.size());
+           py::array_t<double> err_out(n);
+           py::array_t<int64_t> corr_out(n);
+           for (py::ssize_t i = 0; i < n; i++) {
+             err_out.mutable_at(i) = err[i];
+             corr_out.mutable_at(i) = n_corr[i];
+           }
+           return py::make_tuple(err_out, corr_out);
+         },
+         py::arg("poses"));
 
   py::class_<VgicpCuda, LsqReg, std::shared_ptr<VgicpCuda>>(m, "FastVGICPCuda")
     .def(py::init([]() { return std::make_shared<VgicpCuda>(0); }))

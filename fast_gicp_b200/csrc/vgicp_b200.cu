@@ -164,6 +164,16 @@ struct vgicp_context {
   double* h_out = nullptr;    // pinned + mapped: in latency mode the kernel's last block writes the result straight here
   unsigned long long* h_flag = nullptr;  // pinned + mapped completion word
   unsigned long long eval_seq = 0;
+  // multi-pose evaluations (vgicp_align_multi / vgicp_evaluate_poses) have buffers of their own, so that they leave every piece
+  // of single-pose state (lin, partials, d_out, h_out, eval_seq) as it was; allocated at the first multi-pose call
+  DevBuf<double> multi_partials;            // [rows][grid][kLinStride]
+  unsigned int* d_multi_tickets = nullptr;  // [kMultiMaxHyp]
+  unsigned char* d_multi_in = nullptr;      // per-launch input: poses [hypotheses][2], then the row -> hypothesis list
+  unsigned char* h_multi_in = nullptr;      // pinned staging of d_multi_in
+  double* d_multi_out = nullptr;            // [kMultiMaxHyp][kMultiOut] (throughput hint)
+  double* h_multi_out = nullptr;            // pinned + mapped, same shape (latency hint: written by the kernels directly)
+  unsigned long long* h_multi_done = nullptr;  // pinned + mapped per-row completion words
+  unsigned long long multi_seq = 0;
 
   // NDT (NDTCudaCore, ndt_cuda.cu): 0 = VGICP problem, 1 = NDT point-to-distribution, 2 = NDT distribution-to-distribution
   int problem = 0;
@@ -667,6 +677,15 @@ LinLaunch make_lin_launch(vgicp_handle h) {
   return L;
 }
 
+// DIRECT1 on a large cloud with the direct-mapped index: the bandwidth-bound shape, streamed through shared memory by bulk copies
+// (k_linearize_stream); returns its grid, or 0 when the compacted kernels run
+int stream_kernel_grid(vgicp_handle h, const LinArgs& a) {
+  const bool stream_kernel = h->offset_mode == 1 && a.dense.cells != nullptr && a.n >= 65536 && h->lin_stream != 0 && (reinterpret_cast<uintptr_t>(a.covB) & 15) == 0;
+  if (!stream_kernel) return 0;
+  const int tiles = (a.n + kLinStreamTile - 1) / kLinStreamTile;
+  return tiles < kLinStreamMaxBlocks ? tiles : kLinStreamMaxBlocks;
+}
+
 // one evaluation: launches the fused lookup+derivative kernel; result lands in h->h_out after the stream sync
 int launch_linearize(vgicp_handle h, const Pose& Teval, bool want_H, bool direct_to_host = false, bool spec = false) {
   LinLaunch L = make_lin_launch(h);
@@ -692,11 +711,8 @@ int launch_linearize(vgicp_handle h, const Pose& Teval, bool want_H, bool direct
     else LAUNCH_LIN_G(MODE, 1);          \
   } while (0)
   prof_begin(h, want_H ? VGICP_PROF_LINEARIZE : VGICP_PROF_ERROR, h->stream);
-  // DIRECT1 on a large cloud with the direct-mapped index: the bandwidth-bound shape, streamed through shared memory by bulk copies
-  const bool stream_kernel = h->offset_mode == 1 && a.dense.cells != nullptr && a.n >= 65536 && h->lin_stream != 0 && (reinterpret_cast<uintptr_t>(a.covB) & 15) == 0;
-  if (stream_kernel) {
-    const int tiles = (a.n + kLinStreamTile - 1) / kLinStreamTile;
-    const int sgrid = tiles < kLinStreamMaxBlocks ? tiles : kLinStreamMaxBlocks;
+  const int sgrid = stream_kernel_grid(h, a);
+  if (sgrid > 0) {
     const size_t smem = sizeof(LinStreamSmem);
     if (spec) k_linearize_stream<2><<<sgrid, kLinThreads, smem, h->stream>>>(a);
     else if (want_H) k_linearize_stream<1><<<sgrid, kLinThreads, smem, h->stream>>>(a);
@@ -868,6 +884,144 @@ int evaluate_spec(vgicp_handle h, const double* T, double* err_old, double* H36,
   return VGICP_OK;
 }
 
+// ---- multi-pose evaluation (vgicp_align_multi, vgicp_evaluate_poses) -------------------------------------------------------
+enum { kEvalLinearize = 0, kEvalError = 1, kEvalSpec = 2 };  // what every row of one multi-pose launch computes
+
+// the preconditions of vgicp_align, for the calls that evaluate many poses
+int check_ready_for_multi(vgicp_handle h, const char* who) {
+  if (h->comm_ranks > 1) return fail(h, VGICP_ERR_UNSUPPORTED, std::string(who) + ": not available on a handle in a multi-GPU communicator");
+  if (h->problem == 0) {
+    if (!h->source.has_pts || !h->source.has_cov) return fail(h, VGICP_ERR_BAD_STATE, std::string(who) + ": source points and covariances required");
+    if (!h->map.built && !h->map.pending) return fail(h, VGICP_ERR_BAD_STATE, std::string(who) + ": target voxel map not built");
+  } else if (!h->source.has_pts || !h->target.has_pts) {
+    return fail(h, VGICP_ERR_BAD_STATE, std::string(who) + ": NDT needs source and target clouds");
+  }
+  return VGICP_OK;
+}
+
+// a multi-pose launch's row grid: the single-pose launch's grid (compacted kernels or the streaming kernel)
+int multi_grid(vgicp_handle h, const LinLaunch& L) {
+  const int sgrid = stream_kernel_grid(h, L.a);
+  return sgrid > 0 ? sgrid : L.grid;
+}
+
+// fixed-size buffers on first use; the partial sums grow with rows x grid (256 bytes per block and row)
+int multi_reserve(vgicp_handle h, int rows, int grid) {
+  if (!h->h_multi_out) {
+    const size_t in_bytes = (size_t)kMultiMaxHyp * (2 * sizeof(Pose) + sizeof(int)) + 16;
+    const size_t out_bytes = (size_t)kMultiMaxHyp * kMultiOut * sizeof(double);
+    CU_TRY(h, cudaMalloc(&h->d_multi_tickets, kMultiMaxHyp * sizeof(unsigned int)));
+    CU_TRY(h, cudaMemsetAsync(h->d_multi_tickets, 0, kMultiMaxHyp * sizeof(unsigned int), h->stream));
+    CU_TRY(h, cudaMalloc(&h->d_multi_in, in_bytes));
+    CU_TRY(h, cudaMallocHost(&h->h_multi_in, in_bytes));
+    CU_TRY(h, cudaMalloc(&h->d_multi_out, out_bytes));
+    CU_TRY(h, cudaHostAlloc(&h->h_multi_done, kMultiMaxHyp * sizeof(unsigned long long), cudaHostAllocMapped));
+    memset(h->h_multi_done, 0, kMultiMaxHyp * sizeof(unsigned long long));
+    CU_TRY(h, cudaHostAlloc(&h->h_multi_out, out_bytes, cudaHostAllocMapped));  // (last: it marks the set as complete)
+  }
+  CU_TRY(h, h->multi_partials.reserve((size_t)rows * grid * kLinStride));
+  return VGICP_OK;
+}
+
+// Staged input of one round, in h->h_multi_in: Pose[n_hyp][2] (Tlin, Teval per hypothesis), then the row list (hypothesis per
+// row, the rows of all launches of the round back to back).  One copy to the device per round.
+Pose* multi_poses(vgicp_handle h) { return reinterpret_cast<Pose*>(h->h_multi_in); }
+size_t multi_rows_offset(int n_hyp) { return ((size_t)n_hyp * 2 * sizeof(Pose) + 15) & ~(size_t)15; }
+int* multi_rows(vgicp_handle h, int n_hyp) { return reinterpret_cast<int*>(h->h_multi_in + multi_rows_offset(n_hyp)); }
+int multi_upload(vgicp_handle h, int n_hyp, int n_rows) {
+  CU_TRY(h, cudaMemcpyAsync(h->d_multi_in, h->h_multi_in, multi_rows_offset(n_hyp) + (size_t)n_rows * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+  return VGICP_OK;
+}
+
+// one launch over rows [row0, row0 + n) of the staged row list, all computing `kind`; the records land in rows [row0, row0 + n)
+// of the multi-pose output.  count: also count the hits (kEvalLinearize / kEvalError only).
+int launch_multi(vgicp_handle h, const LinLaunch& L, int n_hyp, int kind, bool count, int row0, int n) {
+  const LinArgs& a = L.a;
+  const bool direct = h->exec_hint == 0;
+  MultiArgs m;
+  m.hyp = reinterpret_cast<const int*>(h->d_multi_in + multi_rows_offset(n_hyp)) + row0;
+  m.poses = reinterpret_cast<const Pose*>(h->d_multi_in);
+  m.partials = h->multi_partials.p;  // (the launches of a round run one after the other on the stream: slices and tickets are reused)
+  m.tickets = h->d_multi_tickets;
+  m.out = (direct ? h->h_multi_out : h->d_multi_out) + (size_t)row0 * kMultiOut;
+  m.done = direct ? h->h_multi_done + row0 : nullptr;
+  m.done_seq = h->multi_seq;
+  const int sgrid = stream_kernel_grid(h, a), G = L.G;
+  const dim3 grid(sgrid > 0 ? sgrid : L.grid, n);
+#define LAUNCH_MULTI_G(MODE, GG)                                                                                           \
+  do {                                                                                                                     \
+    if (kind == kEvalSpec) k_linearize_spec_multi<MODE, GG><<<grid, kLinThreads, 0, h->stream>>>(a, m);                  \
+    else if (kind == kEvalLinearize && count) k_linearize_multi<MODE, true, GG, true><<<grid, kLinThreads, 0, h->stream>>>(a, m); \
+    else if (kind == kEvalLinearize) k_linearize_multi<MODE, true, GG, false><<<grid, kLinThreads, 0, h->stream>>>(a, m); \
+    else if (count) k_linearize_multi<MODE, false, GG, true><<<grid, kLinThreads, 0, h->stream>>>(a, m);                  \
+    else k_linearize_multi<MODE, false, GG, false><<<grid, kLinThreads, 0, h->stream>>>(a, m);                           \
+  } while (0)
+#define LAUNCH_MULTI(MODE)                    \
+  do {                                        \
+    if (G == 8) LAUNCH_MULTI_G(MODE, 8);      \
+    else if (G == 4) LAUNCH_MULTI_G(MODE, 4); \
+    else LAUNCH_MULTI_G(MODE, 1);             \
+  } while (0)
+  prof_begin(h, kind == kEvalError ? VGICP_PROF_ERROR : VGICP_PROF_LINEARIZE, h->stream);
+  if (sgrid > 0) {
+    const size_t smem = sizeof(LinStreamSmem);
+    if (kind == kEvalSpec) k_linearize_stream_multi<2, false><<<grid, kLinThreads, smem, h->stream>>>(a, m);
+    else if (kind == kEvalLinearize && count) k_linearize_stream_multi<1, true><<<grid, kLinThreads, smem, h->stream>>>(a, m);
+    else if (kind == kEvalLinearize) k_linearize_stream_multi<1, false><<<grid, kLinThreads, smem, h->stream>>>(a, m);
+    else if (count) k_linearize_stream_multi<0, true><<<grid, kLinThreads, smem, h->stream>>>(a, m);
+    else k_linearize_stream_multi<0, false><<<grid, kLinThreads, smem, h->stream>>>(a, m);
+  } else
+  switch (h->offset_mode) {
+    case 1: LAUNCH_MULTI_G(1, 1); break;
+    case 7: LAUNCH_MULTI(7); break;
+    case 27:
+      if (G == 3) LAUNCH_MULTI_G(27, 3);
+      else LAUNCH_MULTI_G(27, 1);
+      break;
+    default: LAUNCH_MULTI(0); break;
+  }
+#undef LAUNCH_MULTI_G
+#undef LAUNCH_MULTI
+  prof_end(h, h->stream);
+  h->launches++;
+  CU_TRY(h, cudaGetLastError());
+  return VGICP_OK;
+}
+
+// waits for rows [0, n_rows) of the current round; returns the records (host memory, kMultiOut doubles per row)
+int multi_wait(vgicp_handle h, int n_rows, const double** rec) {
+  if (h->exec_hint == 0) {  // latency: every row's last block writes its record to mapped memory and then its completion word
+    volatile unsigned long long* done = h->h_multi_done;
+    for (int r = 0; r < n_rows; r++) {
+      long spins = 0;
+      while (done[r] != h->multi_seq) {
+        __builtin_ia32_pause();
+        if (++spins > 2000000L) {  // fall back to a blocking wait (also surfaces launch errors)
+          CU_TRY(h, cudaStreamSynchronize(h->stream));
+          if (done[r] != h->multi_seq) return fail(h, VGICP_ERR_CUDA, "multi-pose evaluation: kernel finished without publishing its result");
+          break;
+        }
+      }
+    }
+    __sync_synchronize();
+  } else {
+    CU_TRY(h, cudaMemcpyAsync(h->h_multi_out, h->d_multi_out, (size_t)n_rows * kMultiOut * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+    CU_TRY(h, cudaStreamSynchronize(h->stream));
+  }
+  *rec = h->h_multi_out;
+  return VGICP_OK;
+}
+
+// lm_advance, plus the one case where the state machine and vgicp_align's loop part ways: with lm_max_iterations <= 0 the loop
+// tries no step at all and reports "lm not converged" right after the linearisation
+void multi_advance(LmState* st, const double* out) {
+  lm_advance(st, out);
+  if (st->phase == kLmError && st->lm_max_iterations <= 0) {
+    st->lm_failed = 1;
+    st->phase = kLmDone;
+  }
+}
+
 }  // namespace
 
 // =====================================================================================================================
@@ -956,6 +1110,13 @@ int vgicp_destroy(vgicp_handle h) {
   if (h->h_flag) cudaFreeHost(h->h_flag);
   if (h->d_lm) cudaFree(h->d_lm);
   if (h->h_lm) cudaFreeHost(h->h_lm);
+  h->multi_partials.release();
+  if (h->d_multi_tickets) cudaFree(h->d_multi_tickets);
+  if (h->d_multi_in) cudaFree(h->d_multi_in);
+  if (h->h_multi_in) cudaFreeHost(h->h_multi_in);
+  if (h->d_multi_out) cudaFree(h->d_multi_out);
+  if (h->h_multi_out) cudaFreeHost(h->h_multi_out);
+  if (h->h_multi_done) cudaFreeHost(h->h_multi_done);
   for (auto& r : h->prof_pending) { cudaEventDestroy(r.a); cudaEventDestroy(r.b); }
   for (auto e : h->prof_pool) cudaEventDestroy(e);
   for (cudaEvent_t e : {h->ev_copy, h->target.ready, h->source.ready})
@@ -1440,6 +1601,128 @@ int vgicp_align(vgicp_handle h, const double guess[16], const vgicp_lsq_params* 
   }
   memcpy(res->T, x0.m, sizeof(x0.m));
   res->converged = converged ? 1 : 0;
+  return VGICP_OK;
+}
+
+// B registrations from B initial guesses.  Each hypothesis runs the LM / GN state machine of the device-resident loop (lm_advance,
+// which walks vgicp_align's iterates), here on the host; every round stages the poses of the running hypotheses and evaluates all
+// of them in one launch per evaluation kind.  With LM and speculation every round after the first is one k_linearize_spec_multi
+// launch: an accepted trial's linearisation feeds the hypothesis's next lm_advance at once, as vgicp_align's have_next does.
+int vgicp_align_multi(vgicp_handle h, const double* guesses, int n_guesses, const vgicp_lsq_params* params, vgicp_align_result* results) {
+  CHECK_HANDLE(h);
+  DeviceGuard g(h->device);
+  if (!guesses || !results || n_guesses < 1 || n_guesses > kMultiMaxHyp) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "align_multi: null argument or n_guesses outside [1, 4096]");
+  int rc = check_ready_for_multi(h, "align_multi");
+  if (rc) return rc;
+  if ((rc = sync_inputs(h))) return rc;
+  vgicp_lsq_params P;
+  if (params) P = *params; else vgicp_lsq_default_params(&P);
+  const int B = n_guesses;
+  const LinLaunch L = make_lin_launch(h);
+  if ((rc = multi_reserve(h, B, multi_grid(h, L)))) return rc;
+  std::vector<LmState> st(B);
+  for (int i = 0; i < B; i++) {  // as vgicp_align's device-resident branch initialises its state block
+    LmState& s = st[i];
+    memset(&s, 0, sizeof(LmState));
+    memcpy(s.x0, guesses + 16 * i, sizeof(s.x0));
+    for (int j = 0; j < 6; j++) s.final_H[j * 7] = 1.0;
+    s.lambda = -1.0;
+    s.nu = 2.0;
+    s.rotation_epsilon = P.rotation_epsilon;
+    s.transformation_epsilon = P.transformation_epsilon;
+    s.lm_init_lambda_factor = P.lm_init_lambda_factor;
+    s.max_iterations = P.max_iterations;
+    s.lm_max_iterations = P.lm_max_iterations;
+    s.use_gauss_newton = P.use_gauss_newton;
+    s.phase = P.max_iterations > 0 ? kLmLinearize : kLmDone;
+    s.lin_pose = to_pose(guesses + 16 * i);
+    s.eval_pose = s.lin_pose;
+  }
+  const bool speculate = h->speculate != 0 && !P.use_gauss_newton;
+  std::vector<int> lin_rows, err_rows;
+  lin_rows.reserve(B);
+  err_rows.reserve(B);
+  for (;;) {
+    lin_rows.clear();
+    err_rows.clear();
+    Pose* poses = multi_poses(h);
+    for (int i = 0; i < B; i++) {
+      if (st[i].phase == kLmDone) continue;
+      (st[i].phase == kLmLinearize ? lin_rows : err_rows).push_back(i);
+      poses[2 * i] = st[i].lin_pose;
+      poses[2 * i + 1] = st[i].eval_pose;
+    }
+    const int n_lin = (int)lin_rows.size(), n_err = (int)err_rows.size();
+    if (n_lin + n_err == 0) break;
+    int* rows = multi_rows(h, B);
+    memcpy(rows, lin_rows.data(), n_lin * sizeof(int));
+    memcpy(rows + n_lin, err_rows.data(), n_err * sizeof(int));
+    h->multi_seq++;
+    if ((rc = multi_upload(h, B, n_lin + n_err))) return rc;
+    if (n_lin && (rc = launch_multi(h, L, B, kEvalLinearize, false, 0, n_lin))) return rc;
+    if (n_err && (rc = launch_multi(h, L, B, speculate ? kEvalSpec : kEvalError, false, n_lin, n_err))) return rc;
+    const double* rec = nullptr;
+    if ((rc = multi_wait(h, n_lin + n_err, &rec))) return rc;
+    for (int r = 0; r < n_lin; r++) multi_advance(&st[lin_rows[r]], rec + (size_t)r * kMultiOut);
+    for (int r = 0; r < n_err; r++) {
+      const double* o = rec + (size_t)(n_lin + r) * kMultiOut;
+      LmState* s = &st[err_rows[r]];
+      if (!speculate) {
+        multi_advance(s, o);
+        continue;
+      }
+      const double e_old[43] = {o[43]};  // the trial's error over the current correspondences decides the step (read: [0])
+      multi_advance(s, e_old);
+      if (s->phase == kLmLinearize) multi_advance(s, o);  // accepted: x0 is the trial pose, linearised by the same launch
+    }
+  }
+  for (int i = 0; i < B; i++) {
+    vgicp_align_result& res = results[i];
+    memset(&res, 0, sizeof(res));
+    memcpy(res.T, st[i].x0, sizeof(res.T));
+    memcpy(res.H, st[i].final_H, sizeof(res.H));
+    res.nr_iterations = st[i].nr_iterations;
+    res.converged = st[i].converged;
+    res.n_linearize = st[i].n_linearize;
+    res.n_compute_error = st[i].n_error;
+    res.lm_failed = st[i].lm_failed;
+  }
+  return VGICP_OK;
+}
+
+// B poses scored in one launch: per pose, update_correspondences(T_i) + compute_error(T_i) and the hit count
+int vgicp_evaluate_poses(vgicp_handle h, const double* T, int n_poses, double* err, double* H36, double* b6, int64_t* n_corr) {
+  CHECK_HANDLE(h);
+  DeviceGuard g(h->device);
+  if (!T || !err || n_poses < 1 || n_poses > kMultiMaxHyp || (H36 == nullptr) != (b6 == nullptr))
+    return fail(h, VGICP_ERR_INVALID_ARGUMENT, "evaluate_poses: null argument, H36 without b6 (or b6 without H36), or n_poses outside [1, 4096]");
+  int rc = check_ready_for_multi(h, "evaluate_poses");
+  if (rc) return rc;
+  if ((rc = sync_inputs(h))) return rc;
+  const int B = n_poses;
+  const bool want_H = H36 != nullptr;
+  const LinLaunch L = make_lin_launch(h);
+  if ((rc = multi_reserve(h, B, multi_grid(h, L)))) return rc;
+  Pose* poses = multi_poses(h);
+  int* rows = multi_rows(h, B);
+  for (int i = 0; i < B; i++) {
+    poses[2 * i] = poses[2 * i + 1] = to_pose(T + 16 * i);  // linearized_x = trans.cast<float>(), evaluated at the same pose
+    rows[i] = i;
+  }
+  h->multi_seq++;
+  if ((rc = multi_upload(h, B, B))) return rc;
+  if ((rc = launch_multi(h, L, B, want_H ? kEvalLinearize : kEvalError, true, 0, B))) return rc;
+  const double* rec = nullptr;
+  if ((rc = multi_wait(h, B, &rec))) return rc;
+  for (int i = 0; i < B; i++) {
+    const double* o = rec + (size_t)i * kMultiOut;
+    err[i] = o[0];
+    if (want_H) {
+      memcpy(H36 + 36 * (size_t)i, o + 1, 36 * sizeof(double));
+      memcpy(b6 + 6 * (size_t)i, o + 37, 6 * sizeof(double));
+    }
+    if (n_corr) n_corr[i] = (int64_t)o[kMultiOutCount];
+  }
   return VGICP_OK;
 }
 

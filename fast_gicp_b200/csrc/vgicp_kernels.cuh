@@ -586,7 +586,8 @@ __device__ __forceinline__ LinWarpStage& lin_stage() {
   return stage[threadIdx.x >> 5];
 }
 
-template <int MODE, bool WANT_H, int G, bool DENSE>
+// COUNT: sum[NV] also counts the (source point, voxel) hits under Tl -- the length of the reference's correspondence list
+template <int MODE, bool WANT_H, int G, bool DENSE, bool COUNT = false>
 __device__ __forceinline__ void lin_accumulate_impl(const LinArgs& a, const Pose& Tl, const Pose& Te, float* sum) {
   constexpr int NV = WANT_H ? kLinValues : 1;
   constexpr int NOFF = MODE == 0 ? 0 : MODE;
@@ -599,7 +600,7 @@ __device__ __forceinline__ void lin_accumulate_impl(const LinArgs& a, const Pose
   const int lane = threadIdx.x & 31;
   const unsigned lt_mask = (1u << lane) - 1u;
 #pragma unroll
-  for (int i = 0; i < NV; i++) sum[i] = 0.f;
+  for (int i = 0; i < NV + (COUNT ? 1 : 0); i++) sum[i] = 0.f;
   const int n_off = MODE == 0 ? a.n_off : NOFF;
   const int n_pass = COLUMNS ? 9 / G : (n_off + G * CELLS - 1) / (G * CELLS);
   const long long n_tasks = (long long)a.n * G;
@@ -703,6 +704,7 @@ __device__ __forceinline__ void lin_accumulate_impl(const LinArgs& a, const Pose
         const unsigned m = __ballot_sync(0xffffffffu, hit);
         if (hit) st.queue[(tail + __popc(m & lt_mask)) & (kLinQueue - 1)] = (slot << 27) | found[j];
         tail += __popc(m);
+        if (COUNT && hit) sum[NV] += 1.f;  // (exact: a lane sees far fewer than 2^24 hits)
       }
       __syncwarp();
       while (tail - head >= 32u) {  // full batches: one correspondence per lane
@@ -716,10 +718,10 @@ __device__ __forceinline__ void lin_accumulate_impl(const LinArgs& a, const Pose
   }
 }
 
-template <int MODE, bool WANT_H, int G>
+template <int MODE, bool WANT_H, int G, bool COUNT = false>
 __device__ __forceinline__ void lin_accumulate(const LinArgs& a, const Pose& Tl, const Pose& Te, float* sum) {
-  if (a.dense.cells) lin_accumulate_impl<MODE, WANT_H, G, true>(a, Tl, Te, sum);  // (grid-uniform branch)
-  else lin_accumulate_impl<MODE, WANT_H, G, false>(a, Tl, Te, sum);
+  if (a.dense.cells) lin_accumulate_impl<MODE, WANT_H, G, true, COUNT>(a, Tl, Te, sum);  // (grid-uniform branch)
+  else lin_accumulate_impl<MODE, WANT_H, G, false, COUNT>(a, Tl, Te, sum);
 }
 
 // block reduction (warp shuffles in float -> shared in double -> per-block partial), ticket, fixed-order fold by the last
@@ -727,8 +729,10 @@ __device__ __forceinline__ void lin_accumulate(const LinArgs& a, const Pose& Tl,
 // (Tried and dropped: a first-level reduction over distributed shared memory inside 8-block clusters, so that the last block folds
 // grid/8 partials.  It gained little at 17 k points and lost at 1 M points, where the cluster placement constraint left SMs idle
 // at the tail of the single wave.)
+// `partials` ([gridDim.x][kLinStride]) and `ticket` belong to one evaluation: a.partials / a.ticket, or one hypothesis's slice of a
+// multi-pose launch
 template <int NV>
-__device__ __forceinline__ bool lin_reduce(const LinArgs& a, const float* sum, double (*fin)[kLinStride]) {
+__device__ __forceinline__ bool lin_reduce(const LinArgs& a, const float* sum, double (*fin)[kLinStride], double* partials, unsigned int* ticket) {
   // ---- block reduction: warp shuffles (float) -> shared (double) -> per-block partial ----
   __shared__ double sh[kLinThreads / 32][kLinStride];
   __shared__ bool is_last;
@@ -745,12 +749,12 @@ __device__ __forceinline__ bool lin_reduce(const LinArgs& a, const float* sum, d
     double s = 0.0;
 #pragma unroll
     for (int w = 0; w < kLinThreads / 32; w++) s += sh[w][threadIdx.x];
-    a.partials[(size_t)blockIdx.x * kLinStride + threadIdx.x] = s;
+    partials[(size_t)blockIdx.x * kLinStride + threadIdx.x] = s;
   }
   __threadfence();
   __syncthreads();
   if (threadIdx.x == 0) {
-    unsigned t = atomicAdd(a.ticket, 1u);
+    unsigned t = atomicAdd(ticket, 1u);
     is_last = (t == gridDim.x - 1);
   }
   __syncthreads();
@@ -763,7 +767,7 @@ __device__ __forceinline__ bool lin_reduce(const LinArgs& a, const float* sum, d
       // ld.global.cg: coherent at L2 (the partials were written by other SMs), 16 independent loads in flight per
       // round -- a dependent load->add chain over hundreds of blocks serialises on L2 latency
       double s = 0.0;
-      const double* part = a.partials + v;
+      const double* part = partials + v;
       unsigned b = chain;
       for (; b + 4 * 15 < gridDim.x; b += 4 * 16) {
         double t[16];
@@ -814,6 +818,10 @@ __device__ __forceinline__ bool lin_reduce(const LinArgs& a, const float* sum, d
     __syncthreads();
   }
   return true;
+}
+template <int NV>
+__device__ __forceinline__ bool lin_reduce(const LinArgs& a, const float* sum, double (*fin)[kLinStride]) {
+  return lin_reduce<NV>(a, sum, fin, a.partials, a.ticket);
 }
 
 // unpack the folded sums into err, H (36, column-major), b (6)
@@ -866,21 +874,25 @@ __global__ void __launch_bounds__(kLinThreads) k_linearize(const LinArgs a) {
 // an accepted step saves a launch and a host round trip, a rejected one discards the second half.
 //   out[0..42] = err, H, b at xi (linearised at xi);  out[43] = err at xi over the old correspondences
 template <int MODE, int G>
-__global__ void __launch_bounds__(kLinThreads) k_linearize_spec(const LinArgs a) {
-  constexpr int NV = kLinValues + 1;
-  __shared__ double fin[4][kLinStride];
-  float sum[NV];
+__device__ __forceinline__ void lin_spec_accumulate(const LinArgs& a, const Pose& Tl, const Pose& Te, float* sum) {  // sum[kLinValues + 1]
   {
     float e_old[1];
-    lin_accumulate<MODE, false, G>(a, a.Tlin, a.Teval, e_old);
+    lin_accumulate<MODE, false, G>(a, Tl, Te, e_old);
     sum[kLinValues] = e_old[0];
   }
   {
     float lin[kLinValues];
-    lin_accumulate<MODE, true, G>(a, a.Teval, a.Teval, lin);
+    lin_accumulate<MODE, true, G>(a, Te, Te, lin);
 #pragma unroll
     for (int i = 0; i < kLinValues; i++) sum[i] = lin[i];
   }
+}
+template <int MODE, int G>
+__global__ void __launch_bounds__(kLinThreads) k_linearize_spec(const LinArgs a) {
+  constexpr int NV = kLinValues + 1;
+  __shared__ double fin[4][kLinStride];
+  float sum[NV];
+  lin_spec_accumulate<MODE, G>(a, a.Tlin, a.Teval, sum);
   if (!lin_reduce<NV>(a, sum, fin)) return;
   if (threadIdx.x == 0) {
     lin_unpack<true>(fin[0], a.out);
@@ -936,12 +948,14 @@ struct LinStreamSmem {
 };
 
 // one point against the voxel of its cell under the linearisation pose Tl, residual at the evaluation pose Te
-template <bool WANT_H>
+// (COUNT: the slot after the sums counts the hits, as in lin_accumulate_impl)
+template <bool WANT_H, bool COUNT = false>
 __device__ __forceinline__ void lin_stream_point(const LinArgs& a, const Pose& Tl, const Pose& Te, float4 p, float4 ca, float2 cb, float* sum) {
   const float3 pl = transform_point(Tl, p.x, p.y, p.z);
   const int off = dense_offset(a.dense, voxel_coord1(pl.x, a.res), voxel_coord1(pl.y, a.res), voxel_coord1(pl.z, a.res));
   const int id = off >= 0 ? __ldg(&a.dense.cells[off]) : -1;
   if (id < 0) return;
+  if (COUNT) sum[WANT_H ? kLinValues : 1] += 1.f;
   const float4* vr = reinterpret_cast<const float4*>(a.vox + id);
   const float4 mn = __ldg(vr), c0 = __ldg(vr + 1), c1 = __ldg(vr + 2);
   const float3 pe = transform_point(Te, p.x, p.y, p.z);
@@ -968,13 +982,13 @@ __device__ __forceinline__ void lin_stream_point(const LinArgs& a, const Pose& T
   apply_jacobian<WANT_H>(pe, acc, sum);
 }
 
-// WHAT: 0 = error only, 1 = linearisation (H, b, err), 2 = speculative (both)
-template <int WHAT>
-__global__ void __launch_bounds__(kLinThreads) k_linearize_stream(const LinArgs a) {
-  constexpr int NV = WHAT == 0 ? 1 : (WHAT == 1 ? kLinValues : kLinValues + 1);
+// WHAT: 0 = error only, 1 = linearisation (H, b, err), 2 = speculative (both).  COUNT (WHAT 0 / 1): one more slot counts the hits.
+template <int WHAT, bool COUNT = false>
+__device__ __forceinline__ void lin_stream_accumulate(const LinArgs& a, const Pose& Tl, const Pose& Te, float* sum) {
+  constexpr int NV = (WHAT == 0 ? 1 : (WHAT == 1 ? kLinValues : kLinValues + 1)) + (COUNT ? 1 : 0);
+  static_assert(!COUNT || WHAT != 2, "the speculative evaluation does not count hits");
   extern __shared__ __align__(128) unsigned char stream_smem_raw[];
   LinStreamSmem& sm = *reinterpret_cast<LinStreamSmem*>(stream_smem_raw);
-  __shared__ double fin[4][kLinStride];
   const int tid = threadIdx.x;
   if (tid == 0) {
 #pragma unroll
@@ -997,7 +1011,6 @@ __global__ void __launch_bounds__(kLinThreads) k_linearize_stream(const LinArgs 
   };
   if (tid == 0)
     for (int it = 0; it < kLinStreamStages - 1; it++) issue(it);
-  float sum[NV];
 #pragma unroll
   for (int i = 0; i < NV; i++) sum[i] = 0.f;
   for (int it = 0;; it++) {
@@ -1014,17 +1027,25 @@ __global__ void __launch_bounds__(kLinThreads) k_linearize_stream(const LinArgs 
         const float4 p = sm.pts[s][j], ca = sm.covA[s][j];
         const float2 cb = sm.covB[s][j];
         if (WHAT == 0) {
-          lin_stream_point<false>(a, a.Tlin, a.Teval, p, ca, cb, sum);
+          lin_stream_point<false, COUNT>(a, Tl, Te, p, ca, cb, sum);
         } else if (WHAT == 1) {
-          lin_stream_point<true>(a, a.Tlin, a.Teval, p, ca, cb, sum);
+          lin_stream_point<true, COUNT>(a, Tl, Te, p, ca, cb, sum);
         } else {
-          lin_stream_point<false>(a, a.Tlin, a.Teval, p, ca, cb, sum + kLinValues);
-          lin_stream_point<true>(a, a.Teval, a.Teval, p, ca, cb, sum);
+          lin_stream_point<false>(a, Tl, Te, p, ca, cb, sum + kLinValues);
+          lin_stream_point<true>(a, Te, Te, p, ca, cb, sum);
         }
       }
     }
     __syncthreads();  // the stage may be overwritten by the copy issued in the next iteration
   }
+}
+template <int WHAT>
+__global__ void __launch_bounds__(kLinThreads) k_linearize_stream(const LinArgs a) {
+  constexpr int NV = WHAT == 0 ? 1 : (WHAT == 1 ? kLinValues : kLinValues + 1);
+  __shared__ double fin[4][kLinStride];
+  const int tid = threadIdx.x;
+  float sum[NV];
+  lin_stream_accumulate<WHAT>(a, a.Tlin, a.Teval, sum);
   if (!lin_reduce<NV>(a, sum, fin)) return;
   if (tid == 0) {
     if (WHAT == 0) {
@@ -1042,12 +1063,114 @@ __global__ void __launch_bounds__(kLinThreads) k_linearize_stream(const LinArgs 
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// Multi-pose evaluation (vgicp_align_multi / vgicp_evaluate_poses): one launch evaluates many hypotheses -- poses of the same
+// source against the same map.  blockIdx.y is a row of the launch; row y evaluates hypothesis hyp[y] with the poses the host
+// wrote to the device array for this launch.  Every row has exactly the single-pose launch's gridDim.x, lane assignment and
+// fixed-order fold (the same accumulate functions, lin_reduce over the row's own partial slice and ticket), so each row's sums
+// are the single-pose evaluation's sums bit for bit.
+// ---------------------------------------------------------------------------------------------------------------
+// (The multi-pose kernels declare a minimum of one block per SM: without it ptxas capped some of them at 64 / 72 registers and spilled.)
+constexpr int kMultiMaxHyp = 4096;
+constexpr int kMultiOut = 48;        // per-row record: [0..42] err, H, b;  [43] speculative: err over the old correspondences;
+constexpr int kMultiOutCount = 44;   //                 [44] hit count (the length of the reference's correspondence list)
+
+struct MultiArgs {
+  const int* hyp;            // [gridDim.y]: hypothesis evaluated by each row
+  const Pose* poses;         // [hypothesis][2] = Tlin, Teval
+  double* partials;          // [gridDim.y][gridDim.x][kLinStride]
+  unsigned int* tickets;     // [gridDim.y]: zero before the first launch; reset by each row's last block
+  double* out;               // [gridDim.y][kMultiOut]; may be mapped pinned host memory
+  volatile unsigned long long* done;  // optional [gridDim.y] (mapped host memory): set to done_seq once the row's record is complete
+  unsigned long long done_seq;
+};
+
+// the row's Tlin, Teval staged in shared memory (sp[0], sp[1]): read like the single-pose kernels' parameter-space poses, without
+// holding 24 more registers (which made ptxas spill in the error-only kernels)
+__device__ __forceinline__ int multi_row(const MultiArgs& m, Pose* sp) {
+  const int y = blockIdx.y;
+  constexpr int kWords = 2 * (int)(sizeof(Pose) / sizeof(float));
+  if (threadIdx.x < kWords) reinterpret_cast<float*>(sp)[threadIdx.x] = __ldg(reinterpret_cast<const float*>(m.poses + 2 * m.hyp[y]) + threadIdx.x);
+  __syncthreads();
+  return y;
+}
+template <int NV>
+__device__ __forceinline__ bool multi_reduce(const LinArgs& a, const MultiArgs& m, int y, const float* sum, double (*fin)[kLinStride]) {
+  return lin_reduce<NV>(a, sum, fin, m.partials + (size_t)y * gridDim.x * kLinStride, m.tickets + y);
+}
+// thread 0 of a row's last block, after its record is written
+__device__ __forceinline__ void multi_publish(const MultiArgs& m, int y) {
+  m.tickets[y] = 0u;
+  if (m.done) {
+    __threadfence_system();
+    m.done[y] = m.done_seq;
+  }
+}
+
+template <int MODE, bool WANT_H, int G, bool COUNT>
+__global__ void __launch_bounds__(kLinThreads, 1) k_linearize_multi(const LinArgs a, const MultiArgs m) {
+  constexpr int NV = (WANT_H ? kLinValues : 1) + (COUNT ? 1 : 0);
+  __shared__ double fin[4][kLinStride];
+  __shared__ Pose sp[2];
+  const int y = multi_row(m, sp);
+  float sum[NV];
+  lin_accumulate<MODE, WANT_H, G, COUNT>(a, sp[0], sp[1], sum);
+  if (!multi_reduce<NV>(a, m, y, sum, fin)) return;
+  if (threadIdx.x == 0) {
+    double* rec = m.out + (size_t)y * kMultiOut;
+    lin_unpack<WANT_H>(fin[0], rec);
+    if (COUNT) rec[kMultiOutCount] = fin[0][NV - 1];
+    multi_publish(m, y);
+  }
+}
+
+template <int MODE, int G>
+__global__ void __launch_bounds__(kLinThreads, 1) k_linearize_spec_multi(const LinArgs a, const MultiArgs m) {
+  constexpr int NV = kLinValues + 1;
+  __shared__ double fin[4][kLinStride];
+  __shared__ Pose sp[2];
+  const int y = multi_row(m, sp);
+  float sum[NV];
+  lin_spec_accumulate<MODE, G>(a, sp[0], sp[1], sum);
+  if (!multi_reduce<NV>(a, m, y, sum, fin)) return;
+  if (threadIdx.x == 0) {
+    double* rec = m.out + (size_t)y * kMultiOut;
+    lin_unpack<true>(fin[0], rec);
+    rec[43] = fin[0][kLinValues];
+    multi_publish(m, y);
+  }
+}
+
+template <int WHAT, bool COUNT>
+__global__ void __launch_bounds__(kLinThreads, 1) k_linearize_stream_multi(const LinArgs a, const MultiArgs m) {
+  constexpr int NB = WHAT == 0 ? 1 : (WHAT == 1 ? kLinValues : kLinValues + 1);
+  constexpr int NV = NB + (COUNT ? 1 : 0);
+  __shared__ double fin[4][kLinStride];
+  __shared__ Pose sp[2];
+  const int y = multi_row(m, sp);
+  float sum[NV];
+  lin_stream_accumulate<WHAT, COUNT>(a, sp[0], sp[1], sum);
+  if (!multi_reduce<NV>(a, m, y, sum, fin)) return;
+  if (threadIdx.x == 0) {
+    double* rec = m.out + (size_t)y * kMultiOut;
+    if (WHAT == 0) {
+      lin_unpack<false>(fin[0], rec);
+    } else {
+      lin_unpack<true>(fin[0], rec);
+      if (WHAT == 2) rec[43] = fin[0][kLinValues];
+    }
+    if (COUNT) rec[kMultiOutCount] = fin[0][NB];
+    multi_publish(m, y);
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // Device-resident optimiser: LsqRegistration::computeTransformation (lsq_registration_impl.hpp:53-79) with step_gn
 // (:106-120) / step_lm (:123-168) as a chain of evaluation kernels.  Each launch reads the phase and the two poses from
 // the state block, evaluates (linearize = lookup at x0 + H,b,err ; or error only at the candidate xi with the
 // correspondences of x0), and thread 0 of its last block advances the state machine in double -- exactly the host
 // logic, same arithmetic (lsq_math.hpp is shared).  A launch that finds phase == DONE returns at once, so the host
 // can enqueue a fixed number of launches and read the state back once.
+// The state machine is host+device: vgicp_align_multi runs one per hypothesis on the host (host libm, like vgicp_align's loop).
 // ---------------------------------------------------------------------------------------------------------------
 struct LmState {
   double x0[16], xi[16], delta[16];
@@ -1063,7 +1186,7 @@ struct LmState {
 };
 enum { kLmLinearize = 0, kLmError = 1, kLmDone = 2 };
 
-__device__ __forceinline__ Pose pose_from_iso(const double* T) {
+VGICP_HD Pose pose_from_iso(const double* T) {
   Pose p;
   for (int r = 0; r < 3; r++) {
     for (int c = 0; c < 3; c++) p.r[r * 3 + c] = (float)T[c * 4 + r];
@@ -1072,7 +1195,7 @@ __device__ __forceinline__ Pose pose_from_iso(const double* T) {
   return p;
 }
 
-__device__ void lm_propose(LmState* st) {  // solve (H + lambda I) d = -b, delta = exp(d), xi = delta * x0   (:134-139)
+VGICP_HD void lm_propose(LmState* st) {  // solve (H + lambda I) d = -b, delta = exp(d), xi = delta * x0   (:134-139)
   double Hl[36], nb[6];
   for (int j = 0; j < 36; j++) Hl[j] = st->H[j];
   for (int q = 0; q < 6; q++) { Hl[q * 7] += st->lambda; nb[q] = -st->b[q]; }
@@ -1086,7 +1209,7 @@ __device__ void lm_propose(LmState* st) {  // solve (H + lambda I) d = -b, delta
   st->phase = kLmError;
 }
 
-__device__ void lm_finish_outer(LmState* st) {  // end of step_optimize: converged_ = is_converged(delta), next outer iteration (:65-75)
+VGICP_HD void lm_finish_outer(LmState* st) {  // end of step_optimize: converged_ = is_converged(delta), next outer iteration (:65-75)
   Iso3d delta;
   for (int j = 0; j < 16; j++) delta.m[j] = st->delta[j];
   st->converged = is_converged(delta, st->rotation_epsilon, st->transformation_epsilon) ? 1 : 0;
@@ -1098,7 +1221,7 @@ __device__ void lm_finish_outer(LmState* st) {  // end of step_optimize: converg
   st->phase = kLmLinearize;
 }
 
-__device__ void lm_advance(LmState* st, const double* out /*err, H, b*/) {
+VGICP_HD void lm_advance(LmState* st, const double* out /*err, H, b*/) {
   if (st->phase == kLmLinearize) {
     st->y0 = out[0];
     for (int j = 0; j < 36; j++) st->H[j] = out[1 + j];

@@ -106,6 +106,32 @@ class LsqRegistration:
             lm_init_lambda_factor=self.lm_init_lambda_factor_,
         )
 
+    # -- multi-hypothesis alignment (not in the reference): the subclasses provide _core() and _prelude()
+    def align_multi(self, initial_guesses):
+        """Register the source from each of the (B, 4, 4) initial guesses, the evaluations of all hypotheses sharing launches.
+
+        Returns (T (B, 4, 4) float32, converged (B,) bool); T[i] equals what align(initial_guesses[i]) returns.  The state of
+        the single registration (getFinalTransformation, hasConverged, the final Hessian) is left alone."""
+        if self.input_ is None or self.target_ is None:
+            raise RuntimeError("align_multi: input source/target not set")
+        G = np.asarray(initial_guesses, dtype=np.float32).astype(np.float64)  # cast like align's guess
+        if G.ndim != 3 or G.shape[1:] != (4, 4):
+            raise ValueError("initial_guesses must be (B, 4, 4)")
+        self._prelude()
+        res = self._core().align_multi(G, self._params())
+        T = np.stack([_core.pose_from_c(r.T) for r in res]).astype(np.float32)
+        return T, np.array([bool(r.converged) for r in res])
+
+    def evaluate_poses(self, poses):
+        """Score the (B, 4, 4) poses in one launch -> (err (B,), n_corr (B,) int64): the error of update_correspondences(T) +
+        compute_error(T) and the number of (source point, voxel) correspondences at each pose.  A pose without overlap scores
+        err 0 with n_corr 0, so rank hypotheses by err normalised with n_corr."""
+        if self.input_ is None or self.target_ is None:
+            raise RuntimeError("evaluate_poses: input source/target not set")
+        self._prelude()
+        err, _, _, n_corr = self._core().evaluate_poses(np.asarray(poses, dtype=np.float64))
+        return err, n_corr
+
     # pygicp names (main.cpp:152-168)
     def set_input_target(self, points):
         self.setInputTarget(_as_cloud(points))
@@ -190,11 +216,17 @@ class NDTCuda(LsqRegistration):
     def compute_error(self, trans):
         return self.ndt_cuda_.compute_error(trans, want_H=False)[0]
 
+    def _core(self):
+        return self.ndt_cuda_
+
+    def _prelude(self):
+        self.ndt_cuda_.ndt_create_voxelmaps()  # computeTransformation, ndt_cuda_impl.hpp:71-73
+
     def align(self, initial_guess=None, aligned_out=None):
         if self.input_ is None or self.target_ is None:
             raise RuntimeError("align: input source/target not set")
         guess = np.eye(4) if initial_guess is None else np.asarray(initial_guess, dtype=np.float32).astype(np.float64)
-        self.ndt_cuda_.ndt_create_voxelmaps()  # computeTransformation, ndt_cuda_impl.hpp:71-73
+        self._prelude()
         self.converged_ = False
         res = self.ndt_cuda_.align(guess, self._params())
         if res.lm_failed:
@@ -305,6 +337,12 @@ class FastVGICPCuda(LsqRegistration):
         err, H, b = self.vgicp_cuda_.linearize(np.asarray(relative_pose, dtype=np.float32).astype(np.float64))
         return (err, H, b) if want_H else err
 
+    def _core(self):
+        return self.vgicp_cuda_
+
+    def _prelude(self):
+        self.vgicp_cuda_.set_resolution(self.voxel_resolution_)  # :145 (the wrapper's stale resolution, SURVEY Q3)
+
     def align(self, initial_guess=None, return_aligned=False, aligned_out=None):
         """pcl::Registration::align -> computeTransformation (:144-148 + lsq_registration_impl.hpp:53-79).
 
@@ -315,7 +353,7 @@ class FastVGICPCuda(LsqRegistration):
         if self.input_ is None or self.target_ is None:
             raise RuntimeError("align: input source/target not set")
         guess = np.eye(4) if initial_guess is None else np.asarray(initial_guess, dtype=np.float32).astype(np.float64)
-        self.vgicp_cuda_.set_resolution(self.voxel_resolution_)  # :145 (the wrapper's stale resolution, SURVEY Q3)
+        self._prelude()
         self.converged_ = False
         res = self.vgicp_cuda_.align(guess, self._params())
         if res.lm_failed:

@@ -153,6 +153,24 @@ VGICP_API void vgicp_lsq_default_params(vgicp_lsq_params* p);
  * Driven from the host by default (one 344-byte result per evaluation through mapped memory); vgicp_set_align_mode selects the
  * device-resident state machine, vgicp_set_speculation the fused trial evaluation.  result->T = final_transformation_. */
 VGICP_API int vgicp_align(vgicp_handle h, const double guess[16], const vgicp_lsq_params* params, vgicp_align_result* result);
+/* ---- multi-hypothesis alignment (global localisation, relocalisation, loop-closure checks) ----------------------------------
+ * B registrations of the current source against the current target map, from B initial guesses (B x 16 doubles, column-major),
+ * with the evaluations of all still-running hypotheses in shared launches: one evaluation kernel per optimiser round and kind
+ * (with LM and speculation, one launch per round; with GN, one linearisation launch per round), each hypothesis a row of blocks
+ * with the single-pose launch's grid, so its sums are the single-pose sums.  results[i] equals vgicp_align(h, guesses + 16 i,
+ * params) bit for bit (T, H, nr_iterations, converged, n_linearize, n_compute_error, lm_failed), under either execution hint and
+ * speculation setting; the host-driven LM loop is used whatever vgicp_set_align_mode says.  1 <= n_guesses <= 4096.
+ * The handle's linearisation point and the rest of its single-pose state are left as they were.  Working memory: 256 bytes per
+ * evaluation block and hypothesis (about 0.1 MB per hypothesis at 17 k points, 0.27 MB at 1 M points with DIRECT1), grow-only.
+ * Errors: VGICP_ERR_INVALID_ARGUMENT (null pointer, n_guesses out of range), VGICP_ERR_BAD_STATE (the preconditions of
+ * vgicp_align), VGICP_ERR_UNSUPPORTED (handle in a multi-GPU communicator); none of them launches a kernel. */
+VGICP_API int vgicp_align_multi(vgicp_handle h, const double* guesses, int n_guesses, const vgicp_lsq_params* params, vgicp_align_result* results);
+/* B poses scored in one launch: err[i] (and H36 + 36 i, b6 + 6 i when H36 and b6 are not NULL; both or neither) equal
+ * vgicp_update_correspondences(T_i) + vgicp_compute_error(T_i) bit for bit; n_corr[i] (optional) is the number of (source point,
+ * voxel) correspondences at T_i, the count vgicp_get_voxel_correspondences reports.  A pose without overlap has err 0 and no
+ * correspondences, so rank hypotheses by err normalised with n_corr, not by err alone.  Handle state unchanged; 1 <= n_poses <= 4096;
+ * errors as vgicp_align_multi. */
+VGICP_API int vgicp_evaluate_poses(vgicp_handle h, const double* T, int n_poses, double* err, double* H36, double* b6, int64_t* n_corr);
 /* One whole registration: clearTarget/clearSource + setInputTarget + setInputSource + align (the body of the reference's
  * benchmark loop, src/align.cpp:72-81) with GPU k-NN covariances.  xyz are host pointers, or device pointers when on_device != 0. */
 VGICP_API int vgicp_register(vgicp_handle h, const float* target_xyz, size_t n_target, const float* source_xyz, size_t n_source, size_t stride_bytes, int on_device, int k,
