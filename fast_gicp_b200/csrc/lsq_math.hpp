@@ -1,34 +1,27 @@
 // lsq_math.hpp -- small fixed-size double-precision helpers for the host side of the registration loop:
 // SE(3) exponential (reference include/fast_gicp/so3/so3.hpp:58-104), 6x6 pivoted LDL^T solve (stands in for
 // Eigen::LDLT<Matrix<double,6,6>>, lsq_registration_impl.hpp:111,134), isometry product, convergence test
-// (lsq_registration_impl.hpp:82-91).  Header-only, no dependencies (Eigen is not available in this environment);
-// __host__ __device__ so the device-resident LM loop shares the exact same code.
+// (lsq_registration_impl.hpp:82-91).  Header-only, no dependencies (Eigen is not available in this environment).
 #pragma once
 #include <math.h>
-
-#if defined(__CUDACC__)
-#define VGICP_HD __host__ __device__ inline
-#else
-#define VGICP_HD inline
-#endif
 
 namespace vgicp {
 
 // 4x4 column-major isometry image, identical to Eigen::Isometry3d::data()
 struct Iso3d {
   double m[16];
-  VGICP_HD double& operator()(int r, int c) { return m[c * 4 + r]; }
-  VGICP_HD double operator()(int r, int c) const { return m[c * 4 + r]; }
+  double& operator()(int r, int c) { return m[c * 4 + r]; }
+  double operator()(int r, int c) const { return m[c * 4 + r]; }
 };
 
-VGICP_HD Iso3d iso_identity() {
+inline Iso3d iso_identity() {
   Iso3d T;
   for (int i = 0; i < 16; i++) T.m[i] = (i % 5 == 0) ? 1.0 : 0.0;
   return T;
 }
 
 // delta * x0 for affine 4x4 (last row 0 0 0 1)
-VGICP_HD Iso3d iso_mul(const Iso3d& A, const Iso3d& B) {
+inline Iso3d iso_mul(const Iso3d& A, const Iso3d& B) {
   Iso3d C;
   for (int c = 0; c < 4; c++)
     for (int r = 0; r < 3; r++) {
@@ -42,7 +35,7 @@ VGICP_HD Iso3d iso_mul(const Iso3d& A, const Iso3d& B) {
 }
 
 // so3.hpp:80-104 (rotation-first 6-vector [omega, v]); so3_exp :58-77; Eigen's Quaternion::toRotationMatrix
-VGICP_HD Iso3d se3_exp(const double* a) {
+inline Iso3d se3_exp(const double* a) {
   const double ox = a[0], oy = a[1], oz = a[2];
   const double theta_sq = ox * ox + oy * oy + oz * oz;
   const double theta = sqrt(theta_sq);
@@ -85,7 +78,7 @@ VGICP_HD Iso3d se3_exp(const double* a) {
 }
 
 // Solve A x = rhs, A symmetric 6x6 column-major; LDL^T with diagonal pivoting.
-VGICP_HD void ldlt_solve6(const double* A_in, const double* rhs, double* x) {
+inline void ldlt_solve6(const double* A_in, const double* rhs, double* x) {
   double A[6][6];
   int perm[6];
   for (int r = 0; r < 6; r++) {
@@ -122,7 +115,7 @@ VGICP_HD void ldlt_solve6(const double* A_in, const double* rhs, double* x) {
 }
 
 // lsq_registration_impl.hpp:82-91
-VGICP_HD bool is_converged(const Iso3d& delta, double rotation_epsilon, double transformation_epsilon) {
+inline bool is_converged(const Iso3d& delta, double rotation_epsilon, double transformation_epsilon) {
   double mr = 0.0, mt = 0.0;
   for (int r = 0; r < 3; r++)
     for (int c = 0; c < 3; c++) {

@@ -151,9 +151,6 @@ struct vgicp_context {
   int stage1_sharding = 0;
   int speculate = 1;  // LM trial evaluations also linearise at the trial pose (vgicp_set_speculation)
   int exec_hint = 0;  // 0 = latency (one registration should finish as soon as possible), 1 = throughput (many concurrent handles)
-  int align_mode = 1;  // 1 = host-driven loop over the evaluation kernels (default: faster today), 0 = device-resident LM chain
-  LmState* d_lm = nullptr;
-  LmState* h_lm = nullptr;  // pinned
   int lin_stream = 1;   // VGICP_LIN_STREAM=0 disables the bulk-copy streaming kernel of DIRECT1 (A/B measurements)
   int force_lin_g = 0;  // VGICP_LIN_G override of the lanes-per-point split (experiments)
   int knn_mode = 0;  // 0 = hash grid (default), 1 = warp-cooperative scan of the whole cloud, 2 = legacy per-thread scan
@@ -686,13 +683,16 @@ int stream_kernel_grid(vgicp_handle h, const LinArgs& a) {
   return tiles < kLinStreamMaxBlocks ? tiles : kLinStreamMaxBlocks;
 }
 
-// one evaluation: launches the fused lookup+derivative kernel; result lands in h->h_out after the stream sync
-int launch_linearize(vgicp_handle h, const Pose& Teval, bool want_H, bool direct_to_host = false, bool spec = false) {
+enum { kEvalLinearize = 0, kEvalError = 1, kEvalSpec = 2 };  // what an evaluation launch computes (every row of a multi-pose one alike)
+
+// one evaluation: launches the fused lookup+derivative kernel at Teval over the correspondences of h->lin
+int launch_linearize(vgicp_handle h, const Pose& Teval, int kind) {
+  const bool want_H = kind != kEvalError, spec = kind == kEvalSpec;
   LinLaunch L = make_lin_launch(h);
   LinArgs& a = L.a;
   a.Teval = Teval;
   a.comm_seq = h->comm_seq++;
-  if (direct_to_host) {  // UVA: the mapped pinned pointers are valid on the device
+  if (h->exec_hint == 0) {  // latency: the result goes straight to mapped host memory (UVA: the pinned pointers are valid on the device)
     a.out = h->h_out;
     a.done_flag = h->h_flag;
     a.done_seq = ++h->eval_seq;
@@ -729,36 +729,6 @@ int launch_linearize(vgicp_handle h, const Pose& Teval, bool want_H, bool direct
   }
 #undef LAUNCH_LIN_G
 #undef LAUNCH_LIN
-  prof_end(h, h->stream);
-  h->launches++;
-  CU_TRY(h, cudaGetLastError());
-  return VGICP_OK;
-}
-
-// one link of the device-resident optimiser chain
-int launch_lm_step(vgicp_handle h, const LinLaunch& L) {
-  LinArgs a = L.a;
-  a.comm_seq = h->comm_seq++;  // (links that find the chain finished return before the exchange, on every rank alike)
-  const int grid = L.grid, G = L.G;
-#define LAUNCH_LM_G(MODE, GG) k_lm_step<MODE, GG><<<grid, kLinThreads, 0, h->stream>>>(a, h->d_lm)
-#define LAUNCH_LM(MODE)                 \
-  do {                                  \
-    if (G == 8) LAUNCH_LM_G(MODE, 8);   \
-    else if (G == 4) LAUNCH_LM_G(MODE, 4); \
-    else LAUNCH_LM_G(MODE, 1);          \
-  } while (0)
-  prof_begin(h, VGICP_PROF_LINEARIZE, h->stream);
-  switch (h->offset_mode) {
-    case 1: LAUNCH_LM_G(1, 1); break;
-    case 7: LAUNCH_LM(7); break;
-    case 27:
-      if (G == 3) LAUNCH_LM_G(27, 3);
-      else LAUNCH_LM_G(27, 1);
-      break;
-    default: LAUNCH_LM(0); break;
-  }
-#undef LAUNCH_LM_G
-#undef LAUNCH_LM
   prof_end(h, h->stream);
   h->launches++;
   CU_TRY(h, cudaGetLastError());
@@ -822,71 +792,43 @@ int ndt_prepare(vgicp_handle h) {
   return VGICP_OK;
 }
 
-int evaluate(vgicp_handle h, const double* T, double* H36, double* b6, double* err) {
-  const bool want_H = (H36 != nullptr && b6 != nullptr);  // compute_derivatives.cu:160
-  const bool direct = h->exec_hint == 0;  // latency mode: result written to mapped host memory, host spins on a flag
-  int rc = launch_linearize(h, to_pose(T), want_H, direct);
-  if (rc) return rc;
-  if (direct) {
-    const unsigned long long want = h->eval_seq;
-    volatile unsigned long long* flag = h->h_flag;
-    long spins = 0;
-    while (*flag != want) {
-      __builtin_ia32_pause();
-      if (++spins > 2000000L) {  // ~a few ms without an answer: fall back to a blocking wait (also surfaces launch errors)
-        CU_TRY(h, cudaStreamSynchronize(h->stream));
-        if (*flag != want) return fail(h, VGICP_ERR_CUDA, "evaluate: kernel finished without publishing its result");
-        break;
+// Waits for the records of the launch just enqueued and leaves them in `host`.  Latency hint: the kernels write them to mapped host
+// memory and then set the completion words done[0, n) to seq, on which the host spins; throughput hint: `count` doubles are copied
+// back from `dev` behind the launch.
+int wait_records(vgicp_handle h, const volatile unsigned long long* done, int n, unsigned long long seq, double* host, const double* dev, size_t count) {
+  if (h->exec_hint == 0) {
+    for (int r = 0; r < n; r++) {
+      long spins = 0;
+      while (done[r] != seq) {
+        __builtin_ia32_pause();
+        if (++spins > 2000000L) {  // ~a few ms without an answer: fall back to a blocking wait (also surfaces launch errors)
+          CU_TRY(h, cudaStreamSynchronize(h->stream));
+          if (done[r] != seq) return fail(h, VGICP_ERR_CUDA, "evaluation kernel finished without publishing its result");
+          break;
+        }
       }
     }
     __sync_synchronize();
   } else {
-    CU_TRY(h, cudaMemcpyAsync(h->h_out, h->d_out, sizeof(double) * (h->comm_ranks > 1 ? kLinOutCommError + 1 : (want_H ? 43 : 1)), cudaMemcpyDeviceToHost, h->stream));
+    CU_TRY(h, cudaMemcpyAsync(host, dev, count * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
     CU_TRY(h, cudaStreamSynchronize(h->stream));
-  }
-  if (h->comm_ranks > 1 && h->h_out[kLinOutCommError] != 0.0) return fail(h, VGICP_ERR_COMM, "evaluate: a peer rank did not deliver its sums in time (vgicp_comm_error)");
-  if (err) *err = h->h_out[0];
-  if (want_H) {
-    memcpy(H36, h->h_out + 1, 36 * sizeof(double));
-    memcpy(b6, h->h_out + 37, 6 * sizeof(double));
   }
   return VGICP_OK;
 }
 
-// trial-pose evaluation for the LM loop: error at T over the current correspondences (*err_old) plus the linearisation at T itself
-// (k_linearize_spec); h->lin stays the current linearisation point
-int evaluate_spec(vgicp_handle h, const double* T, double* err_old, double* H36, double* b6, double* err_new) {
-  const bool direct = h->exec_hint == 0;
-  int rc = launch_linearize(h, to_pose(T), true, direct, true);
+// One single-pose evaluation at Teval over the correspondences of h->lin.  *rec: the result mailbox, valid until the next one:
+// [0] err, [1..36] H and [37..42] b (kEvalLinearize, kEvalSpec: at Teval itself), [43] err over the correspondences of h->lin (kEvalSpec)
+int evaluate(vgicp_handle h, const Pose& Teval, int kind, const double** rec) {
+  int rc = launch_linearize(h, Teval, kind);
   if (rc) return rc;
-  if (direct) {
-    const unsigned long long want = h->eval_seq;
-    volatile unsigned long long* flag = h->h_flag;
-    long spins = 0;
-    while (*flag != want) {
-      __builtin_ia32_pause();
-      if (++spins > 2000000L) {
-        CU_TRY(h, cudaStreamSynchronize(h->stream));
-        if (*flag != want) return fail(h, VGICP_ERR_CUDA, "evaluate: kernel finished without publishing its result");
-        break;
-      }
-    }
-    __sync_synchronize();
-  } else {
-    CU_TRY(h, cudaMemcpyAsync(h->h_out, h->d_out, sizeof(double) * (kLinOutCommError + 1), cudaMemcpyDeviceToHost, h->stream));
-    CU_TRY(h, cudaStreamSynchronize(h->stream));
-  }
+  const size_t count = (h->comm_ranks > 1 || kind == kEvalSpec) ? kLinOutCommError + 1 : (kind == kEvalLinearize ? 43 : 1);
+  if ((rc = wait_records(h, h->h_flag, 1, h->eval_seq, h->h_out, h->d_out, count))) return rc;
   if (h->comm_ranks > 1 && h->h_out[kLinOutCommError] != 0.0) return fail(h, VGICP_ERR_COMM, "evaluate: a peer rank did not deliver its sums in time (vgicp_comm_error)");
-  *err_new = h->h_out[0];
-  memcpy(H36, h->h_out + 1, 36 * sizeof(double));
-  memcpy(b6, h->h_out + 37, 6 * sizeof(double));
-  *err_old = h->h_out[43];
+  *rec = h->h_out;
   return VGICP_OK;
 }
 
 // ---- multi-pose evaluation (vgicp_align_multi, vgicp_evaluate_poses) -------------------------------------------------------
-enum { kEvalLinearize = 0, kEvalError = 1, kEvalSpec = 2 };  // what every row of one multi-pose launch computes
-
 // the preconditions of vgicp_align, for the calls that evaluate many poses
 int check_ready_for_multi(vgicp_handle h, const char* who) {
   if (h->comm_ranks > 1) return fail(h, VGICP_ERR_UNSUPPORTED, std::string(who) + ": not available on a handle in a multi-GPU communicator");
@@ -990,36 +932,134 @@ int launch_multi(vgicp_handle h, const LinLaunch& L, int n_hyp, int kind, bool c
 
 // waits for rows [0, n_rows) of the current round; returns the records (host memory, kMultiOut doubles per row)
 int multi_wait(vgicp_handle h, int n_rows, const double** rec) {
-  if (h->exec_hint == 0) {  // latency: every row's last block writes its record to mapped memory and then its completion word
-    volatile unsigned long long* done = h->h_multi_done;
-    for (int r = 0; r < n_rows; r++) {
-      long spins = 0;
-      while (done[r] != h->multi_seq) {
-        __builtin_ia32_pause();
-        if (++spins > 2000000L) {  // fall back to a blocking wait (also surfaces launch errors)
-          CU_TRY(h, cudaStreamSynchronize(h->stream));
-          if (done[r] != h->multi_seq) return fail(h, VGICP_ERR_CUDA, "multi-pose evaluation: kernel finished without publishing its result");
-          break;
-        }
-      }
-    }
-    __sync_synchronize();
-  } else {
-    CU_TRY(h, cudaMemcpyAsync(h->h_multi_out, h->d_multi_out, (size_t)n_rows * kMultiOut * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-    CU_TRY(h, cudaStreamSynchronize(h->stream));
-  }
   *rec = h->h_multi_out;
-  return VGICP_OK;
+  return wait_records(h, h->h_multi_done, n_rows, h->multi_seq, h->h_multi_out, h->d_multi_out, (size_t)n_rows * kMultiOut);
 }
 
-// lm_advance, plus the one case where the state machine and vgicp_align's loop part ways: with lm_max_iterations <= 0 the loop
-// tries no step at all and reports "lm not converged" right after the linearisation
-void multi_advance(LmState* st, const double* out) {
-  lm_advance(st, out);
-  if (st->phase == kLmError && st->lm_max_iterations <= 0) {
-    st->lm_failed = 1;
-    st->phase = kLmDone;
+// ---- LsqRegistration::computeTransformation (lsq_registration_impl.hpp:53-79) with step_gn (:106-120) / step_lm (:123-168) --------
+// as a state machine that takes one evaluation record at a time, in host double arithmetic.  vgicp_align drives one with single-pose
+// launches, vgicp_align_multi many with shared multi-pose launches.  The lookup pose of every evaluation is the float image of x0
+// (x0 does not move between a linearisation and its trials); it is evaluated at x0 in phase kLmLinearize, at xi in phase kLmError.
+struct LmState {
+  vgicp_lsq_params p;
+  Iso3d x0, xi, delta;  // estimate, LM trial pose, increment of the last step
+  double H[36], b[6], d[6], final_H[36];
+  double y0, lambda, nu;
+  int phase;  // kLmLinearize: err, H, b at x0;  kLmError: err at xi over the correspondences of x0;  kLmDone
+  int it, lm_j, converged, lm_failed, n_linearize, n_error, nr_iterations;
+};
+enum { kLmLinearize = 0, kLmError = 1, kLmDone = 2 };
+
+LmState lm_init(const double* guess, const vgicp_lsq_params& P) {
+  LmState st;
+  memset(&st, 0, sizeof(st));
+  st.p = P;
+  memcpy(st.x0.m, guess, sizeof(st.x0.m));
+  for (int j = 0; j < 6; j++) st.final_H[j * 7] = 1.0;  // final_hessian_.setIdentity()
+  st.lambda = -1.0;
+  st.nu = 2.0;
+  st.phase = P.max_iterations > 0 ? kLmLinearize : kLmDone;
+  return st;
+}
+
+void lm_propose(LmState* st) {  // solve (H + lambda I) d = -b, delta = exp(d), xi = delta * x0   (:134-139)
+  double Hl[36], nb[6];
+  memcpy(Hl, st->H, sizeof(Hl));
+  for (int q = 0; q < 6; q++) { Hl[q * 7] += st->lambda; nb[q] = -st->b[q]; }
+  ldlt_solve6(Hl, nb, st->d);
+  st->delta = se3_exp(st->d);
+  st->xi = iso_mul(st->delta, st->x0);
+  st->phase = kLmError;
+}
+
+void lm_finish_outer(LmState* st) {  // end of step_optimize: converged_ = is_converged(delta), next outer iteration (:65-75)
+  st->converged = is_converged(st->delta, st->p.rotation_epsilon, st->p.transformation_epsilon) ? 1 : 0;
+  st->it++;
+  if (st->converged || st->it >= st->p.max_iterations) { st->phase = kLmDone; return; }
+  st->nr_iterations = st->it;
+  st->phase = kLmLinearize;
+}
+
+void lm_advance(LmState* st, const double* out /*err, H, b*/) {
+  if (st->phase == kLmLinearize) {
+    st->y0 = out[0];
+    memcpy(st->H, out + 1, sizeof(st->H));
+    memcpy(st->b, out + 37, sizeof(st->b));
+    st->n_linearize++;
+    if (st->p.use_gauss_newton) {  // step_gn
+      double nb[6];
+      for (int q = 0; q < 6; q++) nb[q] = -st->b[q];
+      ldlt_solve6(st->H, nb, st->d);
+      st->delta = se3_exp(st->d);
+      st->x0 = iso_mul(st->delta, st->x0);
+      memcpy(st->final_H, st->H, sizeof(st->H));
+      lm_finish_outer(st);
+      return;
+    }
+    if (st->lambda < 0.0) {  // :128-130
+      double mx = 0.0;
+      for (int j = 0; j < 6; j++) mx = fmax(mx, fabs(st->H[j * 7]));
+      st->lambda = st->p.lm_init_lambda_factor * mx;
+    }
+    st->nu = 2.0;
+    st->lm_j = 0;
+    if (st->p.lm_max_iterations <= 0) {  // step_lm tries no step and returns false: "lm not converged!!"
+      st->lm_failed = 1;
+      st->phase = kLmDone;
+      return;
+    }
+    lm_propose(st);
+    return;
   }
+  // phase == kLmError  (:140-164)
+  const double yi = out[0];
+  st->n_error++;
+  double den = 0.0;
+  for (int q = 0; q < 6; q++) den += st->d[q] * (st->lambda * st->d[q] - st->b[q]);
+  const double rho = (st->y0 - yi) / den;
+  if (rho < 0) {
+    if (is_converged(st->delta, st->p.rotation_epsilon, st->p.transformation_epsilon)) { lm_finish_outer(st); return; }  // :151-154
+    st->lambda = st->nu * st->lambda;
+    st->nu = 2 * st->nu;
+    st->lm_j++;
+    if (st->lm_j >= st->p.lm_max_iterations) {  // step_lm returns false -> "lm not converged!!" (:69-72)
+      st->lm_failed = 1;
+      st->phase = kLmDone;
+      return;
+    }
+    lm_propose(st);
+    return;
+  }
+  st->x0 = st->xi;  // :161-164
+  const double f = 1.0 - pow(2.0 * rho - 1.0, 3);
+  st->lambda = st->lambda * fmax(1.0 / 3.0, f);
+  memcpy(st->final_H, st->H, sizeof(st->H));
+  lm_finish_outer(st);
+}
+
+// Takes one evaluation record (the single-pose mailbox and a multi-pose row share the layout: err, H, b in [0..42], [43] the trial's
+// error over the current correspondences in a kEvalSpec record).  A speculative record's [43] decides the trial; when the trial is
+// accepted and the optimisation goes on, the linearisation at the trial pose in [0..42] is taken at once.  Returns true in that case.
+bool lm_consume(LmState* st, const double* rec, bool spec) {
+  if (!spec) {
+    lm_advance(st, rec);
+    return false;
+  }
+  lm_advance(st, rec + 43);
+  if (st->phase != kLmLinearize) return false;
+  lm_advance(st, rec);
+  return true;
+}
+
+void lm_result(const LmState& st, vgicp_align_result* res) {
+  memset(res, 0, sizeof(*res));
+  memcpy(res->T, st.x0.m, sizeof(res->T));
+  memcpy(res->H, st.final_H, sizeof(res->H));
+  res->nr_iterations = st.nr_iterations;
+  res->converged = st.converged;
+  res->n_linearize = st.n_linearize;
+  res->n_compute_error = st.n_error;
+  res->lm_failed = st.lm_failed;
 }
 
 }  // namespace
@@ -1067,8 +1107,6 @@ int vgicp_create(int device, vgicp_handle* out) {
   ok = ok && cudaHostAlloc(&h->h_out, 64 * sizeof(double), cudaHostAllocMapped) == cudaSuccess;
   ok = ok && cudaHostAlloc(&h->h_flag, 64, cudaHostAllocMapped) == cudaSuccess;
   if (ok) *h->h_flag = 0;
-  ok = ok && cudaMalloc(&h->d_lm, sizeof(LmState)) == cudaSuccess;
-  ok = ok && cudaMallocHost(&h->h_lm, sizeof(LmState)) == cudaSuccess;
   ok = ok && h->partials.reserve((size_t)kLinStreamMaxBlocks * kLinStride) == cudaSuccess;
   ok = ok && cudaMemsetAsync(h->d_ticket, 0, sizeof(unsigned int), h->stream) == cudaSuccess;
   ok = ok && cudaStreamSynchronize(h->stream) == cudaSuccess;
@@ -1108,8 +1146,6 @@ int vgicp_destroy(vgicp_handle h) {
   if (h->d_out) cudaFree(h->d_out);
   if (h->h_out) cudaFreeHost(h->h_out);
   if (h->h_flag) cudaFreeHost(h->h_flag);
-  if (h->d_lm) cudaFree(h->d_lm);
-  if (h->h_lm) cudaFreeHost(h->h_lm);
   h->multi_partials.release();
   if (h->d_multi_tickets) cudaFree(h->d_multi_tickets);
   if (h->d_multi_in) cudaFree(h->d_multi_in);
@@ -1456,7 +1492,15 @@ int vgicp_compute_error(vgicp_handle h, const double T[16], double* H36, double*
   int rc = check_ready_for_eval(h, "compute_error");
   if (rc) return rc;
   if ((rc = sync_inputs(h))) return rc;
-  return evaluate(h, T, H36, b6, err);
+  const bool want_H = (H36 != nullptr && b6 != nullptr);  // compute_derivatives.cu:160
+  const double* rec = nullptr;
+  if ((rc = evaluate(h, to_pose(T), want_H ? kEvalLinearize : kEvalError, &rec))) return rc;
+  if (err) *err = rec[0];
+  if (want_H) {
+    memcpy(H36, rec + 1, 36 * sizeof(double));
+    memcpy(b6, rec + 37, 6 * sizeof(double));
+  }
+  return VGICP_OK;
 }
 
 void vgicp_lsq_default_params(vgicp_lsq_params* p) {  // lsq_registration_impl.hpp:9-22
@@ -1470,7 +1514,8 @@ void vgicp_lsq_default_params(vgicp_lsq_params* p) {  // lsq_registration_impl.h
 }
 
 // LsqRegistration::computeTransformation (lsq_registration_impl.hpp:53-79) with step_gn (:106-120) / step_lm (:123-168);
-// linearize = update_correspondences + compute_error (fast_vgicp_cuda_impl.hpp:170-173).
+// linearize = update_correspondences + compute_error (fast_vgicp_cuda_impl.hpp:170-173).  One single-pose launch per step of the
+// state machine.  With LM and speculation every trial also linearises at the trial pose, so an accepted step needs no launch of its own.
 int vgicp_align(vgicp_handle h, const double guess[16], const vgicp_lsq_params* params, vgicp_align_result* res) {
   CHECK_HANDLE(h);
   DeviceGuard g(h->device);
@@ -1484,130 +1529,27 @@ int vgicp_align(vgicp_handle h, const double guess[16], const vgicp_lsq_params* 
     return fail(h, VGICP_ERR_BAD_STATE, "align: NDT needs source and target clouds");
   }
   { int rc = sync_inputs(h); if (rc) return rc; }
-
-  if (h->align_mode == 0) {
-    // device-resident loop: initialise the state block, enqueue evaluation links, read the state back once per chunk
-    LmState* st = h->h_lm;
-    memset(st, 0, sizeof(LmState));
-    memcpy(st->x0, guess, sizeof(st->x0));
-    for (int i = 0; i < 6; i++) st->final_H[i * 7] = 1.0;  // final_hessian_.setIdentity()
-    st->lambda = -1.0;
-    st->nu = 2.0;
-    st->rotation_epsilon = P.rotation_epsilon;
-    st->transformation_epsilon = P.transformation_epsilon;
-    st->lm_init_lambda_factor = P.lm_init_lambda_factor;
-    st->max_iterations = P.max_iterations;
-    st->lm_max_iterations = P.lm_max_iterations;
-    st->use_gauss_newton = P.use_gauss_newton;
-    st->phase = P.max_iterations > 0 ? kLmLinearize : kLmDone;
-    st->lin_pose = to_pose(guess);
-    st->eval_pose = st->lin_pose;
-    CU_TRY(h, cudaMemcpyAsync(h->d_lm, st, sizeof(LmState), cudaMemcpyHostToDevice, h->stream));
-    const LinLaunch L = make_lin_launch(h);
-    const int chunk = 12;  // a typical registration needs ~10 evaluations; finished chains return immediately
-    for (int guard = 0; guard < 4096; guard++) {
-      for (int c = 0; c < chunk; c++) {
-        int rc = launch_lm_step(h, L);
-        if (rc) return rc;
-      }
-      CU_TRY(h, cudaMemcpyAsync(st, h->d_lm, sizeof(LmState), cudaMemcpyDeviceToHost, h->stream));
-      CU_TRY(h, cudaStreamSynchronize(h->stream));
-      if (st->phase == kLmDone) break;
-    }
-    memset(res, 0, sizeof(*res));
-    memcpy(res->T, st->x0, sizeof(res->T));
-    memcpy(res->H, st->final_H, sizeof(res->H));
-    res->nr_iterations = st->nr_iterations;
-    res->converged = st->converged;
-    res->n_linearize = st->n_linearize;
-    res->n_compute_error = st->n_error;
-    res->lm_failed = st->lm_failed;
-    h->lin = st->lin_pose;  // linearized_x of the last linearisation
-    h->has_lin = true;
-    return VGICP_OK;
-  }
-
-  Iso3d x0;
-  memcpy(x0.m, guess, sizeof(x0.m));
-  double lambda = -1.0;
-  bool converged = false;
-  memset(res, 0, sizeof(*res));
-  for (int i = 0; i < 6; i++) res->H[i * 7] = 1.0;  // final_hessian_.setIdentity()
-  // speculative evaluation: every LM trial also linearises at the trial pose, so an accepted step needs no launch of its own
   const bool speculate = h->speculate != 0 && !P.use_gauss_newton;
-  bool have_next = false;
-  double Hn[36], bn[6], yn = 0.0;
-  for (int it = 0; it < P.max_iterations && !converged; it++) {
-    res->nr_iterations = it;
-    double H[36], b[6], nb[6], d[6], y0 = 0.0;
-    h->lin = to_pose(x0.m);
-    h->has_lin = true;
-    int rc = VGICP_OK;
-    if (have_next) {  // linearised at this very pose by the trial evaluation that accepted it
-      memcpy(H, Hn, sizeof(H)); memcpy(b, bn, sizeof(b)); y0 = yn;
-      have_next = false;
-    } else {
-      rc = evaluate(h, x0.m, H, b, &y0);
+  LmState st = lm_init(guess, P);
+  while (st.phase != kLmDone) {
+    const bool lin = st.phase == kLmLinearize;
+    const Pose Teval = to_pose(lin ? st.x0.m : st.xi.m);
+    if (lin) {  // linearized_x: the correspondences of this evaluation and of the trials from it
+      h->lin = Teval;
+      h->has_lin = true;
     }
+    const double* rec = nullptr;
+    int rc = evaluate(h, Teval, lin ? kEvalLinearize : (speculate ? kEvalSpec : kEvalError), &rec);
     if (rc) return rc;
-    res->n_linearize++;
-    for (int j = 0; j < 6; j++) nb[j] = -b[j];
-    Iso3d delta = iso_identity();
-    bool ok = false;
-    if (P.use_gauss_newton) {
-      ldlt_solve6(H, nb, d);
-      delta = se3_exp(d);
-      x0 = iso_mul(delta, x0);
-      memcpy(res->H, H, sizeof(H));
-      ok = true;
-    } else {
-      if (lambda < 0.0) {
-        double mx = 0.0;
-        for (int j = 0; j < 6; j++) mx = fmax(mx, fabs(H[j * 7]));
-        lambda = P.lm_init_lambda_factor * mx;
-      }
-      double nu = 2.0;
-      for (int j = 0; j < P.lm_max_iterations; j++) {
-        double Hl[36];
-        memcpy(Hl, H, sizeof(H));
-        for (int q = 0; q < 6; q++) Hl[q * 7] += lambda;
-        ldlt_solve6(Hl, nb, d);
-        delta = se3_exp(d);
-        Iso3d xi = iso_mul(delta, x0);
-        double yi = 0.0;
-        rc = speculate ? evaluate_spec(h, xi.m, &yi, Hn, bn, &yn) : evaluate(h, xi.m, nullptr, nullptr, &yi);
-        if (rc) return rc;
-        res->n_compute_error++;
-        double den = 0.0;
-        for (int q = 0; q < 6; q++) den += d[q] * (lambda * d[q] - b[q]);
-        double rho = (y0 - yi) / den;
-        if (rho < 0) {
-          if (is_converged(delta, P.rotation_epsilon, P.transformation_epsilon)) { ok = true; break; }
-          lambda = nu * lambda;
-          nu = 2 * nu;
-          continue;
-        }
-        x0 = xi;
-        have_next = speculate;
-        double f = 1.0 - pow(2.0 * rho - 1.0, 3);
-        lambda = lambda * fmax(1.0 / 3.0, f);
-        memcpy(res->H, H, sizeof(H));
-        ok = true;
-        break;
-      }
-    }
-    if (!ok) { res->lm_failed = 1; break; }  // "lm not converged!!"
-    converged = is_converged(delta, P.rotation_epsilon, P.transformation_epsilon);
+    if (lm_consume(&st, rec, !lin && speculate)) h->lin = Teval;  // accepted trial, linearised at its pose by the same launch
   }
-  memcpy(res->T, x0.m, sizeof(x0.m));
-  res->converged = converged ? 1 : 0;
+  lm_result(st, res);
   return VGICP_OK;
 }
 
-// B registrations from B initial guesses.  Each hypothesis runs the LM / GN state machine of the device-resident loop (lm_advance,
-// which walks vgicp_align's iterates), here on the host; every round stages the poses of the running hypotheses and evaluates all
-// of them in one launch per evaluation kind.  With LM and speculation every round after the first is one k_linearize_spec_multi
-// launch: an accepted trial's linearisation feeds the hypothesis's next lm_advance at once, as vgicp_align's have_next does.
+// B registrations from B initial guesses.  Each hypothesis runs vgicp_align's state machine; every round stages the poses of the
+// running hypotheses and evaluates all of them in one launch per evaluation kind.  With LM and speculation every round after the
+// first is one k_linearize_spec_multi launch, whose accepted trials feed their linearisation straight back, as in vgicp_align.
 int vgicp_align_multi(vgicp_handle h, const double* guesses, int n_guesses, const vgicp_lsq_params* params, vgicp_align_result* results) {
   CHECK_HANDLE(h);
   DeviceGuard g(h->device);
@@ -1621,72 +1563,34 @@ int vgicp_align_multi(vgicp_handle h, const double* guesses, int n_guesses, cons
   const LinLaunch L = make_lin_launch(h);
   if ((rc = multi_reserve(h, B, multi_grid(h, L)))) return rc;
   std::vector<LmState> st(B);
-  for (int i = 0; i < B; i++) {  // as vgicp_align's device-resident branch initialises its state block
-    LmState& s = st[i];
-    memset(&s, 0, sizeof(LmState));
-    memcpy(s.x0, guesses + 16 * i, sizeof(s.x0));
-    for (int j = 0; j < 6; j++) s.final_H[j * 7] = 1.0;
-    s.lambda = -1.0;
-    s.nu = 2.0;
-    s.rotation_epsilon = P.rotation_epsilon;
-    s.transformation_epsilon = P.transformation_epsilon;
-    s.lm_init_lambda_factor = P.lm_init_lambda_factor;
-    s.max_iterations = P.max_iterations;
-    s.lm_max_iterations = P.lm_max_iterations;
-    s.use_gauss_newton = P.use_gauss_newton;
-    s.phase = P.max_iterations > 0 ? kLmLinearize : kLmDone;
-    s.lin_pose = to_pose(guesses + 16 * i);
-    s.eval_pose = s.lin_pose;
-  }
+  for (int i = 0; i < B; i++) st[i] = lm_init(guesses + 16 * i, P);
   const bool speculate = h->speculate != 0 && !P.use_gauss_newton;
-  std::vector<int> lin_rows, err_rows;
-  lin_rows.reserve(B);
-  err_rows.reserve(B);
   for (;;) {
-    lin_rows.clear();
-    err_rows.clear();
     Pose* poses = multi_poses(h);
-    for (int i = 0; i < B; i++) {
-      if (st[i].phase == kLmDone) continue;
-      (st[i].phase == kLmLinearize ? lin_rows : err_rows).push_back(i);
-      poses[2 * i] = st[i].lin_pose;
-      poses[2 * i + 1] = st[i].eval_pose;
-    }
-    const int n_lin = (int)lin_rows.size(), n_err = (int)err_rows.size();
-    if (n_lin + n_err == 0) break;
     int* rows = multi_rows(h, B);
-    memcpy(rows, lin_rows.data(), n_lin * sizeof(int));
-    memcpy(rows + n_lin, err_rows.data(), n_err * sizeof(int));
-    h->multi_seq++;
-    if ((rc = multi_upload(h, B, n_lin + n_err))) return rc;
-    if (n_lin && (rc = launch_multi(h, L, B, kEvalLinearize, false, 0, n_lin))) return rc;
-    if (n_err && (rc = launch_multi(h, L, B, speculate ? kEvalSpec : kEvalError, false, n_lin, n_err))) return rc;
-    const double* rec = nullptr;
-    if ((rc = multi_wait(h, n_lin + n_err, &rec))) return rc;
-    for (int r = 0; r < n_lin; r++) multi_advance(&st[lin_rows[r]], rec + (size_t)r * kMultiOut);
-    for (int r = 0; r < n_err; r++) {
-      const double* o = rec + (size_t)(n_lin + r) * kMultiOut;
-      LmState* s = &st[err_rows[r]];
-      if (!speculate) {
-        multi_advance(s, o);
-        continue;
+    int n = 0;
+    for (int i = 0; i < B; i++)
+      if (st[i].phase == kLmLinearize) {
+        rows[n++] = i;
+        poses[2 * i] = poses[2 * i + 1] = to_pose(st[i].x0.m);
       }
-      const double e_old[43] = {o[43]};  // the trial's error over the current correspondences decides the step (read: [0])
-      multi_advance(s, e_old);
-      if (s->phase == kLmLinearize) multi_advance(s, o);  // accepted: x0 is the trial pose, linearised by the same launch
-    }
+    const int n_lin = n;
+    for (int i = 0; i < B; i++)
+      if (st[i].phase == kLmError) {
+        rows[n++] = i;
+        poses[2 * i] = to_pose(st[i].x0.m);
+        poses[2 * i + 1] = to_pose(st[i].xi.m);
+      }
+    if (n == 0) break;
+    h->multi_seq++;
+    if ((rc = multi_upload(h, B, n))) return rc;
+    if (n_lin && (rc = launch_multi(h, L, B, kEvalLinearize, false, 0, n_lin))) return rc;
+    if (n > n_lin && (rc = launch_multi(h, L, B, speculate ? kEvalSpec : kEvalError, false, n_lin, n - n_lin))) return rc;
+    const double* rec = nullptr;
+    if ((rc = multi_wait(h, n, &rec))) return rc;
+    for (int r = 0; r < n; r++) lm_consume(&st[rows[r]], rec + (size_t)r * kMultiOut, r >= n_lin && speculate);
   }
-  for (int i = 0; i < B; i++) {
-    vgicp_align_result& res = results[i];
-    memset(&res, 0, sizeof(res));
-    memcpy(res.T, st[i].x0, sizeof(res.T));
-    memcpy(res.H, st[i].final_H, sizeof(res.H));
-    res.nr_iterations = st[i].nr_iterations;
-    res.converged = st[i].converged;
-    res.n_linearize = st[i].n_linearize;
-    res.n_compute_error = st[i].n_error;
-    res.lm_failed = st[i].lm_failed;
-  }
+  for (int i = 0; i < B; i++) lm_result(st[i], &results[i]);
   return VGICP_OK;
 }
 
@@ -1950,13 +1854,6 @@ int vgicp_set_execution_hint(vgicp_handle h, int hint) {
   CHECK_HANDLE(h);
   if (hint < 0 || hint > 1) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "set_execution_hint: 0 latency, 1 throughput");
   h->exec_hint = hint;
-  return VGICP_OK;
-}
-
-int vgicp_set_align_mode(vgicp_handle h, int mode) {
-  CHECK_HANDLE(h);
-  if (mode < 0 || mode > 1) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "set_align_mode: 0 device-resident loop, 1 host-driven loop");
-  h->align_mode = mode;
   return VGICP_OK;
 }
 

@@ -20,7 +20,6 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-#include "lsq_math.hpp"
 #include "vgicp_sort.cuh"
 #include "vgicp_stage1.cuh"
 
@@ -1160,147 +1159,6 @@ __global__ void __launch_bounds__(kLinThreads, 1) k_linearize_stream_multi(const
     }
     if (COUNT) rec[kMultiOutCount] = fin[0][NB];
     multi_publish(m, y);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// Device-resident optimiser: LsqRegistration::computeTransformation (lsq_registration_impl.hpp:53-79) with step_gn
-// (:106-120) / step_lm (:123-168) as a chain of evaluation kernels.  Each launch reads the phase and the two poses from
-// the state block, evaluates (linearize = lookup at x0 + H,b,err ; or error only at the candidate xi with the
-// correspondences of x0), and thread 0 of its last block advances the state machine in double -- exactly the host
-// logic, same arithmetic (lsq_math.hpp is shared).  A launch that finds phase == DONE returns at once, so the host
-// can enqueue a fixed number of launches and read the state back once.
-// The state machine is host+device: vgicp_align_multi runs one per hypothesis on the host (host libm, like vgicp_align's loop).
-// ---------------------------------------------------------------------------------------------------------------
-struct LmState {
-  double x0[16], xi[16], delta[16];
-  double H[36], b[6], d[6], final_H[36];
-  double y0, lambda, nu;
-  // parameters
-  double rotation_epsilon, transformation_epsilon, lm_init_lambda_factor;
-  int max_iterations, lm_max_iterations, use_gauss_newton;
-  // progress
-  int phase;  // 0 = linearize at x0, 1 = error at xi, 2 = done
-  int it, lm_j, converged, lm_failed, n_linearize, n_error, nr_iterations;
-  Pose lin_pose, eval_pose;
-};
-enum { kLmLinearize = 0, kLmError = 1, kLmDone = 2 };
-
-VGICP_HD Pose pose_from_iso(const double* T) {
-  Pose p;
-  for (int r = 0; r < 3; r++) {
-    for (int c = 0; c < 3; c++) p.r[r * 3 + c] = (float)T[c * 4 + r];
-    p.t[r] = (float)T[12 + r];
-  }
-  return p;
-}
-
-VGICP_HD void lm_propose(LmState* st) {  // solve (H + lambda I) d = -b, delta = exp(d), xi = delta * x0   (:134-139)
-  double Hl[36], nb[6];
-  for (int j = 0; j < 36; j++) Hl[j] = st->H[j];
-  for (int q = 0; q < 6; q++) { Hl[q * 7] += st->lambda; nb[q] = -st->b[q]; }
-  ldlt_solve6(Hl, nb, st->d);
-  Iso3d delta = se3_exp(st->d);
-  Iso3d x0;
-  for (int j = 0; j < 16; j++) x0.m[j] = st->x0[j];
-  Iso3d xi = iso_mul(delta, x0);
-  for (int j = 0; j < 16; j++) { st->delta[j] = delta.m[j]; st->xi[j] = xi.m[j]; }
-  st->eval_pose = pose_from_iso(st->xi);
-  st->phase = kLmError;
-}
-
-VGICP_HD void lm_finish_outer(LmState* st) {  // end of step_optimize: converged_ = is_converged(delta), next outer iteration (:65-75)
-  Iso3d delta;
-  for (int j = 0; j < 16; j++) delta.m[j] = st->delta[j];
-  st->converged = is_converged(delta, st->rotation_epsilon, st->transformation_epsilon) ? 1 : 0;
-  st->it++;
-  if (st->converged || st->it >= st->max_iterations) { st->phase = kLmDone; return; }
-  st->nr_iterations = st->it;
-  st->lin_pose = pose_from_iso(st->x0);
-  st->eval_pose = st->lin_pose;
-  st->phase = kLmLinearize;
-}
-
-VGICP_HD void lm_advance(LmState* st, const double* out /*err, H, b*/) {
-  if (st->phase == kLmLinearize) {
-    st->y0 = out[0];
-    for (int j = 0; j < 36; j++) st->H[j] = out[1 + j];
-    for (int j = 0; j < 6; j++) st->b[j] = out[37 + j];
-    st->n_linearize++;
-    if (st->use_gauss_newton) {  // step_gn
-      double nb[6];
-      for (int q = 0; q < 6; q++) nb[q] = -st->b[q];
-      ldlt_solve6(st->H, nb, st->d);
-      Iso3d delta = se3_exp(st->d), x0;
-      for (int j = 0; j < 16; j++) x0.m[j] = st->x0[j];
-      x0 = iso_mul(delta, x0);
-      for (int j = 0; j < 16; j++) { st->x0[j] = x0.m[j]; st->delta[j] = delta.m[j]; }
-      for (int j = 0; j < 36; j++) st->final_H[j] = st->H[j];
-      lm_finish_outer(st);
-      return;
-    }
-    if (st->lambda < 0.0) {  // :128-130
-      double mx = 0.0;
-      for (int j = 0; j < 6; j++) mx = fmax(mx, fabs(st->H[j * 7]));
-      st->lambda = st->lm_init_lambda_factor * mx;
-    }
-    st->nu = 2.0;
-    st->lm_j = 0;
-    lm_propose(st);
-    return;
-  }
-  // phase == kLmError  (:140-164)
-  const double yi = out[0];
-  st->n_error++;
-  double den = 0.0;
-  for (int q = 0; q < 6; q++) den += st->d[q] * (st->lambda * st->d[q] - st->b[q]);
-  const double rho = (st->y0 - yi) / den;
-  if (rho < 0) {
-    Iso3d delta;
-    for (int j = 0; j < 16; j++) delta.m[j] = st->delta[j];
-    if (is_converged(delta, st->rotation_epsilon, st->transformation_epsilon)) { lm_finish_outer(st); return; }  // :151-154
-    st->lambda = st->nu * st->lambda;
-    st->nu = 2 * st->nu;
-    st->lm_j++;
-    if (st->lm_j >= st->lm_max_iterations) {  // step_lm returns false -> "lm not converged!!" (:69-72)
-      st->lm_failed = 1;
-      st->phase = kLmDone;
-      return;
-    }
-    lm_propose(st);
-    return;
-  }
-  for (int j = 0; j < 16; j++) st->x0[j] = st->xi[j];  // :161-164
-  const double f = 1.0 - pow(2.0 * rho - 1.0, 3);
-  st->lambda = st->lambda * fmax(1.0 / 3.0, f);
-  for (int j = 0; j < 36; j++) st->final_H[j] = st->H[j];
-  lm_finish_outer(st);
-}
-
-template <int MODE, int G>
-__global__ void __launch_bounds__(kLinThreads) k_lm_step(const LinArgs a, LmState* st) {
-  __shared__ double fin[4][kLinStride];
-  __shared__ double out[44];
-  const int phase = st->phase;
-  if (phase == kLmDone) return;
-  const Pose Tl = st->lin_pose, Te = st->eval_pose;
-  bool last;
-  if (phase == kLmLinearize) {
-    float sum[kLinValues];
-    lin_accumulate<MODE, true, G>(a, Tl, Te, sum);
-    last = lin_reduce<kLinValues>(a, sum, fin);
-  } else {
-    float sum[1];
-    lin_accumulate<MODE, false, G>(a, Tl, Te, sum);
-    last = lin_reduce<1>(a, sum, fin);
-  }
-  if (!last) return;
-  if (threadIdx.x == 0) {
-    if (phase == kLmLinearize) lin_unpack<true>(fin[0], out);
-    else lin_unpack<false>(fin[0], out);
-    lm_advance(st, out);
-    __threadfence();
-    *a.ticket = 0u;
   }
 }
 

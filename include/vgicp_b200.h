@@ -150,8 +150,8 @@ typedef struct {
 VGICP_API void vgicp_lsq_default_params(vgicp_lsq_params* p);
 /* Whole LsqRegistration::computeTransformation loop (lsq_registration_impl.hpp:53-79,106-168) inside the library: the same
  * linearize / compute_error evaluations and the same LM / GN logic in double, without crossing the ABI once per evaluation.
- * Driven from the host by default (one 344-byte result per evaluation through mapped memory); vgicp_set_align_mode selects the
- * device-resident state machine, vgicp_set_speculation the fused trial evaluation.  result->T = final_transformation_. */
+ * Driven from the host (one 344-byte result per evaluation through mapped memory); vgicp_set_speculation selects the fused trial
+ * evaluation.  result->T = final_transformation_. */
 VGICP_API int vgicp_align(vgicp_handle h, const double guess[16], const vgicp_lsq_params* params, vgicp_align_result* result);
 /* ---- multi-hypothesis alignment (global localisation, relocalisation, loop-closure checks) ----------------------------------
  * B registrations of the current source against the current target map, from B initial guesses (B x 16 doubles, column-major),
@@ -159,7 +159,7 @@ VGICP_API int vgicp_align(vgicp_handle h, const double guess[16], const vgicp_ls
  * (with LM and speculation, one launch per round; with GN, one linearisation launch per round), each hypothesis a row of blocks
  * with the single-pose launch's grid, so its sums are the single-pose sums.  results[i] equals vgicp_align(h, guesses + 16 i,
  * params) bit for bit (T, H, nr_iterations, converged, n_linearize, n_compute_error, lm_failed), under either execution hint and
- * speculation setting; the host-driven LM loop is used whatever vgicp_set_align_mode says.  1 <= n_guesses <= 4096.
+ * speculation setting: both calls run the same optimiser state machine on the host.  1 <= n_guesses <= 4096.
  * The handle's linearisation point and the rest of its single-pose state are left as they were.  Working memory: 256 bytes per
  * evaluation block and hypothesis (about 0.1 MB per hypothesis at 17 k points, 0.27 MB at 1 M points with DIRECT1), grow-only.
  * Errors: VGICP_ERR_INVALID_ARGUMENT (null pointer, n_guesses out of range), VGICP_ERR_BAD_STATE (the preconditions of
@@ -223,11 +223,6 @@ VGICP_API int vgicp_ndt_create_voxelmaps(vgicp_handle h);
  * evaluations are read back with a copy and a stream wait, so the host thread sleeps instead of spinning).  Results are identical.
  * bench.py uses the latency shape. */
 VGICP_API int vgicp_set_execution_hint(vgicp_handle h, int hint);
-/* vgicp_align driver: 1 = host-driven loop over the evaluation kernels (default; one 344-byte readback per evaluation, like
- * the reference), 0 = device-resident loop (the LM state machine runs in the last block of each evaluation kernel, the host
- * reads one state block back per chunk of launches).  Both walk the same iterates; the serial double-precision LM step
- * on one GPU thread costs about what the host round trip saves, so the host-driven loop stays the default. */
-VGICP_API int vgicp_set_align_mode(vgicp_handle h, int mode);
 /* k-NN engine used by find_*_neighbors: 0 = multi-level hash grid (default), 1 = warp-cooperative scan of the whole cloud,
  * 2 = one-thread-per-query scan (the shape of the reference's brute_force_knn.cu).  All three return identical rows. */
 VGICP_API int vgicp_set_knn_mode(vgicp_handle h, int mode);

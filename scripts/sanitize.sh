@@ -8,11 +8,11 @@ sys.path.insert(0, ".")
 from fast_gicp_b200.core import Core
 d = np.load("tests/golden/pair_0p2.npz")
 tgt, src = d["target"][::3].copy(), d["source"][::3].copy()
-for method, knn_mode, align_mode, hint, vindex, spec in (("DIRECT27", 0, 1, 0, 0, 1), ("DIRECT7", 0, 0, 1, 0, 1), ("DIRECT1", 1, 1, 0, 1, 0), ("DIRECT_RADIUS", 0, 1, 1, 1, 1),
-                                                         ("DIRECT27", 0, 1, 0, 1, 0)):
+for method, knn_mode, hint, vindex, spec in (("DIRECT27", 0, 0, 0, 1), ("DIRECT7", 0, 1, 0, 1), ("DIRECT1", 1, 0, 1, 0), ("DIRECT_RADIUS", 0, 1, 1, 1),
+                                             ("DIRECT27", 0, 0, 1, 0)):
     c = Core(0)
     c.set_neighbor_search_method(method, 1.5)
-    c.set_knn_mode(knn_mode); c.set_align_mode(align_mode); c.set_execution_hint(hint)
+    c.set_knn_mode(knn_mode); c.set_execution_hint(hint)
     c.set_voxel_index(vindex); c.set_speculation(spec)
     r = c.register(tgt, src)
     c.calculate_source_covariances_rbf(3)

@@ -84,6 +84,7 @@ CASES = {
     "ndt_p2d": dict(method=O.DIRECT7, problem=1),
     "ndt_d2d": dict(method=O.DIRECT7, problem=2),
     "ndt_d2d_direct1": dict(method=O.DIRECT1, problem=2, spec=0),
+    "lm_no_trials": dict(method=O.DIRECT7, params=dict(lm_max_iterations=0)),
 }
 
 
@@ -97,14 +98,17 @@ def test_align_multi_is_bit_identical_to_align(pair02, relative_pose, case):
     c.set_speculation(cfg.get("spec", 1))
     c.set_voxel_index(cfg.get("index", 0))
     setup(c, *pair02, method=cfg["method"], radius=cfg.get("radius", -1.0), problem=cfg.get("problem", 0), rbf=cfg.get("rbf", False))
-    params = default_params(use_gauss_newton=cfg.get("gn", 0))
+    params = default_params(use_gauss_newton=cfg.get("gn", 0), **cfg.get("params", {}))
     G = guesses(relative_pose)
     multi = c.align_multi(G, params)
     assert len(multi) == len(G)
     for i, g in enumerate(G):
         assert_same(multi[i], c.align(g, params), f"{case} guess {i}")
     assert_same(multi[4], multi[21])  # the duplicated guess
-    assert sum(r.converged for r in multi) >= 4
+    if params.lm_max_iterations > 0:
+        assert sum(r.converged for r in multi) >= 4
+    else:  # step_lm tries no step: one linearisation each, then "lm not converged"
+        assert all(r.lm_failed and r.n_linearize == 1 and r.n_compute_error == 0 for r in multi)
     c.close()
 
 
