@@ -13,6 +13,7 @@ from .registration import (  # noqa: F401
     NearestNeighborMethod,
     NeighborSearchMethod,
     RegularizationMethod,
+    RobustKernel,
 )
 
 load_library()  # fail loudly at import time when the extension is missing

@@ -21,6 +21,9 @@ REG_NONE, REG_MIN_EIG, REG_NORMALIZED_MIN_EIG, REG_PLANE, REG_FROBENIUS = range(
 DIRECT27, DIRECT7, DIRECT1, DIRECT_RADIUS = range(4)
 REGULARIZATION = {"NONE": REG_NONE, "MIN_EIG": REG_MIN_EIG, "NORMALIZED_MIN_EIG": REG_NORMALIZED_MIN_EIG, "PLANE": REG_PLANE, "FROBENIUS": REG_FROBENIUS}
 NEIGHBOR_SEARCH = {"DIRECT27": DIRECT27, "DIRECT7": DIRECT7, "DIRECT1": DIRECT1, "DIRECT_RADIUS": DIRECT_RADIUS}
+# vgicp_set_robust_kernel kinds (include/vgicp_b200.h)
+ROBUST_NONE, ROBUST_HUBER, ROBUST_CAUCHY, ROBUST_GEMAN_MCCLURE = range(4)
+ROBUST_KERNEL = {"NONE": ROBUST_NONE, "HUBER": ROBUST_HUBER, "CAUCHY": ROBUST_CAUCHY, "GEMAN_MCCLURE": ROBUST_GEMAN_MCCLURE}
 
 # every symbol include/vgicp_b200.h declares (tests check the library exports all of them)
 EXPORTED_SYMBOLS = [
@@ -41,7 +44,7 @@ EXPORTED_SYMBOLS = [
     "vgicp_set_knn_mode", "vgicp_set_voxel_index", "vgicp_set_speculation", "vgicp_register", "vgicp_get_fitness_score", "vgicp_set_execution_hint", "vgicp_set_problem", "vgicp_ndt_create_voxelmaps",
     "vgicp_comm_export", "vgicp_comm_init", "vgicp_comm_shutdown", "vgicp_comm_error", "vgicp_set_source_shard", "vgicp_clear_source_shard",
     "vgicp_comm_export_arena", "vgicp_comm_init_arena", "vgicp_set_stage1_sharding", "vgicp_set_source_covariances", "vgicp_set_target_covariances",
-    "vgicp_align_multi", "vgicp_evaluate_poses",
+    "vgicp_align_multi", "vgicp_evaluate_poses", "vgicp_set_robust_kernel",
 ]
 PROF_NUM_CATEGORIES = 7
 
@@ -92,6 +95,7 @@ def load_library():
         "vgicp_destroy": [hp],
         "vgicp_set_resolution": [hp, C.c_double],
         "vgicp_set_kernel_params": [hp, C.c_double, C.c_double],
+        "vgicp_set_robust_kernel": [hp, C.c_int, C.c_double],
         "vgicp_set_neighbor_search_method": [hp, C.c_int, C.c_double],
         "vgicp_set_source_cloud": [hp, C.c_void_p, C.c_size_t, C.c_size_t],
         "vgicp_set_target_cloud": [hp, C.c_void_p, C.c_size_t, C.c_size_t],
@@ -221,6 +225,13 @@ class Core:
 
     def set_kernel_params(self, kernel_width, kernel_max_dist):
         self._check(self._lib.vgicp_set_kernel_params(self._h, float(kernel_width), float(kernel_max_dist)))
+
+    def set_robust_kernel(self, kind, scale=1.0):
+        """Robust kernel of the Mahalanobis residual: "NONE" (default), "HUBER", "CAUCHY" or "GEMAN_MCCLURE" (or the
+        ROBUST_* value); scale = delta in Mahalanobis units (ignored for NONE).  Kept across set_*_cloud and swap."""
+        if isinstance(kind, str):
+            kind = ROBUST_KERNEL[kind]
+        self._check(self._lib.vgicp_set_robust_kernel(self._h, int(kind), float(scale)))
 
     def set_neighbor_search_method(self, method, radius=-1.0):
         if isinstance(method, str):

@@ -9,6 +9,9 @@
 
 namespace fast_gicp {
 
+// Robust kernel of the Mahalanobis residual (an extension, not in the reference): VGICP_ROBUST_* of include/vgicp_b200.h
+enum class RobustKernel { NONE, HUBER, CAUCHY, GEMAN_MCCLURE };
+
 template <typename PointSource, typename PointTarget>
 class FastVGICPCuda : public LsqRegistration<PointSource, PointTarget> {
 public:
@@ -52,6 +55,8 @@ public:
     check(vgicp_set_neighbor_search_method(vgicp_cuda_, static_cast<int>(method), radius));
   }
   void setNearestNeighborSearchMethod(NearestNeighborMethod method) { neighbor_search_method_ = method; }
+  // scale = delta in Mahalanobis units (ignored for NONE); a setting of the core, kept across input changes and swaps
+  void setRobustKernel(RobustKernel kind, double scale = 1.0) { check(vgicp_set_robust_kernel(vgicp_cuda_, static_cast<int>(kind), scale)); }
 
   virtual void swapSourceAndTarget() override {  // impl:69-72
     check(vgicp_swap_source_and_target(vgicp_cuda_));

@@ -31,6 +31,14 @@ static fast_gicp::NeighborSearchMethod search_method(const std::string& m) {  //
   return fast_gicp::NeighborSearchMethod::DIRECT1;
 }
 
+static fast_gicp::RobustKernel robust_kernel(const std::string& k) {  // vgicp_set_robust_kernel kinds
+  if (k == "NONE") return fast_gicp::RobustKernel::NONE;
+  if (k == "HUBER") return fast_gicp::RobustKernel::HUBER;
+  if (k == "CAUCHY") return fast_gicp::RobustKernel::CAUCHY;
+  if (k == "GEMAN_MCCLURE") return fast_gicp::RobustKernel::GEMAN_MCCLURE;
+  throw std::invalid_argument("unknown robust kernel " + k + " (NONE, HUBER, CAUCHY or GEMAN_MCCLURE)");
+}
+
 static Cloud::Ptr eigen2pcl(const ArrD& points) {  // main.cpp:36-44 (double -> float)
   if (points.ndim() != 2 || points.shape(1) < 3) throw std::invalid_argument("points must be (N, 3)");
   auto cloud = pcl::make_shared<Cloud>();
@@ -218,6 +226,8 @@ PYBIND11_MODULE(pygicp, m) {
     .def("set_neighbor_search_method", [](VgicpCuda& v, const std::string& method, double radius) { v.setNeighborSearchMethod(search_method(method), radius); },
          py::arg("method") = "DIRECT1", py::arg("radius") = 1.5)
     .def("set_correspondence_randomness", &VgicpCuda::setCorrespondenceRandomness)
+    .def("set_robust_kernel", [](VgicpCuda& v, const std::string& kind, double scale) { v.setRobustKernel(robust_kernel(kind), scale); }, py::arg("kind") = "NONE",
+         py::arg("scale") = 1.0)
     .def("get_fitness_score",
          [](VgicpCuda& v, double max_range) {
            double T[16], score = 0.0;

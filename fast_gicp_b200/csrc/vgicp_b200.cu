@@ -11,9 +11,11 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <cmath>
 #include <limits>
 #include <new>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "lsq_math.hpp"
@@ -125,6 +127,8 @@ struct vgicp_context {
   double kernel_width = 0.25;
   double kernel_max_dist = 3.0;
   int offset_mode = 1;  // 1 / 7 / 27 = fixed tables, 0 = generic list
+  int robust_kind = 0;        // VGICP_ROBUST_* (vgicp_set_robust_kernel)
+  double robust_scale = 1.0;  // delta, Mahalanobis units
   int voxel_index_mode = 0;  // 0: direct-mapped index when the map's bounding box fits (else the hash table), 1: hash table only
   std::vector<int4> h_offsets;
   DevBuf<int4> d_offsets;
@@ -638,6 +642,8 @@ LinLaunch make_lin_launch(vgicp_handle h) {
   LinLaunch L;
   LinArgs& a = L.a;
   a.ndt = h->problem != 0 ? 1 : 0;
+  a.robust = h->problem == 0 ? h->robust_kind : 0;  // (the NDT entry points refuse a robust kind before they get here)
+  a.robust_d2 = a.robust ? (float)(h->robust_scale * h->robust_scale) : 0.0f;
   if (h->problem != 0) {  // NDT: target map = ndt_t; source = points + zero covariances (P2D) or source voxel Gaussians (D2D)
     a.pts = h->problem == 2 ? h->ndt_src_pts.p : s.pts.p;
     a.covA = h->ndt_src_covA.p; a.covB = h->ndt_src_covB.p; a.n = h->ndt_src_n;
@@ -698,11 +704,12 @@ int launch_linearize(vgicp_handle h, const Pose& Teval, int kind) {
     a.done_seq = ++h->eval_seq;
   }
   const int grid = L.grid, G = L.G;
-#define LAUNCH_LIN_G(MODE, GG)                                                           \
-  do {                                                                                   \
-    if (spec) k_linearize_spec<MODE, GG><<<grid, kLinThreads, 0, h->stream>>>(a);        \
-    else if (want_H) k_linearize<MODE, true, GG><<<grid, kLinThreads, 0, h->stream>>>(a); \
-    else k_linearize<MODE, false, GG><<<grid, kLinThreads, 0, h->stream>>>(a);           \
+  // rb: std::bool_constant of the robust-kernel instantiations (a.robust != 0)
+#define LAUNCH_LIN_G(MODE, GG)                                                                       \
+  do {                                                                                               \
+    if (spec) k_linearize_spec<MODE, GG, RB><<<grid, kLinThreads, 0, h->stream>>>(a);                \
+    else if (want_H) k_linearize<MODE, true, GG, RB><<<grid, kLinThreads, 0, h->stream>>>(a);        \
+    else k_linearize<MODE, false, GG, RB><<<grid, kLinThreads, 0, h->stream>>>(a);                   \
   } while (0)
 #define LAUNCH_LIN(MODE)                 \
   do {                                   \
@@ -712,26 +719,38 @@ int launch_linearize(vgicp_handle h, const Pose& Teval, int kind) {
   } while (0)
   prof_begin(h, want_H ? VGICP_PROF_LINEARIZE : VGICP_PROF_ERROR, h->stream);
   const int sgrid = stream_kernel_grid(h, a);
-  if (sgrid > 0) {
-    const size_t smem = sizeof(LinStreamSmem);
-    if (spec) k_linearize_stream<2><<<sgrid, kLinThreads, smem, h->stream>>>(a);
-    else if (want_H) k_linearize_stream<1><<<sgrid, kLinThreads, smem, h->stream>>>(a);
-    else k_linearize_stream<0><<<sgrid, kLinThreads, smem, h->stream>>>(a);
-  } else
-  switch (h->offset_mode) {
-    case 1: LAUNCH_LIN_G(1, 1); break;
-    case 7: LAUNCH_LIN(7); break;
-    case 27:
-      if (G == 3) LAUNCH_LIN_G(27, 3);
-      else LAUNCH_LIN_G(27, 1);
-      break;
-    default: LAUNCH_LIN(0); break;
-  }
+  auto launch = [&](auto rb) {
+    constexpr bool RB = decltype(rb)::value;
+    if (sgrid > 0) {
+      const size_t smem = sizeof(LinStreamSmem);
+      if (spec) k_linearize_stream<2, RB><<<sgrid, kLinThreads, smem, h->stream>>>(a);
+      else if (want_H) k_linearize_stream<1, RB><<<sgrid, kLinThreads, smem, h->stream>>>(a);
+      else k_linearize_stream<0, RB><<<sgrid, kLinThreads, smem, h->stream>>>(a);
+    } else
+    switch (h->offset_mode) {
+      case 1: LAUNCH_LIN_G(1, 1); break;
+      case 7: LAUNCH_LIN(7); break;
+      case 27:
+        if (G == 3) LAUNCH_LIN_G(27, 3);
+        else LAUNCH_LIN_G(27, 1);
+        break;
+      default: LAUNCH_LIN(0); break;
+    }
+  };
+  if (a.robust) launch(std::true_type{});
+  else launch(std::false_type{});
 #undef LAUNCH_LIN_G
 #undef LAUNCH_LIN
   prof_end(h, h->stream);
   h->launches++;
   CU_TRY(h, cudaGetLastError());
+  return VGICP_OK;
+}
+
+// a robust kind is defined for the VGICP problem only: NDT carries its own Cauchy weight
+int check_robust_problem(vgicp_handle h, const char* who) {
+  if (h->problem != 0 && h->robust_kind != VGICP_ROBUST_NONE)
+    return fail(h, VGICP_ERR_UNSUPPORTED, std::string(who) + ": a robust kernel is set (vgicp_set_robust_kernel) and an NDT problem is selected; NDT has its own weight");
   return VGICP_OK;
 }
 
@@ -892,11 +911,11 @@ int launch_multi(vgicp_handle h, const LinLaunch& L, int n_hyp, int kind, bool c
   const dim3 grid(sgrid > 0 ? sgrid : L.grid, n);
 #define LAUNCH_MULTI_G(MODE, GG)                                                                                           \
   do {                                                                                                                     \
-    if (kind == kEvalSpec) k_linearize_spec_multi<MODE, GG><<<grid, kLinThreads, 0, h->stream>>>(a, m);                  \
-    else if (kind == kEvalLinearize && count) k_linearize_multi<MODE, true, GG, true><<<grid, kLinThreads, 0, h->stream>>>(a, m); \
-    else if (kind == kEvalLinearize) k_linearize_multi<MODE, true, GG, false><<<grid, kLinThreads, 0, h->stream>>>(a, m); \
-    else if (count) k_linearize_multi<MODE, false, GG, true><<<grid, kLinThreads, 0, h->stream>>>(a, m);                  \
-    else k_linearize_multi<MODE, false, GG, false><<<grid, kLinThreads, 0, h->stream>>>(a, m);                           \
+    if (kind == kEvalSpec) k_linearize_spec_multi<MODE, GG, RB><<<grid, kLinThreads, 0, h->stream>>>(a, m);              \
+    else if (kind == kEvalLinearize && count) k_linearize_multi<MODE, true, GG, true, RB><<<grid, kLinThreads, 0, h->stream>>>(a, m); \
+    else if (kind == kEvalLinearize) k_linearize_multi<MODE, true, GG, false, RB><<<grid, kLinThreads, 0, h->stream>>>(a, m); \
+    else if (count) k_linearize_multi<MODE, false, GG, true, RB><<<grid, kLinThreads, 0, h->stream>>>(a, m);              \
+    else k_linearize_multi<MODE, false, GG, false, RB><<<grid, kLinThreads, 0, h->stream>>>(a, m);                       \
   } while (0)
 #define LAUNCH_MULTI(MODE)                    \
   do {                                        \
@@ -905,23 +924,28 @@ int launch_multi(vgicp_handle h, const LinLaunch& L, int n_hyp, int kind, bool c
     else LAUNCH_MULTI_G(MODE, 1);             \
   } while (0)
   prof_begin(h, kind == kEvalError ? VGICP_PROF_ERROR : VGICP_PROF_LINEARIZE, h->stream);
-  if (sgrid > 0) {
-    const size_t smem = sizeof(LinStreamSmem);
-    if (kind == kEvalSpec) k_linearize_stream_multi<2, false><<<grid, kLinThreads, smem, h->stream>>>(a, m);
-    else if (kind == kEvalLinearize && count) k_linearize_stream_multi<1, true><<<grid, kLinThreads, smem, h->stream>>>(a, m);
-    else if (kind == kEvalLinearize) k_linearize_stream_multi<1, false><<<grid, kLinThreads, smem, h->stream>>>(a, m);
-    else if (count) k_linearize_stream_multi<0, true><<<grid, kLinThreads, smem, h->stream>>>(a, m);
-    else k_linearize_stream_multi<0, false><<<grid, kLinThreads, smem, h->stream>>>(a, m);
-  } else
-  switch (h->offset_mode) {
-    case 1: LAUNCH_MULTI_G(1, 1); break;
-    case 7: LAUNCH_MULTI(7); break;
-    case 27:
-      if (G == 3) LAUNCH_MULTI_G(27, 3);
-      else LAUNCH_MULTI_G(27, 1);
-      break;
-    default: LAUNCH_MULTI(0); break;
-  }
+  auto launch = [&](auto rb) {  // rb: std::bool_constant of the robust-kernel instantiations
+    constexpr bool RB = decltype(rb)::value;
+    if (sgrid > 0) {
+      const size_t smem = sizeof(LinStreamSmem);
+      if (kind == kEvalSpec) k_linearize_stream_multi<2, false, RB><<<grid, kLinThreads, smem, h->stream>>>(a, m);
+      else if (kind == kEvalLinearize && count) k_linearize_stream_multi<1, true, RB><<<grid, kLinThreads, smem, h->stream>>>(a, m);
+      else if (kind == kEvalLinearize) k_linearize_stream_multi<1, false, RB><<<grid, kLinThreads, smem, h->stream>>>(a, m);
+      else if (count) k_linearize_stream_multi<0, true, RB><<<grid, kLinThreads, smem, h->stream>>>(a, m);
+      else k_linearize_stream_multi<0, false, RB><<<grid, kLinThreads, smem, h->stream>>>(a, m);
+    } else
+    switch (h->offset_mode) {
+      case 1: LAUNCH_MULTI_G(1, 1); break;
+      case 7: LAUNCH_MULTI(7); break;
+      case 27:
+        if (G == 3) LAUNCH_MULTI_G(27, 3);
+        else LAUNCH_MULTI_G(27, 1);
+        break;
+      default: LAUNCH_MULTI(0); break;
+    }
+  };
+  if (a.robust) launch(std::true_type{});
+  else launch(std::false_type{});
 #undef LAUNCH_MULTI_G
 #undef LAUNCH_MULTI
   prof_end(h, h->stream);
@@ -1083,7 +1107,7 @@ int vgicp_create(int device, vgicp_handle* out) {
   DeviceGuard g(device);
   // the kernel image is sm_90a only: fail loudly on anything else instead of falling back
   cudaFuncAttributes fa;
-  if (cudaFuncGetAttributes(&fa, k_linearize<1, true, 1>) != cudaSuccess) {
+  if (cudaFuncGetAttributes(&fa, k_linearize<1, true, 1, false>) != cudaSuccess) {
     cudaGetLastError();
     delete h;
     return VGICP_ERR_NO_DEVICE;
@@ -1169,6 +1193,18 @@ int vgicp_set_resolution(vgicp_handle h, double resolution) {
   CHECK_HANDLE(h);
   if (!(resolution > 0.0)) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "set_resolution: resolution must be positive");
   h->resolution = resolution;
+  return VGICP_OK;
+}
+
+static_assert((int)kRobustNone == (int)VGICP_ROBUST_NONE && (int)kRobustHuber == (int)VGICP_ROBUST_HUBER && (int)kRobustCauchy == (int)VGICP_ROBUST_CAUCHY &&
+                  (int)kRobustGemanMcClure == (int)VGICP_ROBUST_GEMAN_MCCLURE,
+              "the kernels' robust kinds are the C ABI's");
+int vgicp_set_robust_kernel(vgicp_handle h, int kind, double scale) {
+  CHECK_HANDLE(h);
+  if (kind < VGICP_ROBUST_NONE || kind > VGICP_ROBUST_GEMAN_MCCLURE) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "set_robust_kernel: unknown kind");
+  if (kind != VGICP_ROBUST_NONE && !(std::isfinite(scale) && scale > 0.0)) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "set_robust_kernel: scale must be finite and positive");
+  h->robust_kind = kind;
+  h->robust_scale = kind != VGICP_ROBUST_NONE ? scale : 1.0;
   return VGICP_OK;
 }
 
@@ -1489,7 +1525,9 @@ int vgicp_compute_error(vgicp_handle h, const double T[16], double* H36, double*
   CHECK_HANDLE(h);
   DeviceGuard g(h->device);
   if (!T) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "compute_error: null pose");
-  int rc = check_ready_for_eval(h, "compute_error");
+  int rc = check_robust_problem(h, "compute_error");
+  if (rc) return rc;
+  rc = check_ready_for_eval(h, "compute_error");
   if (rc) return rc;
   if ((rc = sync_inputs(h))) return rc;
   const bool want_H = (H36 != nullptr && b6 != nullptr);  // compute_derivatives.cu:160
@@ -1520,6 +1558,7 @@ int vgicp_align(vgicp_handle h, const double guess[16], const vgicp_lsq_params* 
   CHECK_HANDLE(h);
   DeviceGuard g(h->device);
   if (!guess || !res) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "align: null argument");
+  { int rc = check_robust_problem(h, "align"); if (rc) return rc; }
   vgicp_lsq_params P;
   if (params) P = *params; else vgicp_lsq_default_params(&P);
   if (h->problem == 0) {
@@ -1554,7 +1593,9 @@ int vgicp_align_multi(vgicp_handle h, const double* guesses, int n_guesses, cons
   CHECK_HANDLE(h);
   DeviceGuard g(h->device);
   if (!guesses || !results || n_guesses < 1 || n_guesses > kMultiMaxHyp) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "align_multi: null argument or n_guesses outside [1, 4096]");
-  int rc = check_ready_for_multi(h, "align_multi");
+  int rc = check_robust_problem(h, "align_multi");
+  if (rc) return rc;
+  rc = check_ready_for_multi(h, "align_multi");
   if (rc) return rc;
   if ((rc = sync_inputs(h))) return rc;
   vgicp_lsq_params P;
@@ -1600,7 +1641,9 @@ int vgicp_evaluate_poses(vgicp_handle h, const double* T, int n_poses, double* e
   DeviceGuard g(h->device);
   if (!T || !err || n_poses < 1 || n_poses > kMultiMaxHyp || (H36 == nullptr) != (b6 == nullptr))
     return fail(h, VGICP_ERR_INVALID_ARGUMENT, "evaluate_poses: null argument, H36 without b6 (or b6 without H36), or n_poses outside [1, 4096]");
-  int rc = check_ready_for_multi(h, "evaluate_poses");
+  int rc = check_robust_problem(h, "evaluate_poses");
+  if (rc) return rc;
+  rc = check_ready_for_multi(h, "evaluate_poses");
   if (rc) return rc;
   if ((rc = sync_inputs(h))) return rc;
   const int B = n_poses;

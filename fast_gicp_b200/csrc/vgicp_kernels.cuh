@@ -443,6 +443,10 @@ struct LinArgs {
   int comm_rank;
   unsigned long long comm_seq;   // evaluation number (same on every rank), selects the mailbox half
   CommMailbox* comm_peers[kCommMaxRanks];  // peers' mailboxes (index = rank; own mailbox included)
+  // VGICP only: robust kernel of the Mahalanobis residual (kRobust*, 0 = none; robust_rho) and its scale squared, delta^2.
+  // (Last, so that the parameter offsets of every other field are unchanged.)
+  int robust;
+  float robust_d2;
 };
 
 __device__ __forceinline__ int lookup_voxel(const int4* __restrict__ buckets, unsigned mask, int max_scan, uint64_t h, int cx, int cy, int cz) {
@@ -463,11 +467,76 @@ struct PointAcc {
   float err;
 };
 
+// ---------------------------------------------------------------------------------------------------------------
+// Robust kernels (an extension, not in the reference).  Per correspondence, with s = e^T M e and w = sqrt(n):
+//   err += w rho(s),   H += w rho'(s) J^T M J,   b += w rho'(s) J^T M e        (IRLS: the rho'' term is dropped)
+//   HUBER          rho = s (s <= d2), 2 sqrt(d2 s) - d2 (else)       rho' = 1, sqrt(d2 / s)
+//   CAUCHY         rho = d2 ln(1 + s / d2)                           rho' = d2 / (d2 + s)
+//   GEMAN_MCCLURE  rho = s d2 / (d2 + s)                             rho' = (d2 / (d2 + s))^2
+// d2 = delta^2 in Mahalanobis units.  Every operation is spelled as an IEEE single operation, so that the CPU checker (compiled
+// without contraction) forms the same rho and rho' from the same s; the logarithm is log1p_det below, evaluated identically there.
+// ---------------------------------------------------------------------------------------------------------------
+enum { kRobustNone = 0, kRobustHuber = 1, kRobustCauchy = 2, kRobustGemanMcClure = 3 };
+
+// ln(u), u > 0 finite, from IEEE single operations: u = m 2^k with m in [sqrt(1/2), sqrt(2)), ln m = 2 atanh(f), f = (m-1)/(m+1),
+// by its odd series to f^9 (|f| <= 0.172: truncation below 2^-25 relative); ln 2 split in Cephes' hi / lo parts (k ln2_hi exact)
+__device__ __forceinline__ float log_det(float u) {
+  if (!(u > 0.0f)) return __int_as_float(0x7fc00000);
+  if (!(u < __int_as_float(0x7f800000))) return u;
+  const int bits = __float_as_int(u);
+  int k = ((bits >> 23) & 0xff) - 127;
+  float m = __int_as_float((bits & 0x007fffff) | 0x3f800000);
+  if (m > 1.41421356f) {
+    m = __fmul_rn(m, 0.5f);
+    k += 1;
+  }
+  const float f = __fdiv_rn(__fsub_rn(m, 1.0f), __fadd_rn(m, 1.0f));
+  const float f2 = __fmul_rn(f, f);
+  float p = __fmaf_rn(f2, 0.111111111f, 0.142857143f);
+  p = __fmaf_rn(f2, p, 0.2f);
+  p = __fmaf_rn(f2, p, 0.333333333f);
+  const float two_f = __fadd_rn(f, f);
+  const float ln_m = __fmaf_rn(__fmul_rn(two_f, f2), p, two_f);
+  const float kf = (float)k;
+  return __fadd_rn(__fmul_rn(kf, 0.693359375f), __fmaf_rn(kf, -2.12194440e-4f, ln_m));
+}
+// ln(1 + x), x > -1: Goldberg's form ln(u) * x / (u - 1) with u = 1 + x, exact to a few ulp also where 1 + x rounds
+__device__ __forceinline__ float log1p_det(float x) {
+  const float u = __fadd_rn(1.0f, x);
+  if (u == 1.0f) return x;
+  return __fmul_rn(log_det(u), __fdiv_rn(x, __fsub_rn(u, 1.0f)));
+}
+// rho(s) and rho'(s) of a robust kind (not kRobustNone)
+__device__ __forceinline__ void robust_rho(int kind, float d2, float s, float& rho, float& drho) {
+  if (kind == kRobustHuber) {
+    if (s <= d2) {
+      rho = s;
+      drho = 1.0f;
+    } else {
+      const float r = __fsqrt_rn(__fmul_rn(d2, s));
+      rho = __fsub_rn(__fadd_rn(r, r), d2);
+      drho = __fsqrt_rn(__fdiv_rn(d2, s));
+    }
+    return;
+  }
+  const float q = __fdiv_rn(d2, __fadd_rn(d2, s));
+  if (kind == kRobustCauchy) {
+    rho = __fmul_rn(d2, log1p_det(__fdiv_rn(s, d2)));
+    drho = q;
+  } else {  // kRobustGemanMcClure
+    rho = __fmul_rn(q, s);
+    drho = __fmul_rn(q, q);
+  }
+}
+
 // one correspondence: S = C_B + R C_A R^T (symmetric), M = S^-1 by cofactors (Eigen Matrix3f::inverse), w = sqrt(n);
 // `hit` = false contributes exactly zero (the voxel record read for a miss is voxel 0, only there to keep the load
-// unconditional so that all loads of a lane can be in flight together).
-template <bool WANT_H>
-__device__ __forceinline__ void accumulate_voxel(float4 mn, float4 c0, float4 c1, bool hit, const float* rcr, float3 pe, PointAcc<WANT_H>& acc, int ndt, float res) {
+// unconditional so that all loads of a lane can be in flight together).  RB (VGICP only): err gets w rho(s), H and b w rho'(s) for
+// the robust kind `robust` (robust_rho).  The plain sum is its own instantiation (RB = false) rather than a runtime branch: the branch
+// changed the register allocation of the default kernels.
+template <bool WANT_H, bool RB>
+__device__ __forceinline__ void accumulate_voxel(float4 mn, float4 c0, float4 c1, bool hit, const float* rcr, float3 pe, PointAcc<WANT_H>& acc, int ndt, float res, int robust,
+                                                 float robust_d2) {
   int np = __float_as_int(mn.w);
   if (ndt ? (np <= 6) : (WANT_H && np <= 0)) hit = false;  // ndt_compute_derivatives.cu:61,132 / compute_derivatives.cu:62-64
   float a = c0.x + rcr[0], b = c0.y + rcr[1], c = c0.z + rcr[2], d = c0.w + rcr[3], e = c1.x + rcr[4], f = c1.y + rcr[5];
@@ -490,10 +559,17 @@ __device__ __forceinline__ void accumulate_voxel(float4 mn, float4 c0, float4 c1
   float mey = (m01 * ex + m11 * ey) + m12 * ez;
   float mez = (m02 * ex + m12 * ey) + m22 * ez;
   if (hit) {
-    acc.err += w * ((ex * mex + ey * mey) + ez * mez);
+    const float s = (ex * mex + ey * mey) + ez * mez;
+    float rho = s, wd = w;  // rho(s) and w rho'(s)
+    if (RB) {
+      float drho;
+      robust_rho(robust, robust_d2, s, rho, drho);
+      wd = __fmul_rn(w, drho);
+    }
+    acc.err += w * rho;
     if (WANT_H) {
-      acc.m[0] += w * m00; acc.m[1] += w * m01; acc.m[2] += w * m02; acc.m[3] += w * m11; acc.m[4] += w * m12; acc.m[5] += w * m22;
-      acc.v[0] += w * mex; acc.v[1] += w * mey; acc.v[2] += w * mez;
+      acc.m[0] += wd * m00; acc.m[1] += wd * m01; acc.m[2] += wd * m02; acc.m[3] += wd * m11; acc.m[4] += wd * m12; acc.m[5] += wd * m22;
+      acc.v[0] += wd * mex; acc.v[1] += wd * mey; acc.v[2] += wd * mez;
     }
   }
 }
@@ -552,7 +628,7 @@ struct LinWarpStage {
 };
 
 // one correspondence from the queue: entry = slot << 27 | voxel id
-template <bool WANT_H>
+template <bool WANT_H, bool RB>
 __device__ __forceinline__ void lin_process_hit(const LinArgs& a, const LinWarpStage& st, int entry, float* sum) {
   const int slot = (int)((unsigned)entry >> 27), id = entry & 0x7ffffff;
   const float4* vr = reinterpret_cast<const float4*>(a.vox + id);
@@ -566,7 +642,7 @@ __device__ __forceinline__ void lin_process_hit(const LinArgs& a, const LinWarpS
   for (int q = 0; q < 6; q++) acc.m[q] = 0.f;
   acc.v[0] = acc.v[1] = acc.v[2] = 0.f;
   acc.err = 0.f;
-  accumulate_voxel<WANT_H>(mn, c0, c1, true, rcr, pe, acc, a.ndt, a.res);
+  accumulate_voxel<WANT_H, RB>(mn, c0, c1, true, rcr, pe, acc, a.ndt, a.res, a.robust, a.robust_d2);
   apply_jacobian<WANT_H>(pe, acc, sum);
 }
 
@@ -585,8 +661,9 @@ __device__ __forceinline__ LinWarpStage& lin_stage() {
   return stage[threadIdx.x >> 5];
 }
 
-// COUNT: sum[NV] also counts the (source point, voxel) hits under Tl -- the length of the reference's correspondence list
-template <int MODE, bool WANT_H, int G, bool DENSE, bool COUNT = false>
+// COUNT: sum[NV] also counts the (source point, voxel) hits under Tl -- the length of the reference's correspondence list;
+// RB: robust kernel (accumulate_voxel)
+template <int MODE, bool WANT_H, int G, bool DENSE, bool COUNT, bool RB>
 __device__ __forceinline__ void lin_accumulate_impl(const LinArgs& a, const Pose& Tl, const Pose& Te, float* sum) {
   constexpr int NV = WANT_H ? kLinValues : 1;
   constexpr int NOFF = MODE == 0 ? 0 : MODE;
@@ -707,20 +784,20 @@ __device__ __forceinline__ void lin_accumulate_impl(const LinArgs& a, const Pose
       }
       __syncwarp();
       while (tail - head >= 32u) {  // full batches: one correspondence per lane
-        lin_process_hit<WANT_H>(a, st, st.queue[(head + lane) & (kLinQueue - 1)], sum);
+        lin_process_hit<WANT_H, RB>(a, st, st.queue[(head + lane) & (kLinQueue - 1)], sum);
         head += 32u;
       }
     }
     if (tail != head) {  // the set's last, partial batch
-      if (lane < (int)(tail - head)) lin_process_hit<WANT_H>(a, st, st.queue[(head + lane) & (kLinQueue - 1)], sum);
+      if (lane < (int)(tail - head)) lin_process_hit<WANT_H, RB>(a, st, st.queue[(head + lane) & (kLinQueue - 1)], sum);
     }
   }
 }
 
-template <int MODE, bool WANT_H, int G, bool COUNT = false>
+template <int MODE, bool WANT_H, int G, bool COUNT, bool RB>
 __device__ __forceinline__ void lin_accumulate(const LinArgs& a, const Pose& Tl, const Pose& Te, float* sum) {
-  if (a.dense.cells) lin_accumulate_impl<MODE, WANT_H, G, true, COUNT>(a, Tl, Te, sum);  // (grid-uniform branch)
-  else lin_accumulate_impl<MODE, WANT_H, G, false, COUNT>(a, Tl, Te, sum);
+  if (a.dense.cells) lin_accumulate_impl<MODE, WANT_H, G, true, COUNT, RB>(a, Tl, Te, sum);  // (grid-uniform branch)
+  else lin_accumulate_impl<MODE, WANT_H, G, false, COUNT, RB>(a, Tl, Te, sum);
 }
 
 // block reduction (warp shuffles in float -> shared in double -> per-block partial), ticket, fixed-order fold by the last
@@ -849,12 +926,12 @@ __device__ __forceinline__ void lin_unpack(const double* s, double* out) {
 // One evaluation (update_correspondences + compute_error fused).  MODE: 0 = offsets from memory (DIRECT_RADIUS or anything),
 // 1 / 7 / 27 = the reference's fixed tables; G = lanes per source point in the lookup phase (see lin_accumulate_impl): at 17k points
 // a one-thread-per-point mapping would leave one warp per scheduler with 27 serial dependent lookups per thread.
-template <int MODE, bool WANT_H, int G>
+template <int MODE, bool WANT_H, int G, bool RB>
 __global__ void __launch_bounds__(kLinThreads) k_linearize(const LinArgs a) {
   constexpr int NV = WANT_H ? kLinValues : 1;
   __shared__ double fin[4][kLinStride];
   float sum[NV];
-  lin_accumulate<MODE, WANT_H, G>(a, a.Tlin, a.Teval, sum);
+  lin_accumulate<MODE, WANT_H, G, false, RB>(a, a.Tlin, a.Teval, sum);
   if (!lin_reduce<NV>(a, sum, fin)) return;
   if (threadIdx.x == 0) {
     lin_unpack<WANT_H>(fin[0], a.out);
@@ -872,26 +949,26 @@ __global__ void __launch_bounds__(kLinThreads) k_linearize(const LinArgs a) {
 // Tlin = Teval = xi).  Both are the sums the two separate launches would produce, bit for bit (same grid, same per-lane order);
 // an accepted step saves a launch and a host round trip, a rejected one discards the second half.
 //   out[0..42] = err, H, b at xi (linearised at xi);  out[43] = err at xi over the old correspondences
-template <int MODE, int G>
+template <int MODE, int G, bool RB>
 __device__ __forceinline__ void lin_spec_accumulate(const LinArgs& a, const Pose& Tl, const Pose& Te, float* sum) {  // sum[kLinValues + 1]
   {
     float e_old[1];
-    lin_accumulate<MODE, false, G>(a, Tl, Te, e_old);
+    lin_accumulate<MODE, false, G, false, RB>(a, Tl, Te, e_old);
     sum[kLinValues] = e_old[0];
   }
   {
     float lin[kLinValues];
-    lin_accumulate<MODE, true, G>(a, Te, Te, lin);
+    lin_accumulate<MODE, true, G, false, RB>(a, Te, Te, lin);
 #pragma unroll
     for (int i = 0; i < kLinValues; i++) sum[i] = lin[i];
   }
 }
-template <int MODE, int G>
+template <int MODE, int G, bool RB>
 __global__ void __launch_bounds__(kLinThreads) k_linearize_spec(const LinArgs a) {
   constexpr int NV = kLinValues + 1;
   __shared__ double fin[4][kLinStride];
   float sum[NV];
-  lin_spec_accumulate<MODE, G>(a, a.Tlin, a.Teval, sum);
+  lin_spec_accumulate<MODE, G, RB>(a, a.Tlin, a.Teval, sum);
   if (!lin_reduce<NV>(a, sum, fin)) return;
   if (threadIdx.x == 0) {
     lin_unpack<true>(fin[0], a.out);
@@ -948,7 +1025,7 @@ struct LinStreamSmem {
 
 // one point against the voxel of its cell under the linearisation pose Tl, residual at the evaluation pose Te
 // (COUNT: the slot after the sums counts the hits, as in lin_accumulate_impl)
-template <bool WANT_H, bool COUNT = false>
+template <bool WANT_H, bool COUNT, bool RB>
 __device__ __forceinline__ void lin_stream_point(const LinArgs& a, const Pose& Tl, const Pose& Te, float4 p, float4 ca, float2 cb, float* sum) {
   const float3 pl = transform_point(Tl, p.x, p.y, p.z);
   const int off = dense_offset(a.dense, voxel_coord1(pl.x, a.res), voxel_coord1(pl.y, a.res), voxel_coord1(pl.z, a.res));
@@ -977,12 +1054,12 @@ __device__ __forceinline__ void lin_stream_point(const LinArgs& a, const Pose& T
   for (int q = 0; q < 6; q++) acc.m[q] = 0.f;
   acc.v[0] = acc.v[1] = acc.v[2] = 0.f;
   acc.err = 0.f;
-  accumulate_voxel<WANT_H>(mn, c0, c1, true, rcr, pe, acc, a.ndt, a.res);
+  accumulate_voxel<WANT_H, RB>(mn, c0, c1, true, rcr, pe, acc, a.ndt, a.res, a.robust, a.robust_d2);
   apply_jacobian<WANT_H>(pe, acc, sum);
 }
 
 // WHAT: 0 = error only, 1 = linearisation (H, b, err), 2 = speculative (both).  COUNT (WHAT 0 / 1): one more slot counts the hits.
-template <int WHAT, bool COUNT = false>
+template <int WHAT, bool COUNT, bool RB>
 __device__ __forceinline__ void lin_stream_accumulate(const LinArgs& a, const Pose& Tl, const Pose& Te, float* sum) {
   constexpr int NV = (WHAT == 0 ? 1 : (WHAT == 1 ? kLinValues : kLinValues + 1)) + (COUNT ? 1 : 0);
   static_assert(!COUNT || WHAT != 2, "the speculative evaluation does not count hits");
@@ -1026,25 +1103,25 @@ __device__ __forceinline__ void lin_stream_accumulate(const LinArgs& a, const Po
         const float4 p = sm.pts[s][j], ca = sm.covA[s][j];
         const float2 cb = sm.covB[s][j];
         if (WHAT == 0) {
-          lin_stream_point<false, COUNT>(a, Tl, Te, p, ca, cb, sum);
+          lin_stream_point<false, COUNT, RB>(a, Tl, Te, p, ca, cb, sum);
         } else if (WHAT == 1) {
-          lin_stream_point<true, COUNT>(a, Tl, Te, p, ca, cb, sum);
+          lin_stream_point<true, COUNT, RB>(a, Tl, Te, p, ca, cb, sum);
         } else {
-          lin_stream_point<false>(a, Tl, Te, p, ca, cb, sum + kLinValues);
-          lin_stream_point<true>(a, Te, Te, p, ca, cb, sum);
+          lin_stream_point<false, false, RB>(a, Tl, Te, p, ca, cb, sum + kLinValues);
+          lin_stream_point<true, false, RB>(a, Te, Te, p, ca, cb, sum);
         }
       }
     }
     __syncthreads();  // the stage may be overwritten by the copy issued in the next iteration
   }
 }
-template <int WHAT>
+template <int WHAT, bool RB>
 __global__ void __launch_bounds__(kLinThreads) k_linearize_stream(const LinArgs a) {
   constexpr int NV = WHAT == 0 ? 1 : (WHAT == 1 ? kLinValues : kLinValues + 1);
   __shared__ double fin[4][kLinStride];
   const int tid = threadIdx.x;
   float sum[NV];
-  lin_stream_accumulate<WHAT>(a, a.Tlin, a.Teval, sum);
+  lin_stream_accumulate<WHAT, false, RB>(a, a.Tlin, a.Teval, sum);
   if (!lin_reduce<NV>(a, sum, fin)) return;
   if (tid == 0) {
     if (WHAT == 0) {
@@ -1105,14 +1182,14 @@ __device__ __forceinline__ void multi_publish(const MultiArgs& m, int y) {
   }
 }
 
-template <int MODE, bool WANT_H, int G, bool COUNT>
+template <int MODE, bool WANT_H, int G, bool COUNT, bool RB>
 __global__ void __launch_bounds__(kLinThreads, 1) k_linearize_multi(const LinArgs a, const MultiArgs m) {
   constexpr int NV = (WANT_H ? kLinValues : 1) + (COUNT ? 1 : 0);
   __shared__ double fin[4][kLinStride];
   __shared__ Pose sp[2];
   const int y = multi_row(m, sp);
   float sum[NV];
-  lin_accumulate<MODE, WANT_H, G, COUNT>(a, sp[0], sp[1], sum);
+  lin_accumulate<MODE, WANT_H, G, COUNT, RB>(a, sp[0], sp[1], sum);
   if (!multi_reduce<NV>(a, m, y, sum, fin)) return;
   if (threadIdx.x == 0) {
     double* rec = m.out + (size_t)y * kMultiOut;
@@ -1122,14 +1199,14 @@ __global__ void __launch_bounds__(kLinThreads, 1) k_linearize_multi(const LinArg
   }
 }
 
-template <int MODE, int G>
+template <int MODE, int G, bool RB>
 __global__ void __launch_bounds__(kLinThreads, 1) k_linearize_spec_multi(const LinArgs a, const MultiArgs m) {
   constexpr int NV = kLinValues + 1;
   __shared__ double fin[4][kLinStride];
   __shared__ Pose sp[2];
   const int y = multi_row(m, sp);
   float sum[NV];
-  lin_spec_accumulate<MODE, G>(a, sp[0], sp[1], sum);
+  lin_spec_accumulate<MODE, G, RB>(a, sp[0], sp[1], sum);
   if (!multi_reduce<NV>(a, m, y, sum, fin)) return;
   if (threadIdx.x == 0) {
     double* rec = m.out + (size_t)y * kMultiOut;
@@ -1139,7 +1216,7 @@ __global__ void __launch_bounds__(kLinThreads, 1) k_linearize_spec_multi(const L
   }
 }
 
-template <int WHAT, bool COUNT>
+template <int WHAT, bool COUNT, bool RB>
 __global__ void __launch_bounds__(kLinThreads, 1) k_linearize_stream_multi(const LinArgs a, const MultiArgs m) {
   constexpr int NB = WHAT == 0 ? 1 : (WHAT == 1 ? kLinValues : kLinValues + 1);
   constexpr int NV = NB + (COUNT ? 1 : 0);
@@ -1147,7 +1224,7 @@ __global__ void __launch_bounds__(kLinThreads, 1) k_linearize_stream_multi(const
   __shared__ Pose sp[2];
   const int y = multi_row(m, sp);
   float sum[NV];
-  lin_stream_accumulate<WHAT, COUNT>(a, sp[0], sp[1], sum);
+  lin_stream_accumulate<WHAT, COUNT, RB>(a, sp[0], sp[1], sum);
   if (!multi_reduce<NV>(a, m, y, sum, fin)) return;
   if (threadIdx.x == 0) {
     double* rec = m.out + (size_t)y * kMultiOut;

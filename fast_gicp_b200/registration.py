@@ -37,6 +37,13 @@ class NearestNeighborMethod(enum.IntEnum):  # fast_vgicp_cuda.hpp:21
     GPU_RBF_KERNEL = 2
 
 
+class RobustKernel(enum.IntEnum):  # vgicp_set_robust_kernel (an extension, not in the reference)
+    NONE = 0
+    HUBER = 1
+    CAUCHY = 2
+    GEMAN_MCCLURE = 3
+
+
 class LSQ_OPTIMIZER_TYPE(enum.IntEnum):  # lsq_registration.hpp:13
     GaussNewton = 0
     LevenbergMarquardt = 1
@@ -280,6 +287,13 @@ class FastVGICPCuda(LsqRegistration):
     def setNearestNeighborSearchMethod(self, method):
         self.neighbor_search_method_ = NearestNeighborMethod(method)
 
+    def setRobustKernel(self, kind, scale=1.0):
+        """Robust kernel of the Mahalanobis residual (an extension): "NONE" (default), "HUBER", "CAUCHY", "GEMAN_MCCLURE"
+        or a RobustKernel; scale = delta in Mahalanobis units.  A setting of the core, kept across input changes."""
+        if isinstance(kind, str):
+            kind = RobustKernel[kind]
+        self.vgicp_cuda_.set_robust_kernel(int(RobustKernel(kind)), scale)
+
     # pygicp names (main.cpp:194-202)
     def set_resolution(self, r):
         self.setResolution(r)
@@ -289,6 +303,9 @@ class FastVGICPCuda(LsqRegistration):
 
     def set_correspondence_randomness(self, k):
         self.setCorrespondenceRandomness(k)
+
+    def set_robust_kernel(self, kind="NONE", scale=1.0):
+        self.setRobustKernel(kind, scale)
 
     # -- state machine (:69-141)
     def swapSourceAndTarget(self):

@@ -175,6 +175,24 @@ VGICP_API int vgicp_evaluate_poses(vgicp_handle h, const double* T, int n_poses,
  * benchmark loop, src/align.cpp:72-81) with GPU k-NN covariances.  xyz are host pointers, or device pointers when on_device != 0. */
 VGICP_API int vgicp_register(vgicp_handle h, const float* target_xyz, size_t n_target, const float* source_xyz, size_t n_source, size_t stride_bytes, int on_device, int k,
                              int regularization_method, const double guess[16], const vgicp_lsq_params* params, vgicp_align_result* result);
+/* ---- robust kernels (outlier down-weighting; not in the reference) -------------------------------------------------------
+ * Per correspondence (source point i, voxel v) at the evaluation pose, with e = mu_v - T a_i, M = (C_v + R C_i R^T)^-1 as always
+ * and s = e^T M e (squared Mahalanobis residual):
+ *   err += sqrt(n_v) rho(s),   H += sqrt(n_v) rho'(s) J^T M J,   b += sqrt(n_v) rho'(s) J^T M e
+ * (iteratively reweighted least squares: the rho'' term is dropped; b is half the gradient of err at fixed correspondences).
+ *   kind            rho(s)                                          rho'(s)
+ *   NONE (default)  s                                               1
+ *   HUBER           s if s <= d^2, else 2 d sqrt(s) - d^2           1 if s <= d^2, else d / sqrt(s)
+ *   CAUCHY          d^2 ln(1 + s / d^2)                             d^2 / (d^2 + s)
+ *   GEMAN_MCCLURE   d^2 s / (d^2 + s)                               (d^2 / (d^2 + s))^2
+ * The scale d > 0 is in Mahalanobis units (dimensionless: s is a squared residual in standard deviations); the kernels use
+ * d^2 = (float)(d * d).  A handle setting like the resolution: it survives set_*_cloud and swap_source_and_target and applies to
+ * vgicp_compute_error, vgicp_align, vgicp_align_multi, vgicp_evaluate_poses and vgicp_register.  NONE reproduces the plain sums bit
+ * for bit.  Errors: VGICP_ERR_INVALID_ARGUMENT for an unknown kind or a scale that is not finite and > 0 (the scale is ignored for
+ * NONE).  NDT carries its own Cauchy weight: with an NDT problem selected and a kind other than NONE, vgicp_compute_error,
+ * vgicp_align, vgicp_align_multi and vgicp_evaluate_poses return VGICP_ERR_UNSUPPORTED without launching anything. */
+enum { VGICP_ROBUST_NONE = 0, VGICP_ROBUST_HUBER = 1, VGICP_ROBUST_CAUCHY = 2, VGICP_ROBUST_GEMAN_MCCLURE = 3 };
+VGICP_API int vgicp_set_robust_kernel(vgicp_handle h, int kind, double scale);
 /* pcl::transformPointCloud of the source by T (lsq_registration_impl.hpp:78) on the device; out: n x stride floats */
 VGICP_API int vgicp_transform_source(vgicp_handle h, const double T[16], float* out_xyz, size_t capacity_points, size_t stride_bytes);
 /* set_{source,target}_cloud with the points already resident in this GPU's memory (device pointer, same layout rules);
