@@ -45,6 +45,7 @@ EXPORTED_SYMBOLS = [
     "vgicp_comm_export", "vgicp_comm_init", "vgicp_comm_shutdown", "vgicp_comm_error", "vgicp_set_source_shard", "vgicp_clear_source_shard",
     "vgicp_comm_export_arena", "vgicp_comm_init_arena", "vgicp_set_stage1_sharding", "vgicp_set_source_covariances", "vgicp_set_target_covariances",
     "vgicp_align_multi", "vgicp_evaluate_poses", "vgicp_set_robust_kernel",
+    "vgicp_append_source_to_target", "vgicp_crop_target",
 ]
 PROF_NUM_CATEGORIES = 7
 
@@ -155,6 +156,8 @@ def load_library():
         "vgicp_set_target_covariances": [hp, fp, C.c_size_t],
         "vgicp_register": [hp, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_int, C.c_int, C.c_int, dp, C.POINTER(LsqParams), C.POINTER(AlignResult)],
         "vgicp_get_profile": [hp, dp, C.POINTER(C.c_uint64), C.c_int],
+        "vgicp_append_source_to_target": [hp, dp],
+        "vgicp_crop_target": [hp, dp, C.c_double, C.c_size_t],
     }
     for name, argtypes in sig.items():
         fn = getattr(L, name)
@@ -493,6 +496,19 @@ class Core:
         s_, ns, ss = self._cloud(source)
         assert st == ss
         return self.register_raw(t.ctypes.data, nt, s_.ctypes.data, ns, st, False, k, reg, guess, params)
+
+    # ---- local map (scan-to-map odometry)
+    def append_source_to_target(self, T):
+        """Append the current source, transformed by the 4x4 T, to the target on the device and rebuild the voxel map.
+        Appended points are transform_source(T)'s; covariances are R C R^T in the order include/vgicp_b200.h documents."""
+        t = pose_to_c(T)
+        self._check(self._lib.vgicp_append_source_to_target(self._h, _dp(t)))
+
+    def crop_target(self, center, radius, max_points=0):
+        """Keep the target points within `radius` of `center` (float32 test), then at most the newest `max_points` of them
+        (0 = no cap); rebuild the voxel map.  A crop that would leave no points raises and changes nothing."""
+        c = np.ascontiguousarray(np.asarray(center, dtype=np.float64).reshape(3))
+        self._check(self._lib.vgicp_crop_target(self._h, _dp(c), float(radius), int(max_points)))
 
     def transform_source(self, T, stride=12, out=None):
         n = self.num_source_points()

@@ -58,6 +58,20 @@ public:
   // scale = delta in Mahalanobis units (ignored for NONE); a setting of the core, kept across input changes and swaps
   void setRobustKernel(RobustKernel kind, double scale = 1.0) { check(vgicp_set_robust_kernel(vgicp_cuda_, static_cast<int>(kind), scale)); }
 
+  // Local map for scan-to-map odometry (an extension).  Afterwards the target on the device is no longer the cloud given to
+  // setInputTarget: target_ becomes a fresh empty placeholder, so align still has a target and setInputTarget(that cloud) reloads it.
+  void appendSourceToTarget(const Matrix4& T) {  // T: e.g. getFinalTransformation()
+    double Td[16];
+    for (int i = 0; i < 16; i++) Td[i] = static_cast<double>(T.v[i]);
+    checkStrict(vgicp_append_source_to_target(vgicp_cuda_, Td));
+    target_ = pcl::make_shared<PointCloudTarget>();
+  }
+  // keep the target points within `radius` of `center`, then at most the newest `max_points` of them (0 = no cap)
+  void cropTarget(const double center[3], double radius, size_t max_points = 0) {
+    checkStrict(vgicp_crop_target(vgicp_cuda_, center, radius, max_points));
+    target_ = pcl::make_shared<PointCloudTarget>();
+  }
+
   virtual void swapSourceAndTarget() override {  // impl:69-72
     check(vgicp_swap_source_and_target(vgicp_cuda_));
     input_.swap(target_);
@@ -132,6 +146,9 @@ private:
   void check(int rc) const {
     if (rc != VGICP_OK && rc != VGICP_ERR_UNSUPPORTED) throw std::runtime_error(std::string("FastVGICPCuda: ") + vgicp_last_error(vgicp_cuda_));
     if (rc == VGICP_ERR_UNSUPPORTED) std::cerr << vgicp_last_error(vgicp_cuda_) << std::endl;  // the reference prints and carries on
+  }
+  void checkStrict(int rc) const {  // the extensions have no reference behaviour to follow: every failure throws
+    if (rc != VGICP_OK) throw std::runtime_error(std::string("FastVGICPCuda: ") + vgicp_last_error(vgicp_cuda_));
   }
 
   int k_correspondences_;

@@ -228,6 +228,14 @@ PYBIND11_MODULE(pygicp, m) {
     .def("set_correspondence_randomness", &VgicpCuda::setCorrespondenceRandomness)
     .def("set_robust_kernel", [](VgicpCuda& v, const std::string& kind, double scale) { v.setRobustKernel(robust_kernel(kind), scale); }, py::arg("kind") = "NONE",
          py::arg("scale") = 1.0)
+    // local map for scan-to-map odometry (not in the reference binding)
+    .def("append_source_to_target", [](VgicpCuda& v, const ArrF& T) { v.appendSourceToTarget(to_mat4f(T)); }, py::arg("T"))
+    .def("crop_target",
+         [](VgicpCuda& v, const ArrD& center, double radius, size_t max_points) {
+           if (center.size() != 3) throw std::invalid_argument("center must have 3 elements");
+           v.cropTarget(center.data(), radius, max_points);
+         },
+         py::arg("center"), py::arg("radius"), py::arg("max_points") = 0)
     .def("get_fitness_score",
          [](VgicpCuda& v, double max_range) {
            double T[16], score = 0.0;

@@ -20,6 +20,7 @@
 
 #include "lsq_math.hpp"
 #include "vgicp_kernels.cuh"
+#include "vgicp_local_map.cuh"
 
 using namespace vgicp;
 
@@ -40,6 +41,26 @@ struct DevBuf {  // grow-only device array
     cudaError_t e = cudaMalloc(&p, want * sizeof(T));
     if (e == cudaSuccess) cap = want;
     return e;
+  }
+  // reserve that keeps the first `keep` elements: copied in stream order on `st`; the old array is freed once `st` has drained,
+  // since work enqueued there may still read it
+  cudaError_t grow(size_t n, size_t keep, cudaStream_t st) {
+    if (n <= cap) return cudaSuccess;
+    if (external) return cudaErrorMemoryAllocation;
+    const size_t want = n + n / 4 + 16;
+    T* q = nullptr;
+    cudaError_t e = cudaMalloc(&q, want * sizeof(T));
+    if (e != cudaSuccess) return e;
+    if (keep) e = cudaMemcpyAsync(q, p, keep * sizeof(T), cudaMemcpyDeviceToDevice, st);
+    if (e == cudaSuccess && p) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) {
+      cudaFree(q);
+      return e;
+    }
+    if (p) cudaFree(p);
+    p = q;
+    cap = want;
+    return cudaSuccess;
   }
   void release() {
     if (p && !external) cudaFree(p);
@@ -184,6 +205,14 @@ struct vgicp_context {
   DevBuf<float2> ndt_src_covB;
   int ndt_src_n = 0;
   bool ndt_ready = false;
+
+  // local map (vgicp_append_source_to_target / vgicp_crop_target)
+  cudaEvent_t ev_append = nullptr;  // end of the last append: the source's stream waits for it before the source is overwritten
+  DevBuf<int> crop_rank;            // per target point: rank among the points that pass the radius test, or -1
+  DevBuf<unsigned long long> crop_state;  // k_crop_rank look-back (epoch-tagged block totals)
+  unsigned crop_epoch = 0;
+  DevBuf<float4> spare_pts, spare_covA;  // the crop compacts into these and swaps them with the target's arrays
+  DevBuf<float2> spare_covB;
 
   // optional per-kernel timing (vgicp_set_profiling): CUDA events on the handle's stream around every launch
   bool prof_on = false;
@@ -1115,6 +1144,7 @@ int vgicp_create(int device, vgicp_handle* out) {
   bool ok = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) == cudaSuccess;
   ok = ok && cudaStreamCreateWithFlags(&h->stream_b, cudaStreamNonBlocking) == cudaSuccess;
   ok = ok && cudaEventCreateWithFlags(&h->ev_copy, cudaEventDisableTiming) == cudaSuccess;
+  ok = ok && cudaEventCreateWithFlags(&h->ev_append, cudaEventDisableTiming) == cudaSuccess;
   ok = ok && cudaEventCreateWithFlags(&h->target.ready, cudaEventDisableTiming) == cudaSuccess;
   ok = ok && cudaEventCreateWithFlags(&h->source.ready, cudaEventDisableTiming) == cudaSuccess;
   h->target.st = h->stream;    // the target (and its voxel map) is built on the main stream, where the evaluations run
@@ -1167,6 +1197,8 @@ int vgicp_destroy(vgicp_handle h) {
     vm->release();
   }
   h->ndt_src_pts.release(); h->ndt_src_covA.release(); h->ndt_src_covB.release();
+  h->crop_rank.release(); h->crop_state.release();
+  h->spare_pts.release(); h->spare_covA.release(); h->spare_covB.release();
   if (h->d_out) cudaFree(h->d_out);
   if (h->h_out) cudaFreeHost(h->h_out);
   if (h->h_flag) cudaFreeHost(h->h_flag);
@@ -1179,7 +1211,7 @@ int vgicp_destroy(vgicp_handle h) {
   if (h->h_multi_done) cudaFreeHost(h->h_multi_done);
   for (auto& r : h->prof_pending) { cudaEventDestroy(r.a); cudaEventDestroy(r.b); }
   for (auto e : h->prof_pool) cudaEventDestroy(e);
-  for (cudaEvent_t e : {h->ev_copy, h->target.ready, h->source.ready})
+  for (cudaEvent_t e : {h->ev_copy, h->ev_append, h->target.ready, h->source.ready})
     if (e) cudaEventDestroy(e);
   if (h->stream_b) cudaStreamDestroy(h->stream_b);
   if (h->stream) cudaStreamDestroy(h->stream);
@@ -1729,6 +1761,110 @@ int vgicp_set_target_cloud_device(vgicp_handle h, const float* d_xyz, size_t n, 
   h->map.built = false;
   h->map.pending = false;
   return set_cloud(h, h->target, d_xyz, n, stride_bytes, true);
+}
+
+// ---- local map: append the registered source to the target, crop the target ----
+static int local_map_check(vgicp_handle h, const char* who) {
+  if (h->problem != 0) return fail(h, VGICP_ERR_UNSUPPORTED, std::string(who) + ": NDT maps are built from the points alone; select the VGICP problem");
+  if (h->stage1_sharding || h->target.covA.external)
+    return fail(h, VGICP_ERR_UNSUPPORTED, std::string(who) + ": the target covariances live in the fixed-capacity exchange arena (stage-1 sharding)");
+  if (!h->target.has_pts || !h->target.has_cov) return fail(h, VGICP_ERR_BAD_STATE, std::string(who) + ": target points and covariances required");
+  return VGICP_OK;
+}
+
+// the target's arrays were replaced on its stream: leave the state set_target_cloud + set_target_covariances +
+// create_target_voxelmap would leave (covariances, no neighbour rows, the map build enqueued at the map's first resolution)
+static int local_map_rebuild(vgicp_handle h) {
+  Cloud& t = h->target;
+  t.k = 0;
+  t.knn_sorted = nullptr;
+  t.knn_q_begin = t.knn_q_end = 0;
+  t.has_cov = true;
+  h->ndt_ready = false;
+  h->ndt_t.built = false;
+  h->ndt_t.pending = false;
+  int rc = voxelmap_begin(h, t, h->map);
+  if (rc) return rc;
+  CU_TRY(h, cudaEventRecord(t.ready, t.st));
+  return VGICP_OK;
+}
+
+int vgicp_append_source_to_target(vgicp_handle h, const double T[16]) {
+  CHECK_HANDLE(h);
+  DeviceGuard g(h->device);
+  if (!T) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "append_source_to_target: null pose");
+  for (int i = 0; i < 16; i++)
+    if (!std::isfinite(T[i])) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "append_source_to_target: non-finite pose");
+  int rc = local_map_check(h, "append_source_to_target");
+  if (rc) return rc;
+  Cloud& s = h->source;
+  Cloud& t = h->target;
+  if (!s.has_pts || !s.has_cov) return fail(h, VGICP_ERR_BAD_STATE, "append_source_to_target: source points and covariances required");
+  const size_t n = (size_t)t.n + (size_t)s.n;
+  if (n > (size_t)0x7fffffff / 64) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "append_source_to_target: the merged target would exceed the points a cloud may hold");
+  if (s.st != t.st) CU_TRY(h, cudaStreamWaitEvent(t.st, s.ready, 0));
+  CU_TRY(h, t.pts.grow(n, t.n, t.st));
+  CU_TRY(h, t.covA.grow(n, t.n, t.st));
+  CU_TRY(h, t.covB.grow(n, t.n, t.st));
+  if (s.n > 0) {
+    KLAUNCH_ST(h, t.st, VGICP_PROF_OTHER,
+               k_append_transformed<<<blocks_for(s.n, 256), 256, 0, t.st>>>(s.pts.p, s.covA.p, s.covB.p, s.n, to_pose(T), t.pts.p + t.n, t.covA.p + t.n, t.covB.p + t.n));
+    CU_TRY(h, cudaGetLastError());
+    // the next upload into the source's arrays (on the source's stream) must not overtake this read of them
+    CU_TRY(h, cudaEventRecord(h->ev_append, t.st));
+    if (s.st != t.st) CU_TRY(h, cudaStreamWaitEvent(s.st, h->ev_append, 0));
+  }
+  t.n = (int)n;
+  return local_map_rebuild(h);
+}
+
+int vgicp_crop_target(vgicp_handle h, const double center[3], double radius, size_t max_points) {
+  CHECK_HANDLE(h);
+  DeviceGuard g(h->device);
+  if (!center) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "crop_target: null center");
+  if (!(radius >= 0.0)) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "crop_target: radius must be >= 0 (NaN is rejected; +inf keeps every point)");
+  int rc = local_map_check(h, "crop_target");
+  if (rc) return rc;
+  Cloud& t = h->target;
+  const int n = t.n;
+  if (n == 0) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "crop_target: the crop would leave no points");
+  const int blocks = blocks_for(n, kCropThreads);
+  CU_TRY(h, h->crop_rank.reserve(n));
+  {
+    const unsigned long long* before = h->crop_state.p;
+    CU_TRY(h, h->crop_state.reserve(blocks));
+    if (h->crop_state.p != before) {  // fresh allocation: no stale epoch may match
+      CU_TRY(h, cudaMemsetAsync(h->crop_state.p, 0, h->crop_state.cap * sizeof(unsigned long long), t.st));
+      h->crop_epoch = 0;
+    }
+    if (++h->crop_epoch == 0) {  // wrapped: clear once and restart
+      CU_TRY(h, cudaMemsetAsync(h->crop_state.p, 0, h->crop_state.cap * sizeof(unsigned long long), t.st));
+      h->crop_epoch = 1;
+    }
+  }
+  CU_TRY(h, h->spare_pts.reserve(n));
+  CU_TRY(h, h->spare_covA.reserve(n));
+  CU_TRY(h, h->spare_covB.reserve(n));
+  int* d_count = h->map.d_counters + 10;
+  KLAUNCH_ST(h, t.st, VGICP_PROF_OTHER,
+             k_crop_rank<<<blocks, kCropThreads, 0, t.st>>>(t.pts.p, n, (float)center[0], (float)center[1], (float)center[2], (float)(radius * radius), h->crop_rank.p, d_count,
+                                                            h->crop_state.p, h->crop_epoch));
+  CU_TRY(h, cudaGetLastError());
+  // the host needs the new size (and must refuse an empty result before anything is modified): one synchronisation
+  CU_TRY(h, cudaMemcpyAsync(h->map.h_counters + 10, d_count, sizeof(int), cudaMemcpyDeviceToHost, t.st));
+  CU_TRY(h, cudaStreamSynchronize(t.st));
+  const size_t passed = (size_t)h->map.h_counters[10];
+  const size_t first = (max_points > 0 && passed > max_points) ? passed - max_points : 0;
+  const int kept = (int)(passed - first);
+  if (kept == 0) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "crop_target: the crop would leave no points");
+  KLAUNCH_ST(h, t.st, VGICP_PROF_OTHER,
+             k_crop_scatter<<<blocks_for(n, 256), 256, 0, t.st>>>(t.pts.p, t.covA.p, t.covB.p, h->crop_rank.p, n, (int)first, h->spare_pts.p, h->spare_covA.p, h->spare_covB.p));
+  CU_TRY(h, cudaGetLastError());
+  std::swap(t.pts, h->spare_pts);
+  std::swap(t.covA, h->spare_covA);
+  std::swap(t.covB, h->spare_covB);
+  t.n = kept;
+  return local_map_rebuild(h);
 }
 
 // ---- multi-GPU: source sharding with an in-kernel exchange of the linear system over NVLink peer memory ----

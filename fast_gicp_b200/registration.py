@@ -250,6 +250,10 @@ class NDTCuda(LsqRegistration):
         return self.ndt_cuda_.fitness_score(self.final_transformation_.astype(np.float64), max_range)
 
 
+class _DeviceMap:
+    """Stands for a target that exists only on the device (a local map built by appends and crops)."""
+
+
 class FastVGICPCuda(LsqRegistration):
     """Fast Voxelized GICP on an H100 behind the reference's FastVGICPCuda interface."""
 
@@ -306,6 +310,24 @@ class FastVGICPCuda(LsqRegistration):
 
     def set_robust_kernel(self, kind="NONE", scale=1.0):
         self.setRobustKernel(kind, scale)
+
+    # -- local map for scan-to-map odometry (an extension).  Afterwards the target on the device is no longer the cloud given to
+    # setInputTarget: target_ becomes a fresh placeholder, so align still has a target and setInputTarget(that cloud) reloads it.
+    def appendSourceToTarget(self, T):
+        """Append the current source, transformed by T (e.g. getFinalTransformation()), to the target map on the device."""
+        self.vgicp_cuda_.append_source_to_target(np.asarray(T, dtype=np.float64))
+        self.target_ = _DeviceMap()
+
+    def cropTarget(self, center, radius, max_points=0):
+        """Keep the target points within `radius` of `center`, then at most the newest `max_points` (0 = no cap)."""
+        self.vgicp_cuda_.crop_target(center, radius, max_points)
+        self.target_ = _DeviceMap()
+
+    def append_source_to_target(self, T):
+        self.appendSourceToTarget(T)
+
+    def crop_target(self, center, radius, max_points=0):
+        self.cropTarget(center, radius, max_points)
 
     # -- state machine (:69-141)
     def swapSourceAndTarget(self):

@@ -193,6 +193,36 @@ VGICP_API int vgicp_register(vgicp_handle h, const float* target_xyz, size_t n_t
  * vgicp_align, vgicp_align_multi and vgicp_evaluate_poses return VGICP_ERR_UNSUPPORTED without launching anything. */
 enum { VGICP_ROBUST_NONE = 0, VGICP_ROBUST_HUBER = 1, VGICP_ROBUST_CAUCHY = 2, VGICP_ROBUST_GEMAN_MCCLURE = 3 };
 VGICP_API int vgicp_set_robust_kernel(vgicp_handle h, int kind, double scale);
+/* ---- local map for scan-to-map odometry (not in the reference) -------------------------------------------------------------
+ * Each frame: register the new scan against the map (vgicp_align), append it at the pose found, crop what is too far or too old.
+ * Both calls work on the device arrays in place (no PCIe traffic for the map) and leave the state that set_target_cloud +
+ * set_target_covariances + create_target_voxelmap with the resulting arrays would leave: the target has covariances, no
+ * neighbour rows (vgicp_get_target_neighbors returns VGICP_ERR_BAD_STATE; find_target_neighbors + calculate_target_covariances
+ * recompute k-NN covariances of the merged map if wanted), and the voxel map is rebuilt over the whole target at the resolution it
+ * was first created with.  Handle settings (robust kernel, neighbour search, ...) are kept.  Neither is available with an NDT
+ * problem selected or with stage-1 sharding (VGICP_ERR_UNSUPPORTED); source sharding is unaffected (every rank makes the same
+ * deterministic change).  Every error below is returned before anything is modified, and all but the empty crop before any launch.
+ *
+ * vgicp_append_source_to_target: the target grows from n_t to n_t + n_s points; rows n_t .. n_t + n_s - 1 hold the current source
+ * transformed by T (column-major 4x4, cast to float like every pose):
+ *   point i       = what vgicp_transform_source(h, T) returns for source point i, bit for bit;
+ *   covariance i  = R C_i R^T, R the float rotation of T, in IEEE single operations without contraction, in this order:
+ *                     M_ik = (R_i0 C_0k + R_i1 C_1k) + R_i2 C_2k,
+ *                     N_ij = (M_i0 R_j0 + M_i1 R_j1) + M_i2 R_j2,
+ *                   stored as set_covariances stores a 3x3: the diagonal N_ii and 0.5f * (N_ij + N_ji) off it.
+ * The source is not changed.  Grow-only, amortised storage; the existing rows are copied on the device when it grows.
+ * Errors: VGICP_ERR_INVALID_ARGUMENT (null or non-finite T, a merged target larger than a cloud may be: 2^31 / 64 points),
+ * VGICP_ERR_BAD_STATE (source or target without points or covariances). */
+VGICP_API int vgicp_append_source_to_target(vgicp_handle h, const double T[16]);
+/* vgicp_crop_target: keep the target points within `radius` of `center`, then at most the newest `max_points` of them; rebuild the map.
+ *   radius test   c = (float)center, dx = p.x - c.x (y, z alike), d^2 = (dx dx + dy dy) + dz dz in IEEE single operations;
+ *                 point p passes when d^2 <= (float)(radius * radius).  radius = +inf keeps every point.
+ *   point cap     when more than max_points points pass, only the last max_points of them in array order are kept (appends go
+ *                 to the end, so these are the newest).  max_points = 0: no cap.
+ * Kept points and their covariances stay in their original order.  One host synchronisation (the new size).
+ * Errors: VGICP_ERR_INVALID_ARGUMENT (null center, NaN or negative radius, a crop that would leave no points: target and map are
+ * then left exactly as they were), VGICP_ERR_BAD_STATE (target without points or covariances). */
+VGICP_API int vgicp_crop_target(vgicp_handle h, const double center[3], double radius, size_t max_points);
 /* pcl::transformPointCloud of the source by T (lsq_registration_impl.hpp:78) on the device; out: n x stride floats */
 VGICP_API int vgicp_transform_source(vgicp_handle h, const double T[16], float* out_xyz, size_t capacity_points, size_t stride_bytes);
 /* set_{source,target}_cloud with the points already resident in this GPU's memory (device pointer, same layout rules);

@@ -33,6 +33,16 @@ c.set_resolution(0.5); c.set_neighbor_search_method("DIRECT1")
 r = c.register(bt, bs)
 print("stream", len(bs), "converged", bool(r.converged))
 c.close()
+# local map: append the registered source (the target's arrays grow with a device copy), crop it (scan + look-back, compaction)
+c = Core(0)
+c.set_neighbor_search_method("DIRECT7")
+r = c.register(tgt, src)
+from fast_gicp_b200.core import pose_from_c
+c.append_source_to_target(pose_from_c(r.T))
+c.crop_target((0.0, 0.0, 0.0), 30.0, len(tgt))
+r = c.align(pose_from_c(r.T))
+print("local map", c.num_target_points(), "converged", bool(r.converged))
+c.close()
 # NDT D2D through the same evaluation kernels
 c = Core(0)
 c.set_problem(2); c.set_neighbor_search_method("DIRECT7")
