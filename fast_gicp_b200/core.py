@@ -45,7 +45,7 @@ EXPORTED_SYMBOLS = [
     "vgicp_comm_export", "vgicp_comm_init", "vgicp_comm_shutdown", "vgicp_comm_error", "vgicp_set_source_shard", "vgicp_clear_source_shard",
     "vgicp_comm_export_arena", "vgicp_comm_init_arena", "vgicp_set_stage1_sharding", "vgicp_set_source_covariances", "vgicp_set_target_covariances",
     "vgicp_align_multi", "vgicp_evaluate_poses", "vgicp_set_robust_kernel",
-    "vgicp_append_source_to_target", "vgicp_crop_target",
+    "vgicp_append_source_to_target", "vgicp_crop_target", "vgicp_deskew_source",
 ]
 PROF_NUM_CATEGORIES = 7
 
@@ -158,6 +158,7 @@ def load_library():
         "vgicp_get_profile": [hp, dp, C.POINTER(C.c_uint64), C.c_int],
         "vgicp_append_source_to_target": [hp, dp],
         "vgicp_crop_target": [hp, dp, C.c_double, C.c_size_t],
+        "vgicp_deskew_source": [hp, C.c_void_p, C.c_size_t, C.c_size_t, dp, C.c_double],
     }
     for name, argtypes in sig.items():
         fn = getattr(L, name)
@@ -193,6 +194,46 @@ def pose_from_c(buf):
 
 def _dp(a):
     return a.ctypes.data_as(C.POINTER(C.c_double))
+
+
+def twist_from_motion(delta, duration):
+    """Constant body twist [omega, v] (rotation first, per time unit) that moves by the 4x4 `delta` in `duration`: the float64
+    SE(3) logarithm, the inverse of se3_exp (csrc/lsq_math.hpp), divided by duration.  For a constant-velocity deskew,
+    twist_from_motion(inv(T_prev) @ T_cur, dt) with the last two estimated poses."""
+    T = np.asarray(delta, dtype=np.float64)
+    R, t = T[:3, :3], T[:3, 3]
+    # quaternion (Shepperd: divide by the largest of the four candidates), w >= 0
+    tr = R[0, 0] + R[1, 1] + R[2, 2]
+    k = int(np.argmax([tr, R[0, 0], R[1, 1], R[2, 2]]))
+    if k == 0:
+        r = np.sqrt(1.0 + tr) * 2.0
+        q = np.array([0.25 * r, (R[2, 1] - R[1, 2]) / r, (R[0, 2] - R[2, 0]) / r, (R[1, 0] - R[0, 1]) / r])
+    elif k == 1:
+        r = np.sqrt(1.0 + R[0, 0] - R[1, 1] - R[2, 2]) * 2.0
+        q = np.array([(R[2, 1] - R[1, 2]) / r, 0.25 * r, (R[0, 1] + R[1, 0]) / r, (R[0, 2] + R[2, 0]) / r])
+    elif k == 2:
+        r = np.sqrt(1.0 + R[1, 1] - R[0, 0] - R[2, 2]) * 2.0
+        q = np.array([(R[0, 2] - R[2, 0]) / r, (R[0, 1] + R[1, 0]) / r, 0.25 * r, (R[1, 2] + R[2, 1]) / r])
+    else:
+        r = np.sqrt(1.0 + R[2, 2] - R[0, 0] - R[1, 1]) * 2.0
+        q = np.array([(R[1, 0] - R[0, 1]) / r, (R[0, 2] + R[2, 0]) / r, (R[1, 2] + R[2, 1]) / r, 0.25 * r])
+    if q[0] < 0.0:
+        q = -q
+    w, vec = q[0], q[1:]
+    nv = np.linalg.norm(vec)
+    theta = 2.0 * np.arctan2(nv, w)
+    omega = vec * (theta / nv if nv > 1e-10 else 2.0 / w * (1.0 - nv * nv / (3.0 * w * w)))
+    # v solves V v = t with V built exactly as se3_exp builds it (V = R below theta = 1e-10), so that the round trip holds at
+    # every angle, the tiny ones included
+    th2 = float(omega @ omega)
+    th = np.sqrt(th2)
+    if th < 1e-10:
+        V = R
+    else:
+        Om = np.array([[0.0, -omega[2], omega[1]], [omega[2], 0.0, -omega[0]], [-omega[1], omega[0], 0.0]])
+        V = np.eye(3) + (1.0 - np.cos(th)) / th2 * Om + (th - np.sin(th)) / (th2 * th) * (Om @ Om)
+    v = np.linalg.solve(V, t)
+    return np.concatenate([omega, v]) / float(duration)
 
 
 class Core:
@@ -509,6 +550,19 @@ class Core:
         (0 = no cap); rebuild the voxel map.  A crop that would leave no points raises and changes nothing."""
         c = np.ascontiguousarray(np.asarray(center, dtype=np.float64).reshape(3))
         self._check(self._lib.vgicp_crop_target(self._h, _dp(c), float(radius), int(max_points)))
+
+    # ---- motion compensation
+    def deskew_source(self, times, twist, t_ref=0.0):
+        """Re-express every source point in the sensor frame at t_ref: point i <- Exp((times[i] - t_ref) twist) p_i, on the device
+        (include/vgicp_b200.h documents the float32 arithmetic).  times: one relative timestamp per source point, a 1-D float32
+        array or a strided float32 column such as cloud["time"] of a structured array; twist: [omega, v] per time unit.
+        Afterwards the source has no neighbours and no covariances, as after set_source_cloud."""
+        a = np.asarray(times)
+        if a.ndim != 1 or a.dtype != np.float32 or a.strides[0] < 4 or a.strides[0] % 4 != 0:
+            a = np.ascontiguousarray(a, dtype=np.float32).reshape(-1)
+        stride = a.strides[0] if len(a) > 1 else 4
+        xi = np.ascontiguousarray(np.asarray(twist, dtype=np.float64).reshape(6))
+        self._check(self._lib.vgicp_deskew_source(self._h, a.ctypes.data, len(a), stride, _dp(xi), float(t_ref)))
 
     def transform_source(self, T, stride=12, out=None):
         n = self.num_source_points()

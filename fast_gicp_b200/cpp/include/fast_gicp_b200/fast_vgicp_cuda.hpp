@@ -72,6 +72,18 @@ public:
     target_ = pcl::make_shared<PointCloudTarget>();
   }
 
+  // Motion compensation (an extension): every source point becomes Exp((t_i - t_ref) twist) p_i, the point in the sensor frame at
+  // t_ref (include/vgicp_b200.h), then the source covariances are recomputed as setInputSource computes them.  t: n float
+  // timestamps stride_bytes apart, e.g. &cloud->points[0].time and sizeof(PointT); twist = [omega, v] per time unit.  Afterwards
+  // input_ is a copy of the cloud given to setInputSource (its fields stay for align's output), so setInputSource(that cloud)
+  // reloads the raw points.
+  void deskewSource(const float* t, size_t n, size_t stride_bytes, const double twist[6], double t_ref = 0.0) {
+    if (!input_) throw std::runtime_error("FastVGICPCuda: deskewSource needs an input source");
+    checkStrict(vgicp_deskew_source(vgicp_cuda_, t, n, stride_bytes, twist, t_ref));
+    sourceCovariances();
+    input_ = pcl::make_shared<PointCloudSource>(*input_);
+  }
+
   virtual void swapSourceAndTarget() override {  // impl:69-72
     check(vgicp_swap_source_and_target(vgicp_cuda_));
     input_.swap(target_);
@@ -83,16 +95,7 @@ public:
     if (cloud == input_) return;
     pcl::Registration<PointSource, PointTarget, Scalar>::setInputSource(cloud);
     check(vgicp_set_source_cloud(vgicp_cuda_, cloud->empty() ? nullptr : &cloud->points[0].x, cloud->size(), sizeof(PointSource)));
-    switch (neighbor_search_method_) {
-      case NearestNeighborMethod::CPU_PARALLEL_KDTREE:  // the same exact neighbour sets, computed on the GPU
-      case NearestNeighborMethod::GPU_BRUTEFORCE:
-        check(vgicp_find_source_neighbors(vgicp_cuda_, k_correspondences_));
-        check(vgicp_calculate_source_covariances(vgicp_cuda_, static_cast<int>(regularization_method_)));
-        break;
-      case NearestNeighborMethod::GPU_RBF_KERNEL:
-        check(vgicp_calculate_source_covariances_rbf(vgicp_cuda_, static_cast<int>(regularization_method_)));
-        break;
-    }
+    sourceCovariances();
   }
 
   virtual void setInputTarget(const PointCloudTargetConstPtr& cloud) override {  // impl:114-141
@@ -146,6 +149,18 @@ private:
   void check(int rc) const {
     if (rc != VGICP_OK && rc != VGICP_ERR_UNSUPPORTED) throw std::runtime_error(std::string("FastVGICPCuda: ") + vgicp_last_error(vgicp_cuda_));
     if (rc == VGICP_ERR_UNSUPPORTED) std::cerr << vgicp_last_error(vgicp_cuda_) << std::endl;  // the reference prints and carries on
+  }
+  void sourceCovariances() {  // impl:96-110
+    switch (neighbor_search_method_) {
+      case NearestNeighborMethod::CPU_PARALLEL_KDTREE:  // the same exact neighbour sets, computed on the GPU
+      case NearestNeighborMethod::GPU_BRUTEFORCE:
+        check(vgicp_find_source_neighbors(vgicp_cuda_, k_correspondences_));
+        check(vgicp_calculate_source_covariances(vgicp_cuda_, static_cast<int>(regularization_method_)));
+        break;
+      case NearestNeighborMethod::GPU_RBF_KERNEL:
+        check(vgicp_calculate_source_covariances_rbf(vgicp_cuda_, static_cast<int>(regularization_method_)));
+        break;
+    }
   }
   void checkStrict(int rc) const {  // the extensions have no reference behaviour to follow: every failure throws
     if (rc != VGICP_OK) throw std::runtime_error(std::string("FastVGICPCuda: ") + vgicp_last_error(vgicp_cuda_));

@@ -236,6 +236,13 @@ PYBIND11_MODULE(pygicp, m) {
            v.cropTarget(center.data(), radius, max_points);
          },
          py::arg("center"), py::arg("radius"), py::arg("max_points") = 0)
+    // motion compensation (not in the reference binding): one relative timestamp per source point, twist = [omega, v]
+    .def("deskew_source",
+         [](VgicpCuda& v, const ArrF& times, const ArrD& twist, double t_ref) {
+           if (twist.size() != 6) throw std::invalid_argument("twist must have 6 elements");
+           v.deskewSource(times.data(), static_cast<size_t>(times.size()), sizeof(float), twist.data(), t_ref);
+         },
+         py::arg("times"), py::arg("twist"), py::arg("t_ref") = 0.0)
     .def("get_fitness_score",
          [](VgicpCuda& v, double max_range) {
            double T[16], score = 0.0;

@@ -21,6 +21,7 @@
 #include "lsq_math.hpp"
 #include "vgicp_kernels.cuh"
 #include "vgicp_local_map.cuh"
+#include "vgicp_deskew.cuh"
 
 using namespace vgicp;
 
@@ -221,6 +222,11 @@ struct vgicp_context {
   std::vector<cudaEvent_t> prof_pool;
   double prof_ms[VGICP_PROF_NUM_CATEGORIES] = {0};
   uint64_t prof_launches[VGICP_PROF_NUM_CATEGORIES] = {0};
+
+  // motion compensation (vgicp_deskew_source); last, so that no other member moves, and created at the first call, so that a handle
+  // that never deskews does no extra work
+  cudaEvent_t ev_deskew = nullptr;  // end of the work enqueued on the main stream: the in-place deskew must not overtake its reads
+  std::vector<float> deskew_times;  // the caller's timestamps, packed contiguously
 };
 
 namespace {
@@ -1211,7 +1217,7 @@ int vgicp_destroy(vgicp_handle h) {
   if (h->h_multi_done) cudaFreeHost(h->h_multi_done);
   for (auto& r : h->prof_pending) { cudaEventDestroy(r.a); cudaEventDestroy(r.b); }
   for (auto e : h->prof_pool) cudaEventDestroy(e);
-  for (cudaEvent_t e : {h->ev_copy, h->ev_append, h->target.ready, h->source.ready})
+  for (cudaEvent_t e : {h->ev_copy, h->ev_append, h->ev_deskew, h->target.ready, h->source.ready})
     if (e) cudaEventDestroy(e);
   if (h->stream_b) cudaStreamDestroy(h->stream_b);
   if (h->stream) cudaStreamDestroy(h->stream);
@@ -1865,6 +1871,64 @@ int vgicp_crop_target(vgicp_handle h, const double center[3], double radius, siz
   std::swap(t.covB, h->spare_covB);
   t.n = kept;
   return local_map_rebuild(h);
+}
+
+// ---- motion compensation: deskew the source from per-point timestamps and a constant body twist ----
+int vgicp_deskew_source(vgicp_handle h, const float* t, size_t n, size_t stride_bytes, const double twist[6], double t_ref) {
+  CHECK_HANDLE(h);
+  DeviceGuard g(h->device);
+  if (n > 0 && (!t || !twist)) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "deskew_source: null timestamps or twist");
+  if (stride_bytes < 4 || (stride_bytes % 4) != 0) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "deskew_source: stride_bytes must be a multiple of 4 and >= 4");
+  Cloud& s = h->source;
+  if (!s.has_pts || s.n == 0) return fail(h, VGICP_ERR_BAD_STATE, "deskew_source: no source points");
+  if (n != (size_t)s.n) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "deskew_source: the number of timestamps differs from the number of source points");
+  // the kernel takes every value as a float: a value finite in double but not in float is rejected too
+  const float tau = (float)t_ref;
+  float xi[6];
+  for (int j = 0; j < 6; j++) xi[j] = (float)twist[j];
+  if (!std::isfinite(tau)) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "deskew_source: non-finite t_ref");
+  for (int j = 0; j < 6; j++)
+    if (!std::isfinite(xi[j])) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "deskew_source: non-finite twist");
+  // one pass over the caller's strided array: validate, find the time range, pack contiguously
+  std::vector<float>& packed = h->deskew_times;
+  packed.resize(n);
+  const unsigned char* raw = reinterpret_cast<const unsigned char*>(t);
+  float lo = 0.0f, hi = 0.0f;
+  for (size_t i = 0; i < n; i++) {
+    float v;
+    memcpy(&v, raw + i * stride_bytes, sizeof(float));
+    if (!std::isfinite(v)) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "deskew_source: non-finite timestamp");
+    if (i == 0 || v < lo) lo = v;
+    if (i == 0 || v > hi) hi = v;
+    packed[i] = v;
+  }
+  const double span = fmax(fabs((double)lo - t_ref), fabs((double)hi - t_ref));
+  const double omega = sqrt(twist[0] * twist[0] + twist[1] * twist[1] + twist[2] * twist[2]);
+  if (omega * span > 1.5707963267948966)
+    return fail(h, VGICP_ERR_INVALID_ARGUMENT, "deskew_source: the rotation over the sweep exceeds pi/2 (|omega| * max |t_i - t_ref|), beyond the series");
+  // the kernel overwrites the source points: it must not overtake the evaluations on the main stream, nor an append that reads them
+  if (s.st != h->stream) {
+    if (!h->ev_deskew) CU_TRY(h, cudaEventCreateWithFlags(&h->ev_deskew, cudaEventDisableTiming));
+    CU_TRY(h, cudaEventRecord(h->ev_deskew, h->stream));
+    CU_TRY(h, cudaStreamWaitEvent(s.st, h->ev_deskew, 0));
+  }
+  if (s.st != h->target.st) CU_TRY(h, cudaStreamWaitEvent(s.st, h->ev_append, 0));
+  CU_TRY(h, s.staging.reserve(n * sizeof(float)));
+  CU_TRY(h, cudaMemcpyAsync(s.staging.p, packed.data(), n * sizeof(float), cudaMemcpyHostToDevice, s.st));
+  CU_TRY(h, cudaEventRecord(h->ev_copy, s.st));
+  KLAUNCH_ST(h, s.st, VGICP_PROF_OTHER,
+             k_deskew_points<<<blocks_for(n, 256), 256, 0, s.st>>>(s.pts.p, reinterpret_cast<const float*>(s.staging.p), (int)n, tau, xi[0], xi[1], xi[2], xi[3], xi[4], xi[5]));
+  CU_TRY(h, cudaGetLastError());
+  CU_TRY(h, cudaEventRecord(s.ready, s.st));
+  // the state set_source_cloud leaves: no neighbour rows, no covariances, the NDT source map reset
+  s.k = 0;
+  s.has_cov = false;
+  h->ndt_ready = false;
+  h->ndt_s.built = false;
+  h->ndt_s.pending = false;
+  // the packed timestamps are reused by the next call: the copy out of them must have landed
+  CU_TRY(h, cudaEventSynchronize(h->ev_copy));
+  return VGICP_OK;
 }
 
 // ---- multi-GPU: source sharding with an in-kernel exchange of the linear system over NVLink peer memory ----

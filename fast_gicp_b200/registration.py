@@ -329,6 +329,20 @@ class FastVGICPCuda(LsqRegistration):
     def crop_target(self, center, radius, max_points=0):
         self.cropTarget(center, radius, max_points)
 
+    # -- motion compensation (an extension).  Afterwards the source on the device is no longer the cloud given to setInputSource:
+    # input_ becomes a copy of it (its points stay for align's output), so setInputSource(that cloud) reloads the raw cloud.
+    def deskewSource(self, times, twist, t_ref=0.0):
+        """Re-express every source point in the sensor frame at t_ref under the constant body twist [omega, v] (per time unit of
+        `times`, one relative timestamp per source point), then recompute the source covariances as setInputSource does."""
+        if self.input_ is None:
+            raise RuntimeError("deskewSource: input source not set")
+        self.vgicp_cuda_.deskew_source(times, twist, t_ref)
+        self._covariances("source")
+        self.input_ = np.array(self.input_, copy=True)
+
+    def deskew_source(self, times, twist, t_ref=0.0):
+        self.deskewSource(times, twist, t_ref)
+
     # -- state machine (:69-141)
     def swapSourceAndTarget(self):
         self.vgicp_cuda_.swap_source_and_target()

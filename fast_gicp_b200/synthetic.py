@@ -63,6 +63,82 @@ def voxel_downsample(pts, leaf):
     return (sums / counts).astype(np.float32)
 
 
+def se3_exp_batch(xi):
+    """Exp of rotation-first twists xi (m, 6) -> (m, 4, 4), float64; the formula of se3_exp in csrc/lsq_math.hpp, vectorised.
+    A zero twist gives the identity exactly."""
+    xi = np.asarray(xi, dtype=np.float64).reshape(-1, 6)
+    w, v = xi[:, :3], xi[:, 3:]
+    th2 = (w * w).sum(axis=1)
+    th = np.sqrt(th2)
+    small = th2 < 1e-10
+    with np.errstate(divide="ignore", invalid="ignore"):
+        imag = np.where(small, 0.5 - th2 / 48.0 + th2 * th2 / 3840.0, np.sin(0.5 * th) / th)
+        real = np.where(small, 1.0 - th2 / 8.0 + th2 * th2 / 384.0, np.cos(0.5 * th))
+        c1 = np.where(small, 0.0, (1.0 - np.cos(th)) / th2)
+        c2 = np.where(small, 0.0, (th - np.sin(th)) / (th2 * th))
+    qx, qy, qz = (imag[:, None] * w).T
+    tx, ty, tz = 2.0 * qx, 2.0 * qy, 2.0 * qz
+    twx, twy, twz = tx * real, ty * real, tz * real
+    txx, txy, txz, tyy, tyz, tzz = tx * qx, ty * qx, tz * qx, ty * qy, tz * qy, tz * qz
+    T = np.zeros((len(xi), 4, 4))
+    T[:, 0, 0], T[:, 0, 1], T[:, 0, 2] = 1.0 - (tyy + tzz), txy - twz, txz + twy
+    T[:, 1, 0], T[:, 1, 1], T[:, 1, 2] = txy + twz, 1.0 - (txx + tzz), tyz - twx
+    T[:, 2, 0], T[:, 2, 1], T[:, 2, 2] = txz - twy, tyz + twx, 1.0 - (txx + tyy)
+    Om = np.zeros((len(xi), 3, 3))
+    Om[:, 0, 1], Om[:, 0, 2], Om[:, 1, 2] = -w[:, 2], w[:, 1], -w[:, 0]
+    Om[:, 1, 0], Om[:, 2, 0], Om[:, 2, 1] = w[:, 2], -w[:, 1], w[:, 0]
+    V = np.eye(3)[None] + c1[:, None, None] * Om + c2[:, None, None] * (Om @ Om)
+    V = np.where(small[:, None, None], T[:, :3, :3], V)
+    T[:, :3, 3] = np.einsum("nij,nj->ni", V, v)
+    T[:, 3, 3] = 1.0
+    return T
+
+
+def distorted_scan(world, beams, az_steps, start_pose, twist, period, noise_rng, max_range=120.0, noise=0.02):
+    """One revolution of a sensor that moves while it spins: azimuth column a is fired at t_a = period * a / az_steps from the
+    pose start_pose @ Exp(t_a twist) (twist = rotation-first [omega, v] per second in the sensor frame at t = 0).  Returns
+    (points, times): each point in the sensor frame of its own firing time (float32), and that time (float32).  With a zero
+    twist the points are scan(world, beams, az_steps, start_pose, ...)'s bytes."""
+    el = np.radians(np.linspace(-24.8, 2.0, beams))
+    az = np.linspace(-np.pi, np.pi, az_steps, endpoint=False)
+    ce, se = np.cos(el)[:, None], np.sin(el)[:, None]
+    d_s = np.stack([ce * np.cos(az)[None, :], ce * np.sin(az)[None, :], np.broadcast_to(se, (beams, az_steps))], axis=-1).reshape(-1, 3)
+    t_col = period * np.arange(az_steps) / az_steps
+    dT = se3_exp_batch(t_col[:, None] * np.asarray(twist, dtype=np.float64)[None, :])  # sensor at t_a in the sensor frame at 0
+    col = np.tile(np.arange(az_steps), beams)
+    R, o = start_pose[:3, :3], start_pose[:3, 3]
+    d = np.einsum("nij,nj->ni", dT[col, :3, :3], d_s) @ R.T
+    o = dT[col, :3, 3] @ R.T + o
+    t = np.full(len(d), np.inf)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        tg = (-1.73 - o[:, 2]) / d[:, 2]  # ground plane z = -1.73
+    t = np.where((tg > 0) & np.isfinite(tg), tg, t)
+    for lo, hi in world:
+        t = np.minimum(t, _ray_box(o, d, lo, hi))
+    ok = np.isfinite(t) & (t < max_range) & (t > 1.0)
+    r = t[ok] + noise_rng.normal(0.0, noise, size=int(ok.sum()))
+    return (d_s[ok] * r[:, None]).astype(np.float32), t_col[col[ok]].astype(np.float32)
+
+
+def voxel_downsample_values(pts, values, leaf):
+    """voxel_downsample that also averages a per-point value channel (e.g. timestamps) over each voxel -> (points, values);
+    the points are voxel_downsample(pts, leaf)'s."""
+    values = np.asarray(values, dtype=np.float32)
+    if leaf <= 0:
+        return pts, values
+    ijk = np.floor(pts / np.float32(leaf)).astype(np.int64)
+    ijk -= ijk.min(axis=0)
+    dims = ijk.max(axis=0) + 1
+    idx = ijk[:, 0] + dims[0] * (ijk[:, 1] + dims[1] * ijk[:, 2])
+    order = np.argsort(idx, kind="stable")
+    idx_s = idx[order]
+    starts = np.flatnonzero(np.r_[True, idx_s[1:] != idx_s[:-1]])
+    sums = np.add.reduceat(pts[order].astype(np.float64), starts, axis=0)
+    vsums = np.add.reduceat(values[order].astype(np.float64), starts)
+    counts = np.diff(np.r_[starts, len(idx_s)])
+    return (sums / counts[:, None]).astype(np.float32), (vsums / counts).astype(np.float32)
+
+
 def kitti_like_pair(beams=64, az_steps=2083, seed=42, pose=(0.8, 0.05, 0.7), downsample=0.25, max_points=None):
     """(target, source, T_gt): target scanned at the origin, source from a sensor moved by pose=(tx, ty, yaw_deg).
     T_gt maps source-frame points into the target frame (what registration should recover)."""

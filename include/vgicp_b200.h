@@ -223,6 +223,38 @@ VGICP_API int vgicp_append_source_to_target(vgicp_handle h, const double T[16]);
  * Errors: VGICP_ERR_INVALID_ARGUMENT (null center, NaN or negative radius, a crop that would leave no points: target and map are
  * then left exactly as they were), VGICP_ERR_BAD_STATE (target without points or covariances). */
 VGICP_API int vgicp_crop_target(vgicp_handle h, const double center[3], double radius, size_t max_points);
+/* ---- motion compensation (not in the reference) ---------------------------------------------------------------------------
+ * A spinning or solid-state LiDAR fires the points of one sweep over its period while the vehicle moves; each point is in the
+ * sensor frame of its own firing time.  vgicp_deskew_source re-expresses every source point in the sensor frame at t_ref under a
+ * constant body velocity, so that the registration result is the pose at t_ref:
+ *   source point i  <-  Exp((t_i - t_ref) xi) p_i,
+ * xi = [omega, v] the twist per time unit in the sensor frame at t_ref, rotation first (the order of se3_exp, so3.hpp).  For a
+ * constant-velocity guess, xi = log(T_{k-1}^-1 T_k) / dt (twist_from_motion in fast_gicp_b200/core.py).
+ *   t, n, stride_bytes  host pointer to n float timestamps stride_bytes apart (stride >= 4, a multiple of 4): &cloud[0].time
+ *                       with sizeof(PointT) reads them out of a PointXYZIT-like struct.  n must equal the source size.  Times
+ *                       are relative (e.g. seconds since the start of the sweep): absolute epoch times have no precision
+ *                       left in a float.
+ * Arithmetic: IEEE single operations without contraction, in this order, so that numpy float32 rebuilds the same bytes:
+ *   tau = (float)t_ref, om_j = (float)xi_j, nu_j = (float)xi_{3+j} (cast once);
+ *   per point: s = t_i - tau, w_j = s om_j, u_j = s nu_j, q = (w0 w0 + w1 w1) + w2 w2  (theta^2);
+ *   A, B, C by Horner, h = h q + c from the first coefficient listed (the series of sin(theta)/theta, (1 - cos(theta))/theta^2,
+ *   (theta - sin(theta))/theta^3 in q, truncated below 2^-24 relative for theta <= pi/2; no trig calls):
+ *     A: 1.6059044e-10f, -2.5052108e-08f, 2.7557319e-06f, -0.0001984127f, 0.008333334f, -0.16666667f, 1.0f
+ *     B: -2.0876756e-09f, 2.755732e-07f, -2.4801588e-05f, 0.0013888889f, -0.041666668f, 0.5f
+ *     C: -1.6059044e-10f, 2.5052108e-08f, -2.7557319e-06f, 0.0001984127f, -0.008333334f, 0.16666667f
+ *   K = [w]x = [[0, -w2, w1], [w2, 0, -w0], [-w1, w0, 0]];  K2_jk = w_j w_k off the diagonal, K2_jj = w_j w_j - q;
+ *   R_jk = (d_jk + A K_jk) + B K2_jk,  V_jk = (d_jk + B K_jk) + C K2_jk  (d_jk = 1 on the diagonal, else 0);
+ *   p'_j = ((R_j0 p0 + R_j1 p1) + R_j2 p2) + ((V_j0 u0 + V_j1 u1) + V_j2 u2).
+ * A zero twist returns every point's value unchanged (only the sign of a zero may differ).
+ * Afterwards the handle is in the state set_source_cloud with the deskewed points would leave: no neighbour rows and no
+ * covariances (find_source_neighbors + calculate_source_covariances come next), the NDT source map reset; handle settings, the
+ * target and its map are kept.  Works under every problem and under source and stage-1 sharding (every rank makes the same
+ * deterministic change).  The timestamps are packed on the host and uploaded (4 bytes per point), one kernel runs on the
+ * source's stream after the work already enqueued that reads the source points.
+ * Errors, all returned before anything is modified or launched: VGICP_ERR_INVALID_ARGUMENT (null t or twist with n > 0, n other
+ * than the source size, a bad stride, a timestamp, twist component or t_ref that is not finite as a float, a rotation over the
+ * sweep beyond the series: |omega| * max_i |t_i - t_ref| > pi/2 in double), VGICP_ERR_BAD_STATE (no source points). */
+VGICP_API int vgicp_deskew_source(vgicp_handle h, const float* t, size_t n, size_t stride_bytes, const double twist[6], double t_ref);
 /* pcl::transformPointCloud of the source by T (lsq_registration_impl.hpp:78) on the device; out: n x stride floats */
 VGICP_API int vgicp_transform_source(vgicp_handle h, const double T[16], float* out_xyz, size_t capacity_points, size_t stride_bytes);
 /* set_{source,target}_cloud with the points already resident in this GPU's memory (device pointer, same layout rules);

@@ -43,6 +43,18 @@ c.crop_target((0.0, 0.0, 0.0), 30.0, len(tgt))
 r = c.align(pose_from_c(r.T))
 print("local map", c.num_target_points(), "converged", bool(r.converged))
 c.close()
+# motion compensation: timestamps read out of a 32-byte point struct, the source deskewed in place, covariances recomputed
+c = Core(0)
+c.set_neighbor_search_method("DIRECT7")
+cloud = np.zeros(len(src), dtype=np.dtype({"names": ["xyz", "time"], "formats": [("<f4", 3), "<f4"], "offsets": [0, 16], "itemsize": 32}))
+cloud["xyz"], cloud["time"] = src[:, :3], np.linspace(0.0, 0.1, len(src), dtype=np.float32)
+c.set_target_cloud(tgt); c.find_target_neighbors(20); c.calculate_target_covariances(3); c.create_target_voxelmap()
+c.set_source_cloud(src)
+c.deskew_source(cloud["time"], [0.0, 0.0, 0.35, 8.0, 0.0, 0.0], 0.05)
+c.find_source_neighbors(20); c.calculate_source_covariances(3)
+r = c.align()
+print("deskew", c.num_source_points(), "converged", bool(r.converged))
+c.close()
 # NDT D2D through the same evaluation kernels
 c = Core(0)
 c.set_problem(2); c.set_neighbor_search_method("DIRECT7")
