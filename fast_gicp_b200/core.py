@@ -41,7 +41,7 @@ EXPORTED_SYMBOLS = [
     "vgicp_lsq_default_params", "vgicp_align", "vgicp_transform_source",
     "vgicp_get_launch_count", "vgicp_synchronize", "vgicp_get_stream",
     "vgicp_set_source_cloud_device", "vgicp_set_target_cloud_device", "vgicp_set_profiling", "vgicp_get_profile", "vgicp_profile_category_name",
-    "vgicp_set_knn_mode", "vgicp_set_voxel_index", "vgicp_set_speculation", "vgicp_register", "vgicp_get_fitness_score", "vgicp_set_execution_hint", "vgicp_set_problem", "vgicp_ndt_create_voxelmaps",
+    "vgicp_set_voxel_index", "vgicp_set_speculation", "vgicp_register", "vgicp_get_fitness_score", "vgicp_set_execution_hint", "vgicp_set_problem", "vgicp_ndt_create_voxelmaps",
     "vgicp_comm_export", "vgicp_comm_init", "vgicp_comm_shutdown", "vgicp_comm_error", "vgicp_set_source_shard", "vgicp_clear_source_shard",
     "vgicp_comm_export_arena", "vgicp_comm_init_arena", "vgicp_set_stage1_sharding", "vgicp_set_source_covariances", "vgicp_set_target_covariances",
     "vgicp_align_multi", "vgicp_evaluate_poses", "vgicp_set_robust_kernel",
@@ -136,7 +136,6 @@ def load_library():
         "vgicp_set_source_cloud_device": [hp, C.c_void_p, C.c_size_t, C.c_size_t],
         "vgicp_set_target_cloud_device": [hp, C.c_void_p, C.c_size_t, C.c_size_t],
         "vgicp_set_profiling": [hp, C.c_int],
-        "vgicp_set_knn_mode": [hp, C.c_int],
         "vgicp_set_voxel_index": [hp, C.c_int],
         "vgicp_set_speculation": [hp, C.c_int],
         "vgicp_get_fitness_score": [hp, dp, C.c_double, dp],
@@ -318,9 +317,6 @@ class Core:
     def set_execution_hint(self, hint):
         """0 = latency (default), 1 = throughput (many handles share the GPU)."""
         self._check(self._lib.vgicp_set_execution_hint(self._h, int(hint)))
-
-    def set_knn_mode(self, mode):
-        self._check(self._lib.vgicp_set_knn_mode(self._h, int(mode)))
 
     def set_voxel_index(self, mode):
         """0: direct-mapped voxel index when the map's bounding box fits (default), 1: hash table only."""

@@ -177,9 +177,6 @@ struct vgicp_context {
   int stage1_sharding = 0;
   int speculate = 1;  // LM trial evaluations also linearise at the trial pose (vgicp_set_speculation)
   int exec_hint = 0;  // 0 = latency (one registration should finish as soon as possible), 1 = throughput (many concurrent handles)
-  int lin_stream = 1;   // VGICP_LIN_STREAM=0 disables the bulk-copy streaming kernel of DIRECT1 (A/B measurements)
-  int force_lin_g = 0;  // VGICP_LIN_G override of the lanes-per-point split (experiments)
-  int knn_mode = 0;  // 0 = hash grid (default), 1 = warp-cooperative scan of the whole cloud, 2 = legacy per-thread scan
   DevBuf<double> partials;
   DevBuf<int> corr_ids;
   unsigned int* d_ticket = nullptr;
@@ -369,27 +366,18 @@ int find_neighbors(vgicp_handle h, Cloud& c, int k) {
   if (!c.has_pts) return fail(h, VGICP_ERR_BAD_STATE, "find_neighbors: cloud not set");
   if (k <= 0 || k > kMaxK || k > c.n) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "find_neighbors: need 1 <= k <= min(num_points, 64)");
   CU_TRY(h, c.nbr.reserve((size_t)c.n * k));
-  cudaError_t ke = cudaSuccess;
-  if (h->knn_mode == 2) {  // legacy one-thread-per-query scan, kept for A/B measurements
-    c.knn_sorted = nullptr;
-    c.knn_q_begin = 0;
-    c.knn_q_end = c.n;
-    KLAUNCH_ST(h, c.st, VGICP_PROF_KNN, ke = launch_knn_bruteforce(c.pts.p, c.n, k, c.nbr.p, c.st));
-  } else {
-    const size_t need = knn_grid_scratch_bytes(c.n, nullptr, nullptr);
-    CU_TRY(h, c.knn_scratch.reserve(need));
-    int nl = 0;
-    c.knn_q_begin = 0;
-    c.knn_q_end = c.n;
-    if (h->stage1_sharding && h->comm_ranks > 1 && h->arena_peers[h->comm_rank]) {  // this rank's slice of the queries (sorted positions)
-      const long long base = c.n / h->comm_ranks, rem = c.n % h->comm_ranks, r = h->comm_rank;
-      c.knn_q_begin = (int)(r * base + (r < rem ? r : rem));
-      c.knn_q_end = c.knn_q_begin + (int)base + (r < rem ? 1 : 0);
-    }
-    KLAUNCH_ST(h, c.st, VGICP_PROF_KNN, ke = launch_knn_grid(c.pts.p, c.n, k, c.nbr.p, c.knn_scratch.p, c.knn_scratch.cap, (h->knn_mode == 1 || c.n < 256) ? 1 : 0, c.knn_q_begin,
-                                                            c.knn_q_end, &nl, &c.knn_sorted, c.st));
-    h->launches += nl > 0 ? nl - 1 : 0;
+  CU_TRY(h, c.knn_scratch.reserve(knn_grid_scratch_bytes(c.n, nullptr, nullptr)));
+  c.knn_q_begin = 0;
+  c.knn_q_end = c.n;
+  if (h->stage1_sharding && h->comm_ranks > 1 && h->arena_peers[h->comm_rank]) {  // this rank's slice of the queries (sorted positions)
+    const long long base = c.n / h->comm_ranks, rem = c.n % h->comm_ranks, r = h->comm_rank;
+    c.knn_q_begin = (int)(r * base + (r < rem ? r : rem));
+    c.knn_q_end = c.knn_q_begin + (int)base + (r < rem ? 1 : 0);
   }
+  cudaError_t ke = cudaSuccess;
+  int nl = 0;
+  KLAUNCH_ST(h, c.st, VGICP_PROF_KNN, ke = launch_knn_grid(c.pts.p, c.n, k, c.nbr.p, c.knn_scratch.p, c.knn_scratch.cap, c.knn_q_begin, c.knn_q_end, &nl, &c.knn_sorted, c.st));
+  h->launches += nl > 0 ? nl - 1 : 0;
   CU_TRY(h, ke);
   CU_TRY(h, cudaEventRecord(c.ready, c.st));
   c.k = k;
@@ -677,11 +665,13 @@ int sync_inputs(vgicp_handle h) {
   return VGICP_OK;
 }
 
-// arguments + launch geometry of an evaluation kernel
+// arguments, kernel and launch geometry of an evaluation, decided once: a multi-pose launch runs, per row, the kernel and grid of the
+// single-pose launch
 struct LinLaunch {
   LinArgs a;
-  int grid;
-  int G;
+  bool stream;  // k_linearize_stream*, else the compacted kernels (k_linearize*)
+  int G;        // compacted kernels: lanes per source point in the lookup phase
+  int grid;     // blocks (per row of a multi-pose launch)
 };
 LinLaunch make_lin_launch(vgicp_handle h) {
   Cloud& s = h->source;
@@ -716,27 +706,54 @@ LinLaunch make_lin_launch(vgicp_handle h) {
   // before the arithmetic the split costs no lane efficiency, so it is used under both execution hints
   const bool cols = h->offset_mode == 27;
   L.G = !wide ? 1 : (cols ? 3 : (n_off <= 7 ? 4 : 8));
-  {
-    const int force_g = h->force_lin_g;  // VGICP_LIN_G, read once in vgicp_create (A/B measurements)
-    if (cols ? (force_g == 1 || force_g == 3) : (force_g == 1 || force_g == 4 || force_g == 8)) L.G = force_g;
+  // DIRECT1 on a large cloud with the direct-mapped index: the bandwidth-bound shape, streamed through shared memory by bulk copies
+  L.stream = h->offset_mode == 1 && a.dense.cells != nullptr && a.n >= 65536 && (reinterpret_cast<uintptr_t>(a.covB) & 15) == 0;
+  if (L.stream) {
+    const int tiles = (a.n + kLinStreamTile - 1) / kLinStreamTile;
+    L.grid = tiles < kLinStreamMaxBlocks ? tiles : kLinStreamMaxBlocks;
+  } else {
+    const int tasks_per_block = (kLinThreads / 32) * ((32 / L.G) * L.G);
+    long long tasks = (long long)(a.n > 0 ? a.n : 1) * L.G;
+    long long grid = (tasks + tasks_per_block - 1) / tasks_per_block;
+    L.grid = (int)(grid > kLinMaxBlocks ? kLinMaxBlocks : grid);
   }
-  const int tasks_per_block = (kLinThreads / 32) * ((32 / L.G) * L.G);
-  long long tasks = (long long)(a.n > 0 ? a.n : 1) * L.G;
-  long long grid = (tasks + tasks_per_block - 1) / tasks_per_block;
-  L.grid = (int)(grid > kLinMaxBlocks ? kLinMaxBlocks : grid);
   return L;
 }
 
-// DIRECT1 on a large cloud with the direct-mapped index: the bandwidth-bound shape, streamed through shared memory by bulk copies
-// (k_linearize_stream); returns its grid, or 0 when the compacted kernels run
-int stream_kernel_grid(vgicp_handle h, const LinArgs& a) {
-  const bool stream_kernel = h->offset_mode == 1 && a.dense.cells != nullptr && a.n >= 65536 && h->lin_stream != 0 && (reinterpret_cast<uintptr_t>(a.covB) & 15) == 0;
-  if (!stream_kernel) return 0;
-  const int tiles = (a.n + kLinStreamTile - 1) / kLinStreamTile;
-  return tiles < kLinStreamMaxBlocks ? tiles : kLinStreamMaxBlocks;
+enum { kEvalLinearize = 0, kEvalError = 1, kEvalSpec = 2 };  // what an evaluation launch computes (every row of a multi-pose one alike)
+
+template <int V>
+using IntC = std::integral_constant<int, V>;
+
+// Calls f(WHAT, RB) with the streaming kernels' WHAT for an evaluation kind (0 error, 1 linearisation, 2 speculative) and RB (robust
+// weights) as compile-time constants.
+template <class F>
+void with_stream_kernel(int kind, bool robust, F&& f) {
+  auto what = [&](auto rb) {
+    if (kind == kEvalSpec) f(IntC<2>{}, rb);
+    else if (kind == kEvalLinearize) f(IntC<1>{}, rb);
+    else f(IntC<0>{}, rb);
+  };
+  if (robust) what(std::true_type{});
+  else what(std::false_type{});
 }
 
-enum { kEvalLinearize = 0, kEvalError = 1, kEvalSpec = 2 };  // what an evaluation launch computes (every row of a multi-pose one alike)
+// The compacted evaluation kernels that exist: offset table MODE (1 / 7 / 27, 0 = generic list) with the lanes per point G that
+// make_lin_launch picks for it.  Calls f(MODE, G, RB) as compile-time constants; false when (mode, G) is not in the table.
+template <int M, int GG>
+struct LinShape { static constexpr int MODE = M, G = GG; };
+template <class F, class RB, class... S>
+bool with_lin_shape(int mode, int G, F& f, RB rb, S...) {
+  return ((S::MODE == mode && S::G == G && (f(IntC<S::MODE>{}, IntC<S::G>{}, rb), true)) || ...);
+}
+template <class F>
+bool with_lin_kernel(int mode, int G, bool robust, F&& f) {
+  auto table = [&](auto rb) {
+    return with_lin_shape(mode, G, f, rb, LinShape<1, 1>{}, LinShape<7, 1>{}, LinShape<7, 4>{}, LinShape<27, 1>{}, LinShape<27, 3>{},
+                          LinShape<0, 1>{}, LinShape<0, 4>{}, LinShape<0, 8>{});
+  };
+  return robust ? table(std::true_type{}) : table(std::false_type{});
+}
 
 // one evaluation: launches the fused lookup+derivative kernel at Teval over the correspondences of h->lin
 int launch_linearize(vgicp_handle h, const Pose& Teval, int kind) {
@@ -750,45 +767,22 @@ int launch_linearize(vgicp_handle h, const Pose& Teval, int kind) {
     a.done_flag = h->h_flag;
     a.done_seq = ++h->eval_seq;
   }
-  const int grid = L.grid, G = L.G;
-  // rb: std::bool_constant of the robust-kernel instantiations (a.robust != 0)
-#define LAUNCH_LIN_G(MODE, GG)                                                                       \
-  do {                                                                                               \
-    if (spec) k_linearize_spec<MODE, GG, RB><<<grid, kLinThreads, 0, h->stream>>>(a);                \
-    else if (want_H) k_linearize<MODE, true, GG, RB><<<grid, kLinThreads, 0, h->stream>>>(a);        \
-    else k_linearize<MODE, false, GG, RB><<<grid, kLinThreads, 0, h->stream>>>(a);                   \
-  } while (0)
-#define LAUNCH_LIN(MODE)                 \
-  do {                                   \
-    if (G == 8) LAUNCH_LIN_G(MODE, 8);   \
-    else if (G == 4) LAUNCH_LIN_G(MODE, 4); \
-    else LAUNCH_LIN_G(MODE, 1);          \
-  } while (0)
   prof_begin(h, want_H ? VGICP_PROF_LINEARIZE : VGICP_PROF_ERROR, h->stream);
-  const int sgrid = stream_kernel_grid(h, a);
-  auto launch = [&](auto rb) {
-    constexpr bool RB = decltype(rb)::value;
-    if (sgrid > 0) {
-      const size_t smem = sizeof(LinStreamSmem);
-      if (spec) k_linearize_stream<2, RB><<<sgrid, kLinThreads, smem, h->stream>>>(a);
-      else if (want_H) k_linearize_stream<1, RB><<<sgrid, kLinThreads, smem, h->stream>>>(a);
-      else k_linearize_stream<0, RB><<<sgrid, kLinThreads, smem, h->stream>>>(a);
-    } else
-    switch (h->offset_mode) {
-      case 1: LAUNCH_LIN_G(1, 1); break;
-      case 7: LAUNCH_LIN(7); break;
-      case 27:
-        if (G == 3) LAUNCH_LIN_G(27, 3);
-        else LAUNCH_LIN_G(27, 1);
-        break;
-      default: LAUNCH_LIN(0); break;
-    }
-  };
-  if (a.robust) launch(std::true_type{});
-  else launch(std::false_type{});
-#undef LAUNCH_LIN_G
-#undef LAUNCH_LIN
+  bool launched = true;
+  if (L.stream)
+    with_stream_kernel(kind, a.robust, [&](auto what, auto rb) {
+      k_linearize_stream<decltype(what)::value, decltype(rb)::value><<<L.grid, kLinThreads, sizeof(LinStreamSmem), h->stream>>>(a);
+    });
+  else
+    launched = with_lin_kernel(h->offset_mode, L.G, a.robust, [&](auto mode, auto g, auto rb) {
+      constexpr int MODE = decltype(mode)::value, G = decltype(g)::value;
+      constexpr bool RB = decltype(rb)::value;
+      if (spec) k_linearize_spec<MODE, G, RB><<<L.grid, kLinThreads, 0, h->stream>>>(a);
+      else if (want_H) k_linearize<MODE, true, G, RB><<<L.grid, kLinThreads, 0, h->stream>>>(a);
+      else k_linearize<MODE, false, G, RB><<<L.grid, kLinThreads, 0, h->stream>>>(a);
+    });
   prof_end(h, h->stream);
+  if (!launched) return fail(h, VGICP_ERR_UNSUPPORTED, "no evaluation kernel for this offset table and lane split");
   h->launches++;
   CU_TRY(h, cudaGetLastError());
   return VGICP_OK;
@@ -907,12 +901,6 @@ int check_ready_for_multi(vgicp_handle h, const char* who) {
   return VGICP_OK;
 }
 
-// a multi-pose launch's row grid: the single-pose launch's grid (compacted kernels or the streaming kernel)
-int multi_grid(vgicp_handle h, const LinLaunch& L) {
-  const int sgrid = stream_kernel_grid(h, L.a);
-  return sgrid > 0 ? sgrid : L.grid;
-}
-
 // fixed-size buffers on first use; the partial sums grow with rows x grid (256 bytes per block and row)
 int multi_reserve(vgicp_handle h, int rows, int grid) {
   if (!h->h_multi_out) {
@@ -954,48 +942,30 @@ int launch_multi(vgicp_handle h, const LinLaunch& L, int n_hyp, int kind, bool c
   m.out = (direct ? h->h_multi_out : h->d_multi_out) + (size_t)row0 * kMultiOut;
   m.done = direct ? h->h_multi_done + row0 : nullptr;
   m.done_seq = h->multi_seq;
-  const int sgrid = stream_kernel_grid(h, a), G = L.G;
-  const dim3 grid(sgrid > 0 ? sgrid : L.grid, n);
-#define LAUNCH_MULTI_G(MODE, GG)                                                                                           \
-  do {                                                                                                                     \
-    if (kind == kEvalSpec) k_linearize_spec_multi<MODE, GG, RB><<<grid, kLinThreads, 0, h->stream>>>(a, m);              \
-    else if (kind == kEvalLinearize && count) k_linearize_multi<MODE, true, GG, true, RB><<<grid, kLinThreads, 0, h->stream>>>(a, m); \
-    else if (kind == kEvalLinearize) k_linearize_multi<MODE, true, GG, false, RB><<<grid, kLinThreads, 0, h->stream>>>(a, m); \
-    else if (count) k_linearize_multi<MODE, false, GG, true, RB><<<grid, kLinThreads, 0, h->stream>>>(a, m);              \
-    else k_linearize_multi<MODE, false, GG, false, RB><<<grid, kLinThreads, 0, h->stream>>>(a, m);                       \
-  } while (0)
-#define LAUNCH_MULTI(MODE)                    \
-  do {                                        \
-    if (G == 8) LAUNCH_MULTI_G(MODE, 8);      \
-    else if (G == 4) LAUNCH_MULTI_G(MODE, 4); \
-    else LAUNCH_MULTI_G(MODE, 1);             \
-  } while (0)
+  const dim3 grid(L.grid, n);
   prof_begin(h, kind == kEvalError ? VGICP_PROF_ERROR : VGICP_PROF_LINEARIZE, h->stream);
-  auto launch = [&](auto rb) {  // rb: std::bool_constant of the robust-kernel instantiations
-    constexpr bool RB = decltype(rb)::value;
-    if (sgrid > 0) {
+  bool launched = true;
+  if (L.stream)
+    with_stream_kernel(kind, a.robust, [&](auto what, auto rb) {
+      constexpr int WHAT = decltype(what)::value;
+      constexpr bool RB = decltype(rb)::value;
       const size_t smem = sizeof(LinStreamSmem);
-      if (kind == kEvalSpec) k_linearize_stream_multi<2, false, RB><<<grid, kLinThreads, smem, h->stream>>>(a, m);
-      else if (kind == kEvalLinearize && count) k_linearize_stream_multi<1, true, RB><<<grid, kLinThreads, smem, h->stream>>>(a, m);
-      else if (kind == kEvalLinearize) k_linearize_stream_multi<1, false, RB><<<grid, kLinThreads, smem, h->stream>>>(a, m);
-      else if (count) k_linearize_stream_multi<0, true, RB><<<grid, kLinThreads, smem, h->stream>>>(a, m);
-      else k_linearize_stream_multi<0, false, RB><<<grid, kLinThreads, smem, h->stream>>>(a, m);
-    } else
-    switch (h->offset_mode) {
-      case 1: LAUNCH_MULTI_G(1, 1); break;
-      case 7: LAUNCH_MULTI(7); break;
-      case 27:
-        if (G == 3) LAUNCH_MULTI_G(27, 3);
-        else LAUNCH_MULTI_G(27, 1);
-        break;
-      default: LAUNCH_MULTI(0); break;
-    }
-  };
-  if (a.robust) launch(std::true_type{});
-  else launch(std::false_type{});
-#undef LAUNCH_MULTI_G
-#undef LAUNCH_MULTI
+      if constexpr (WHAT == 2) k_linearize_stream_multi<2, false, RB><<<grid, kLinThreads, smem, h->stream>>>(a, m);  // (counts no hits)
+      else if (count) k_linearize_stream_multi<WHAT, true, RB><<<grid, kLinThreads, smem, h->stream>>>(a, m);
+      else k_linearize_stream_multi<WHAT, false, RB><<<grid, kLinThreads, smem, h->stream>>>(a, m);
+    });
+  else
+    launched = with_lin_kernel(h->offset_mode, L.G, a.robust, [&](auto mode, auto g, auto rb) {
+      constexpr int MODE = decltype(mode)::value, G = decltype(g)::value;
+      constexpr bool RB = decltype(rb)::value;
+      if (kind == kEvalSpec) k_linearize_spec_multi<MODE, G, RB><<<grid, kLinThreads, 0, h->stream>>>(a, m);
+      else if (kind == kEvalLinearize && count) k_linearize_multi<MODE, true, G, true, RB><<<grid, kLinThreads, 0, h->stream>>>(a, m);
+      else if (kind == kEvalLinearize) k_linearize_multi<MODE, true, G, false, RB><<<grid, kLinThreads, 0, h->stream>>>(a, m);
+      else if (count) k_linearize_multi<MODE, false, G, true, RB><<<grid, kLinThreads, 0, h->stream>>>(a, m);
+      else k_linearize_multi<MODE, false, G, false, RB><<<grid, kLinThreads, 0, h->stream>>>(a, m);
+    });
   prof_end(h, h->stream);
+  if (!launched) return fail(h, VGICP_ERR_UNSUPPORTED, "no evaluation kernel for this offset table and lane split");
   h->launches++;
   CU_TRY(h, cudaGetLastError());
   return VGICP_OK;
@@ -1149,8 +1119,6 @@ int vgicp_create(int device, vgicp_handle* out) {
   vgicp_context* h = new (std::nothrow) vgicp_context();
   if (!h) return VGICP_ERR_CUDA;
   h->device = device;
-  { const char* e = getenv("VGICP_LIN_G"); h->force_lin_g = e ? atoi(e) : 0; }
-  { const char* e = getenv("VGICP_LIN_STREAM"); h->lin_stream = e ? atoi(e) : 1; }
   DeviceGuard g(device);
   // the kernel image is sm_90a only: fail loudly on anything else instead of falling back
   cudaFuncAttributes fa;
@@ -1653,7 +1621,7 @@ int vgicp_align_multi(vgicp_handle h, const double* guesses, int n_guesses, cons
   if (params) P = *params; else vgicp_lsq_default_params(&P);
   const int B = n_guesses;
   const LinLaunch L = make_lin_launch(h);
-  if ((rc = multi_reserve(h, B, multi_grid(h, L)))) return rc;
+  if ((rc = multi_reserve(h, B, L.grid))) return rc;
   std::vector<LmState> st(B);
   for (int i = 0; i < B; i++) st[i] = lm_init(guesses + 16 * i, P);
   const bool speculate = h->speculate != 0 && !P.use_gauss_newton;
@@ -1700,7 +1668,7 @@ int vgicp_evaluate_poses(vgicp_handle h, const double* T, int n_poses, double* e
   const int B = n_poses;
   const bool want_H = H36 != nullptr;
   const LinLaunch L = make_lin_launch(h);
-  if ((rc = multi_reserve(h, B, multi_grid(h, L)))) return rc;
+  if ((rc = multi_reserve(h, B, L.grid))) return rc;
   Pose* poses = multi_poses(h);
   int* rows = multi_rows(h, B);
   for (int i = 0; i < B; i++) {
@@ -1731,9 +1699,9 @@ int vgicp_evaluate_poses(vgicp_handle h, const double* T, int n_poses, double* e
 // streams) and later calls replay it with one cudaGraphLaunch.  The unpack kernels stay outside: their input pointers change on
 // every call.  The host waits, the growth of the voxel table and everything after them (voxelmap_finish, the LM loop) stay eager.
 
-// the plain VGICP path: no profiling (per-launch events), default k-NN engine, no sharding
+// the plain VGICP path: no profiling (per-launch events), no sharding
 static bool stage1_graph_eligible(vgicp_handle h, int reg) {
-  return h->problem == 0 && !h->prof_on && h->knn_mode == 0 && !h->stage1_sharding && h->comm_ranks <= 1 && h->shard_end < 0 &&
+  return h->problem == 0 && !h->prof_on && !h->stage1_sharding && h->comm_ranks <= 1 && h->shard_end < 0 &&
          reg != VGICP_REG_NORMALIZED_MIN_EIG;
 }
 
@@ -2226,13 +2194,6 @@ int vgicp_set_execution_hint(vgicp_handle h, int hint) {
   CHECK_HANDLE(h);
   if (hint < 0 || hint > 1) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "set_execution_hint: 0 latency, 1 throughput");
   h->exec_hint = hint;
-  return VGICP_OK;
-}
-
-int vgicp_set_knn_mode(vgicp_handle h, int mode) {
-  CHECK_HANDLE(h);
-  if (mode < 0 || mode > 2) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "set_knn_mode: 0 grid, 1 warp scan, 2 legacy scan");
-  h->knn_mode = mode;
   return VGICP_OK;
 }
 

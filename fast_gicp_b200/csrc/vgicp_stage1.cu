@@ -16,58 +16,6 @@
 namespace vgicp {
 
 // ---------------------------------------------------------------------------------------------------------------
-// Stage 1a: exact brute-force k-NN inside one cloud (self included).  One query per thread, targets staged through
-// shared memory in tiles (every thread reads the same target -> broadcast, conflict-free), per-thread ascending
-// top-k list in shared memory laid out [k][thread] (conflict-free).  d2 = (dx*dx + dy*dy) + dz*dz, no contraction.
-// Replaces brute_force_knn.cu:16-60 (global-memory heap per thread) and the CPU kd-tree of
-// fast_vgicp_cuda_impl.hpp:152-167.  Output rows ascending in (d2, index).
-// ---------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kKnnThreads) k_knn_bruteforce(const float4* __restrict__ pts, int n, int k, int* __restrict__ nbr) {
-  extern __shared__ float smem_knn[];
-  float4* tile = reinterpret_cast<float4*>(smem_knn);                       // kKnnTile float4
-  float* ld = smem_knn + 4 * kKnnTile;                                      // [k][kKnnThreads]
-  int* li = reinterpret_cast<int*>(ld + (size_t)k * kKnnThreads);           // [k][kKnnThreads]
-  const int tid = threadIdx.x;
-  const int q = blockIdx.x * kKnnThreads + tid;
-  const bool active = q < n;
-  float4 qp = active ? pts[q] : make_float4(0.f, 0.f, 0.f, 0.f);
-  for (int j = 0; j < k; j++) {
-    ld[j * kKnnThreads + tid] = __int_as_float(0x7f800000);  // +inf
-    li[j * kKnnThreads + tid] = -1;
-  }
-  float worst = __int_as_float(0x7f800000);
-  for (int base = 0; base < n; base += kKnnTile) {
-    __syncthreads();
-    for (int j = tid; j < kKnnTile; j += kKnnThreads) {
-      int g = base + j;
-      tile[j] = g < n ? pts[g] : make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-    __syncthreads();
-    if (!active) continue;
-    const int lim = min(kKnnTile, n - base);
-#pragma unroll 4
-    for (int j = 0; j < lim; j++) {
-      float4 t = tile[j];
-      float dx = __fsub_rn(t.x, qp.x), dy = __fsub_rn(t.y, qp.y), dz = __fsub_rn(t.z, qp.z);
-      float d = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
-      if (d < worst) {  // targets arrive in increasing index, so ties keep the smaller index: ascending (d2, index)
-        int p = k - 1;
-        while (p > 0 && ld[(p - 1) * kKnnThreads + tid] > d) {
-          ld[p * kKnnThreads + tid] = ld[(p - 1) * kKnnThreads + tid];
-          li[p * kKnnThreads + tid] = li[(p - 1) * kKnnThreads + tid];
-          p--;
-        }
-        ld[p * kKnnThreads + tid] = d;
-        li[p * kKnnThreads + tid] = base + j;
-        worst = ld[(k - 1) * kKnnThreads + tid];
-      }
-    }
-  }
-  if (active)
-    for (int j = 0; j < k; j++) nbr[(size_t)q * k + j] = li[j * kKnnThreads + tid];
-}
-
-// ---------------------------------------------------------------------------------------------------------------
 // 3x3 helpers (registers).  Full matrices are row-major m[r*3+c] here.
 // ---------------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void inv3_general(const float* m, float* o) {  // Eigen Matrix3f::inverse(): cofactors / det (column 0 expansion)
@@ -1066,16 +1014,6 @@ cudaError_t launch_regularize_voxels(VoxelRec* vox, const int* nv_ptr, int vmax,
   return cudaGetLastError();
 }
 
-size_t knn_smem_bytes(int k) { return sizeof(float4) * kKnnTile + (size_t)k * kKnnThreads * (sizeof(float) + sizeof(int)); }
-
-cudaError_t launch_knn_bruteforce(const float4* pts, int n, int k, int* nbr, cudaStream_t stream) {
-  // per device and thread-safe: set on every call (a host-side attribute write; this engine is the A/B legacy path)
-  cudaError_t e = cudaFuncSetAttribute(k_knn_bruteforce, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)knn_smem_bytes(kMaxK));
-  if (e != cudaSuccess) return e;
-  k_knn_bruteforce<<<(n + kKnnThreads - 1) / kKnnThreads, kKnnThreads, knn_smem_bytes(k), stream>>>(pts, n, k, nbr);
-  return cudaGetLastError();
-}
-
 size_t knn_grid_scratch_bytes(int n, int* levels_out, unsigned* table_size_out) {
   int L = 8;
   for (long m = 16384; m * 4 <= (long)n && L < kGridMaxLevels; m *= 4) L++;
@@ -1092,7 +1030,8 @@ size_t knn_grid_scratch_bytes(int n, int* levels_out, unsigned* table_size_out) 
 //                  [zero-filled : bbox max (16 B) | counters (256 B) | sort scratch (digit histograms, tickets, look-back state)]
 //                  [uninitialised: Morton codes x2 | sort values x2 | sorted points | deferred-query queue]
 // q_begin/q_end: sorted positions whose neighbours are searched (whole cloud: 0, n); the build always covers the whole cloud.
-cudaError_t launch_knn_grid(const float4* pts, int n, int k, int* nbr, unsigned char* scratch, size_t scratch_bytes, int force_bruteforce, int q_begin, int q_end, int* launches,
+// A cloud below 256 points sends every query straight to the block-cooperative scan of the whole cloud (k_knn_deferred).
+cudaError_t launch_knn_grid(const float4* pts, int n, int k, int* nbr, unsigned char* scratch, size_t scratch_bytes, int q_begin, int q_end, int* launches,
                             const float4** sorted_out, cudaStream_t stream) {
   int L;
   unsigned T;
@@ -1145,8 +1084,9 @@ cudaError_t launch_knn_grid(const float4* pts, int n, int k, int* nbr, unsigned 
   const int nq = q_end > q_begin ? q_end - q_begin : 0;
   if (nq > 0) {
     const int sblocks = (nq + kSearchWarps - 1) / kSearchWarps;
-    if (k <= 32) k_knn_search<false><<<sblocks, kSearchWarps * 32, 0, stream>>>(a, force_bruteforce);
-    else k_knn_search<true><<<sblocks, kSearchWarps * 32, 0, stream>>>(a, force_bruteforce);
+    const int whole_cloud = n < 256 ? 1 : 0;
+    if (k <= 32) k_knn_search<false><<<sblocks, kSearchWarps * 32, 0, stream>>>(a, whole_cloud);
+    else k_knn_search<true><<<sblocks, kSearchWarps * 32, 0, stream>>>(a, whole_cloud);
     int hblocks = (nq + kKnnGridWarps - 1) / kKnnGridWarps;
     if (hblocks > 4 * kNumSMs) hblocks = 4 * kNumSMs;  // persistent: items pulled from a counter
     if (k <= 32) k_knn_deferred<false><<<hblocks, kKnnGridWarps * 32, 0, stream>>>(a);

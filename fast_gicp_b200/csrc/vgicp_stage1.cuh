@@ -11,17 +11,15 @@ struct VoxelRec {
   float4 c1;      // cyz czz 0 0
 };
 
-constexpr int kMaxK = 64;         // k-NN list capacity
-constexpr int kKnnThreads = 128;  // queries per block in the brute-force k-NN
-constexpr int kKnnTile = 512;     // targets staged in shared memory per step
-constexpr int kRbfBlock = 512;    // covariance_estimation_rbf.cu:60 BLOCK_SIZE
+constexpr int kMaxK = 64;       // k-NN list capacity
+constexpr int kRbfBlock = 512;  // covariance_estimation_rbf.cu:60 BLOCK_SIZE
 
-// exact k-NN of every point inside its own cloud; rows ascending in (d2, index)
-cudaError_t launch_knn_bruteforce(const float4* pts, int n, int k, int* nbr, cudaStream_t stream);
-// the same result on a Morton-ordered multi-level grid, one thread per query (k <= 64); scratch from knn_grid_scratch_bytes(), 16-byte
-// aligned.  [q_begin, q_end): the sorted positions whose rows are computed (0, n = all; a slice per rank when stage 1 is sharded)
+// exact k-NN of every point inside its own cloud (k <= 64), rows ascending in (d2, index), on a Morton-ordered multi-level grid: one
+// warp per query, a block-cooperative scan for the queries the grid does not narrow down (every query of a cloud below 256 points);
+// scratch from knn_grid_scratch_bytes(), 16-byte aligned.  [q_begin, q_end): the sorted positions whose rows are computed (0, n = all;
+// a slice per rank when stage 1 is sharded)
 size_t knn_grid_scratch_bytes(int n, int* levels_out, unsigned* table_size_out);
-cudaError_t launch_knn_grid(const float4* pts, int n, int k, int* nbr, unsigned char* scratch, size_t scratch_bytes, int force_bruteforce, int q_begin, int q_end, int* launches,
+cudaError_t launch_knn_grid(const float4* pts, int n, int k, int* nbr, unsigned char* scratch, size_t scratch_bytes, int q_begin, int q_end, int* launches,
                             const float4** sorted_out, cudaStream_t stream);
 // covariances of the points at sorted positions [pos_begin, pos_end) of that grid, stored into the covariance arrays of all `nranks`
 // ranks (peer-mapped pointers; the own arrays included)

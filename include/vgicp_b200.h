@@ -298,14 +298,11 @@ VGICP_API int vgicp_clear_source_shard(vgicp_handle h);
  * No kNN and no per-point covariances are involved (the reference's NDTCuda never computes them). */
 VGICP_API int vgicp_set_problem(vgicp_handle h, int problem);
 VGICP_API int vgicp_ndt_create_voxelmaps(vgicp_handle h);
-/* Execution hint: 0 = latency (default: the persistent k-NN kernel takes 4 blocks per SM; every evaluation writes its 43 doubles
- * straight into mapped host memory and the calling thread spins on a completion word), 1 = throughput / polite (2 k-NN blocks per SM;
- * evaluations are read back with a copy and a stream wait, so the host thread sleeps instead of spinning).  Results are identical.
- * bench.py uses the latency shape. */
+/* Execution hint: how an evaluation hands its result to the host.  0 = latency (default: every evaluation writes its 43 doubles
+ * straight into mapped host memory and the calling thread spins on a completion word), 1 = throughput / polite (evaluations are
+ * read back with a copy and a stream wait, so the host thread sleeps instead of spinning).  The kernels, their launch shapes and
+ * the results are the same under both.  bench.py uses the latency shape. */
 VGICP_API int vgicp_set_execution_hint(vgicp_handle h, int hint);
-/* k-NN engine used by find_*_neighbors: 0 = multi-level hash grid (default), 1 = warp-cooperative scan of the whole cloud,
- * 2 = one-thread-per-query scan (the shape of the reference's brute_force_knn.cu).  All three return identical rows. */
-VGICP_API int vgicp_set_knn_mode(vgicp_handle h, int mode);
 /* Voxel lookup structure used by the evaluation kernels (update_correspondences + compute_derivatives fused): 0 = a direct-mapped
  * cell -> voxel-id array over the bounding box of the target's voxel coordinates, built next to the hash table whenever that box
  * has at most 16 Mi cells (default; any LiDAR-like cloud), 1 = always probe the reference-layout hash table

@@ -1,6 +1,6 @@
 #!/bin/bash
-# compute-sanitizer passes over the hot path (run under gpurun): memcheck + racecheck + synccheck on one full registration
-# per k-NN engine / neighbour mode.  Output: gpurun_out/sanitizer_*.log
+# compute-sanitizer passes over the hot path: memcheck + racecheck + synccheck on one full registration per neighbour mode,
+# and on both k-NN search paths.  One log per tool, written by the loop at the end.
 set -u
 cat > /tmp/san_driver.py <<'PY'
 import sys, numpy as np
@@ -8,16 +8,22 @@ sys.path.insert(0, ".")
 from fast_gicp_b200.core import Core
 d = np.load("tests/golden/pair_0p2.npz")
 tgt, src = d["target"][::3].copy(), d["source"][::3].copy()
-for method, knn_mode, hint, vindex, spec in (("DIRECT27", 0, 0, 0, 1), ("DIRECT7", 0, 1, 0, 1), ("DIRECT1", 1, 0, 1, 0), ("DIRECT_RADIUS", 0, 1, 1, 1),
-                                             ("DIRECT27", 0, 0, 1, 0)):
+for method, hint, vindex, spec in (("DIRECT27", 0, 0, 1), ("DIRECT7", 1, 0, 1), ("DIRECT1", 0, 1, 0), ("DIRECT_RADIUS", 1, 1, 1),
+                                   ("DIRECT27", 0, 1, 0)):
     c = Core(0)
     c.set_neighbor_search_method(method, 1.5)
-    c.set_knn_mode(knn_mode); c.set_execution_hint(hint)
+    c.set_execution_hint(hint)
     c.set_voxel_index(vindex); c.set_speculation(spec)
     r = c.register(tgt, src)
     c.calculate_source_covariances_rbf(3)
     print(method, "converged", bool(r.converged), "fitness", c.fitness_score(np.eye(4)))
     c.close()
+# a cloud below 256 points: every query takes the block-cooperative scan of the whole cloud (k <= 32 and the wide k > 32 kernels)
+c = Core(0)
+for k in (20, 64):
+    c.set_source_cloud(src[:200]); c.find_source_neighbors(k)
+    print("small cloud k", k, "rows", c.get_source_neighbors().shape)
+c.close()
 # a far outlier: the voxel bounding box no longer fits the direct-mapped index, the k-NN grid's levels are all coarse there and the deferred (block-cooperative) search takes the queries
 c = Core(0)
 c.set_neighbor_search_method("DIRECT27")

@@ -53,19 +53,20 @@ def test_knn_matches_oracle_exactly(core, prepared):
     assert np.array_equal(got[:, 0], np.arange(len(got)))  # self is neighbour 0 (H6)
 
 
-@pytest.mark.parametrize("mode", [0, 1, 2])
+@pytest.mark.parametrize("cloud", ["grid", "small", "far"])
 @pytest.mark.parametrize("k", [1, 7, 33, 64])
-def test_knn_other_k(core, k, mode):
-    """All three k-NN engines (hash grid, warp scan, per-thread scan) return the oracle's rows; duplicates tie-break by index."""
+def test_knn_other_k(core, k, cloud):
+    """Both k-NN search paths return the oracle's rows; duplicates tie-break by index.  grid: the warp-per-query grid search;
+    small: a cloud below 256 points, every query scans the whole cloud block-cooperatively; far: a few far outliers, whose queries
+    (more of them for k = 64) scan all 1500 points block-cooperatively, for k > 32 with the wide kernels."""
     rng = np.random.default_rng(k)
-    pts = rng.uniform(-20, 20, size=(1500, 3)).astype(np.float32)
+    pts = rng.uniform(-20, 20, size=(200 if cloud == "small" else 1500, 3)).astype(np.float32)
     pts[100:110] = pts[100]  # duplicates: ties broken by index
-    core.set_knn_mode(mode)
+    if cloud == "far":
+        pts[:5] = rng.uniform(2000, 5000, size=(5, 3))
     core.set_source_cloud(pts)
     core.find_source_neighbors(k)
-    got = core.get_source_neighbors()
-    core.set_knn_mode(0)
-    assert np.array_equal(got, O.knn(pts, k, "bruteforce"))
+    assert np.array_equal(core.get_source_neighbors(), O.knn(pts, k, "bruteforce"))
 
 
 @pytest.mark.parametrize("shape", ["line", "clusters", "outliers", "tiny", "identical", "17k"])
@@ -467,8 +468,8 @@ def test_c3_synthetic_kitti_pair_matches_oracle():
 def test_large_cloud_size_independent_properties():
     """C4-sized inputs (1M points) cannot be checked against the CPU oracle in seconds; check properties that do not depend on
     size: every point is its own nearest neighbour, neighbour rows are sorted by distance and duplicate-free, spot-checked rows
-    equal a brute-force scan, the voxel map conserves the points, H is symmetric positive definite, the one-lane and
-    eight-lane evaluation kernels agree, and the registration recovers the generator's motion."""
+    equal a brute-force scan, the voxel map conserves the points, H is symmetric positive definite, an evaluation under the
+    latency and the throughput execution hints agrees, and the registration recovers the generator's motion."""
     from fast_gicp_b200.core import Core, pose_from_c
     from fast_gicp_b200.synthetic import kitti_like_pair
 
@@ -573,39 +574,37 @@ def test_c4_matches_the_oracle_golden():
 
 def test_direct1_streaming_kernel_matches_the_gather_kernel():
     """DIRECT1 evaluations of clouds >= 64k points run in k_linearize_stream (source staged through shared memory by bulk copies);
-    VGICP_LIN_STREAM=0 keeps the ordinary kernel.  Same correspondences, same per-term arithmetic, another summation order: err, H, b
-    agree to float rounding, the registration walks the same iterates, and both match the oracle."""
-    import os
-
+    it reads the direct-mapped voxel index, so with the hash table alone (set_voxel_index(1)) the ordinary kernel runs.  The two
+    indexes return the same voxel ids (test_correspondences_and_linear_system).  Same correspondences, same per-term arithmetic,
+    another summation order: err, H, b agree to float rounding, the registration walks the same iterates, and both match the oracle."""
     from fast_gicp_b200.core import Core, pose_from_c
     from fast_gicp_b200.synthetic import kitti_like_pair
 
     tgt, src, T_gt = kitti_like_pair(beams=64, az_steps=2083, seed=7, pose=(0.6, 0.1, 0.8), downsample=0.0)
     assert len(src) > 65536
     got = {}
-    for flag in ("1", "0"):
-        os.environ["VGICP_LIN_STREAM"] = flag
+    for stream in (True, False):
         c = Core(0)
-        os.environ.pop("VGICP_LIN_STREAM")
+        c.set_voxel_index(0 if stream else 1)  # the hash table alone keeps the ordinary kernel
         _setup_pair(c, dict(tgt=tgt, src=src), O.DIRECT1, res=0.5)
         rows = []
         for T in (np.eye(4), T_gt):
             c.update_correspondences(T)
             rows.append(c.compute_error(T, True) + c.compute_error(T, False)[:1])
         res = c.align()
-        got[flag] = (rows, pose_from_c(res.T), res.nr_iterations, res.n_linearize, res.n_compute_error, bool(res.converged))
-        if flag == "1":
+        got[stream] = (rows, pose_from_c(res.T), res.nr_iterations, res.n_linearize, res.n_compute_error, bool(res.converged))
+        if stream:
             cov_t, cov_s = c.get_target_covariances(), c.get_source_covariances()
         c.close()
-    for (e1, H1, b1, eo1), (e0, H0, b0, eo0) in zip(got["1"][0], got["0"][0]):
+    for (e1, H1, b1, eo1), (e0, H0, b0, eo0) in zip(got[True][0], got[False][0]):
         assert abs(e1 - e0) <= 2e-6 * abs(e0) and abs(eo1 - eo0) <= 2e-6 * abs(eo0)
         assert np.abs(H1 - H0).max() <= 2e-6 * np.abs(H0).max() and np.abs(b1 - b0).max() <= 2e-6 * max(np.abs(b0).max(), 1e-3 * np.abs(H0).max())
-    assert got["1"][2:] == got["0"][2:] and got["1"][5]
-    dt, dr = pose_error(got["0"][1], got["1"][1])
+    assert got[True][2:] == got[False][2:] and got[True][5]
+    dt, dr = pose_error(got[False][1], got[True][1])
     assert dt < 1e-6 and dr < 1e-7, (dt, dr)
     vm = O.VoxelMap(tgt, cov_t, 0.5, accum_double=True)
     e0, H0, b0, _ = O.evaluate(vm, src, cov_s, O.offsets(O.DIRECT1), T_gt, T_gt, True)
-    e1, H1, b1, _ = got["1"][0][1]
+    e1, H1, b1, _ = got[True][0][1]
     assert abs(e1 - e0) <= 2e-5 * abs(e0) and np.abs(H1 - H0).max() <= 2e-5 * np.abs(H0).max()
 
 
