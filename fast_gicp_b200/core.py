@@ -46,6 +46,7 @@ EXPORTED_SYMBOLS = [
     "vgicp_comm_export_arena", "vgicp_comm_init_arena", "vgicp_set_stage1_sharding", "vgicp_set_source_covariances", "vgicp_set_target_covariances",
     "vgicp_align_multi", "vgicp_evaluate_poses", "vgicp_set_robust_kernel",
     "vgicp_append_source_to_target", "vgicp_crop_target", "vgicp_deskew_source",
+    "vgicp_set_source_timestamps", "vgicp_compute_error_ct", "vgicp_align_ct",
 ]
 PROF_NUM_CATEGORIES = 7
 
@@ -71,6 +72,19 @@ class AlignResult(C.Structure):
     _fields_ = [
         ("T", C.c_double * 16),
         ("H", C.c_double * 36),
+        ("nr_iterations", C.c_int),
+        ("converged", C.c_int),
+        ("n_linearize", C.c_int),
+        ("n_compute_error", C.c_int),
+        ("lm_failed", C.c_int),
+    ]
+
+
+class AlignCtResult(C.Structure):
+    _fields_ = [
+        ("T", C.c_double * 16),
+        ("twist", C.c_double * 6),
+        ("H", C.c_double * 144),
         ("nr_iterations", C.c_int),
         ("converged", C.c_int),
         ("n_linearize", C.c_int),
@@ -158,6 +172,9 @@ def load_library():
         "vgicp_append_source_to_target": [hp, dp],
         "vgicp_crop_target": [hp, dp, C.c_double, C.c_size_t],
         "vgicp_deskew_source": [hp, C.c_void_p, C.c_size_t, C.c_size_t, dp, C.c_double],
+        "vgicp_set_source_timestamps": [hp, C.c_void_p, C.c_size_t, C.c_size_t, C.c_double],
+        "vgicp_compute_error_ct": [hp, dp, dp, dp, dp, dp, dp, dp],
+        "vgicp_align_ct": [hp, dp, dp, dp, dp, C.POINTER(LsqParams), C.POINTER(AlignCtResult)],
     }
     for name, argtypes in sig.items():
         fn = getattr(L, name)
@@ -553,12 +570,51 @@ class Core:
         (include/vgicp_b200.h documents the float32 arithmetic).  times: one relative timestamp per source point, a 1-D float32
         array or a strided float32 column such as cloud["time"] of a structured array; twist: [omega, v] per time unit.
         Afterwards the source has no neighbours and no covariances, as after set_source_cloud."""
+        a, stride = self._times(times)
+        xi = np.ascontiguousarray(np.asarray(twist, dtype=np.float64).reshape(6))
+        self._check(self._lib.vgicp_deskew_source(self._h, a.ctypes.data, len(a), stride, _dp(xi), float(t_ref)))
+
+    @staticmethod
+    def _times(times):
+        """A 1-D float32 array (a strided column is passed as it is) -> (array, stride in bytes)."""
         a = np.asarray(times)
         if a.ndim != 1 or a.dtype != np.float32 or a.strides[0] < 4 or a.strides[0] % 4 != 0:
             a = np.ascontiguousarray(a, dtype=np.float32).reshape(-1)
-        stride = a.strides[0] if len(a) > 1 else 4
-        xi = np.ascontiguousarray(np.asarray(twist, dtype=np.float64).reshape(6))
-        self._check(self._lib.vgicp_deskew_source(self._h, a.ctypes.data, len(a), stride, _dp(xi), float(t_ref)))
+        return a, (a.strides[0] if len(a) > 1 else 4)
+
+    # ---- continuous-time registration
+    def set_source_timestamps(self, times, t_ref=0.0):
+        """One timestamp per source point (as deskew_source takes them), kept on the device for compute_error_ct / align_ct.
+        set_source_cloud and swap_source_and_target drop them; deskew_source keeps them."""
+        a, stride = self._times(times)
+        self._check(self._lib.vgicp_set_source_timestamps(self._h, a.ctypes.data, len(a), stride, float(t_ref)))
+
+    def compute_error_ct(self, T_lin, xi_lin, T_eval, xi_eval, want_H=True):
+        """-> (err, H (12,12) | None, b (12,) | None): the data terms at (T_eval, xi_eval) over the correspondences of
+        (T_lin, xi_lin), the state ordered [pose step (rotation first), twist step] (include/vgicp_b200.h)."""
+        tl, te = pose_to_c(T_lin), pose_to_c(T_eval)
+        xl = np.ascontiguousarray(np.asarray(xi_lin, dtype=np.float64).reshape(6))
+        xe = np.ascontiguousarray(np.asarray(xi_eval, dtype=np.float64).reshape(6))
+        err = C.c_double(0.0)
+        if want_H:
+            H = np.zeros(144)
+            b = np.zeros(12)
+            self._check(self._lib.vgicp_compute_error_ct(self._h, _dp(tl), _dp(xl), _dp(te), _dp(xe), _dp(H), _dp(b), C.byref(err)))
+            return err.value, H.reshape(12, 12).T.copy(), b
+        self._check(self._lib.vgicp_compute_error_ct(self._h, _dp(tl), _dp(xl), _dp(te), _dp(xe), None, None, C.byref(err)))
+        return err.value, None, None
+
+    def align_ct(self, guess=None, twist_guess=None, twist_prior=None, twist_weight=None, params=None):
+        """Pose at t_ref and the sweep's body twist together -> AlignCtResult (T, twist, H (144), counters).  twist_prior: the
+        prior mean (default: the twist guess), twist_weight: its 6 weights > 0 (default 1e-6 each)."""
+        g = pose_to_c(np.eye(4) if guess is None else guess)
+        tg = np.ascontiguousarray(np.zeros(6) if twist_guess is None else np.asarray(twist_guess, dtype=np.float64).reshape(6))
+        tp = tg.copy() if twist_prior is None else np.ascontiguousarray(np.asarray(twist_prior, dtype=np.float64).reshape(6))
+        tw = np.full(6, 1e-6) if twist_weight is None else np.ascontiguousarray(np.broadcast_to(np.asarray(twist_weight, dtype=np.float64), (6,)))
+        params = params or default_params()
+        res = AlignCtResult()
+        self._check(self._lib.vgicp_align_ct(self._h, _dp(g), _dp(tg), _dp(tp), _dp(tw), C.byref(params), C.byref(res)))
+        return res
 
     def transform_source(self, T, stride=12, out=None):
         n = self.num_source_points()

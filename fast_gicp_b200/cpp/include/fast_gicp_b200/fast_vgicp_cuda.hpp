@@ -84,6 +84,33 @@ public:
     input_ = pcl::make_shared<PointCloudSource>(*input_);
   }
 
+  // Continuous-time registration (an extension): the pose at t_ref and the sweep's body twist estimated together
+  // (vgicp_align_ct, include/vgicp_b200.h).  setSourceTimestamps takes one timestamp per point of the current source, as
+  // deskewSource does; setInputSource with another cloud and swapSourceAndTarget drop them, deskewSource keeps them.
+  void setSourceTimestamps(const float* t, size_t n, size_t stride_bytes, double t_ref = 0.0) {
+    if (!input_) throw std::runtime_error("FastVGICPCuda: setSourceTimestamps needs an input source");
+    checkStrict(vgicp_set_source_timestamps(vgicp_cuda_, t, n, stride_bytes, t_ref));
+  }
+  // Sets getFinalTransformation() (cast to float like align), hasConverged() and getFinalTwist(); `result` (optional) receives the
+  // whole record (double pose, twist, the 12 x 12 system, counters).  The guess is cast to float, like align's.
+  void alignCT(const Matrix4& guess, const double twist_guess[6], const double twist_prior[6], const double twist_weight[6], vgicp_align_ct_result* result = nullptr) {
+    if (!input_ || !target_) throw std::runtime_error("FastVGICPCuda: alignCT needs an input source and target");
+    multiPrelude();
+    double g[16];
+    for (int i = 0; i < 16; i++) g[i] = static_cast<double>(guess.v[i]);
+    const vgicp_lsq_params P = this->lsqParams();
+    vgicp_align_ct_result r;
+    this->converged_ = false;
+    checkStrict(vgicp_align_ct(vgicp_cuda_, g, twist_guess, twist_prior, twist_weight, &P, &r));
+    if (r.lm_failed) std::cerr << "lm not converged!!" << std::endl;
+    this->nr_iterations_ = r.nr_iterations;
+    this->converged_ = r.converged != 0;
+    for (int i = 0; i < 16; i++) this->final_transformation_.v[i] = static_cast<float>(r.T[i]);
+    for (int j = 0; j < 6; j++) final_twist_[j] = r.twist[j];
+    if (result) *result = r;
+  }
+  const double* getFinalTwist() const { return final_twist_; }
+
   virtual void swapSourceAndTarget() override {  // impl:69-72
     check(vgicp_swap_source_and_target(vgicp_cuda_));
     input_.swap(target_);
@@ -171,6 +198,7 @@ private:
   RegularizationMethod regularization_method_;
   NearestNeighborMethod neighbor_search_method_;
   vgicp_handle vgicp_cuda_ = nullptr;
+  double final_twist_[6] = {0, 0, 0, 0, 0, 0};
 };
 
 }  // namespace fast_gicp

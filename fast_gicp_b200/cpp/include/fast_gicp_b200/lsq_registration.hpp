@@ -86,14 +86,7 @@ public:
     std::vector<double> g(16 * guesses.size());
     for (int i = 0; i < n; i++)
       for (int k = 0; k < 16; k++) g[16 * i + k] = static_cast<double>(guesses[i].v[k]);
-    vgicp_lsq_params P;
-    vgicp_lsq_default_params(&P);
-    P.max_iterations = max_iterations_;
-    P.rotation_epsilon = rotation_epsilon_;
-    P.transformation_epsilon = transformation_epsilon_;
-    P.use_gauss_newton = lsq_optimizer_type_ == LSQ_OPTIMIZER_TYPE::GaussNewton ? 1 : 0;
-    P.lm_max_iterations = lm_max_iterations_;
-    P.lm_init_lambda_factor = lm_init_lambda_factor_;
+    const vgicp_lsq_params P = lsqParams();
     std::vector<vgicp_align_result> r(guesses.size());
     multiCheck(vgicp_align_multi(multiHandle(), g.data(), n, &P, r.data()));
     T_out.resize(guesses.size());
@@ -119,6 +112,18 @@ public:
   }
 
 protected:
+  // this optimiser's settings for the optimisers inside the library (vgicp_align_multi, vgicp_align_ct)
+  vgicp_lsq_params lsqParams() const {
+    vgicp_lsq_params P;
+    vgicp_lsq_default_params(&P);
+    P.max_iterations = max_iterations_;
+    P.rotation_epsilon = rotation_epsilon_;
+    P.transformation_epsilon = transformation_epsilon_;
+    P.use_gauss_newton = lsq_optimizer_type_ == LSQ_OPTIMIZER_TYPE::GaussNewton ? 1 : 0;
+    P.lm_max_iterations = lm_max_iterations_;
+    P.lm_init_lambda_factor = lm_init_lambda_factor_;
+    return P;
+  }
   // the device handle and the computeTransformation prelude of a subclass, for alignMulti / evaluatePoses
   virtual vgicp_handle multiHandle() const = 0;
   virtual void multiPrelude() {}
@@ -169,7 +174,7 @@ protected:
     linearize(x0, &H, &b);
     double nb[6], d[6];
     for (int i = 0; i < 6; i++) nb[i] = -b[i];
-    vgicp::ldlt_solve6(H.data(), nb, d);
+    vgicp::ldlt_solve<6>(H.data(), nb, d);
     delta = vgicp::se3_exp(d);
     x0 = vgicp::iso_mul(delta, x0);
     final_hessian_ = H;
@@ -191,7 +196,7 @@ protected:
       for (int q = 0; q < 6; q++) Hl(q, q) += lm_lambda_;
       double nb[6], d[6];
       for (int q = 0; q < 6; q++) nb[q] = -b[q];
-      vgicp::ldlt_solve6(Hl.data(), nb, d);
+      vgicp::ldlt_solve<6>(Hl.data(), nb, d);
       delta = vgicp::se3_exp(d);
       Isometry3d xi = vgicp::iso_mul(delta, x0);
       double yi = compute_error(xi);

@@ -93,6 +93,11 @@ static py::array_t<S> to_numpy(const Eigen::Matrix<S, N, N>& M) {
   for (int r = 0; r < N; r++) for (int c = 0; c < N; c++) o(r, c) = M(r, c);
   return out;
 }
+static ArrD filled(py::ssize_t n, double v) {
+  ArrD a(n);
+  for (py::ssize_t i = 0; i < n; i++) a.mutable_at(i) = v;
+  return a;
+}
 static ArrF identity4f() {
   ArrF m({4, 4});
   auto o = m.mutable_unchecked<2>();
@@ -243,6 +248,48 @@ PYBIND11_MODULE(pygicp, m) {
            v.deskewSource(times.data(), static_cast<size_t>(times.size()), sizeof(float), twist.data(), t_ref);
          },
          py::arg("times"), py::arg("twist"), py::arg("t_ref") = 0.0)
+    // continuous-time registration (not in the reference binding): pose at t_ref and the sweep's twist together
+    .def("set_source_timestamps",
+         [](VgicpCuda& v, const ArrF& times, double t_ref) { v.setSourceTimestamps(times.data(), static_cast<size_t>(times.size()), sizeof(float), t_ref); },
+         py::arg("times"), py::arg("t_ref") = 0.0)
+    // -> dict: T (4x4, the float transformation as double, like align), twist (6), H (12x12, double), and the counters.
+    // twist_prior None: the twist guess; twist_weight: 6 weights > 0 (a scalar applies to all)
+    .def("align_ct",
+         [](VgicpCuda& v, const ArrF& initial_guess, const ArrD& twist_guess, py::object twist_prior, const ArrD& twist_weight) {
+           if (twist_guess.size() != 6) throw std::invalid_argument("twist_guess must have 6 elements");
+           std::array<double, 6> tg, tp, tw;
+           for (int j = 0; j < 6; j++) tg[j] = twist_guess.data()[j];
+           tp = tg;
+           if (!twist_prior.is_none()) {
+             ArrD p = twist_prior.cast<ArrD>();
+             if (p.size() != 6) throw std::invalid_argument("twist_prior must have 6 elements");
+             for (int j = 0; j < 6; j++) tp[j] = p.data()[j];
+           }
+           if (twist_weight.size() != 6 && twist_weight.size() != 1) throw std::invalid_argument("twist_weight must have 6 elements or one");
+           for (int j = 0; j < 6; j++) tw[j] = twist_weight.data()[twist_weight.size() == 6 ? j : 0];
+           const Eigen::Matrix4f guess = to_mat4f(initial_guess);
+           vgicp_align_ct_result r;
+           {
+             py::gil_scoped_release release;
+             v.alignCT(guess, tg.data(), tp.data(), tw.data(), &r);
+           }
+           py::array_t<double> twist(6), H({12, 12});
+           auto h = H.mutable_unchecked<2>();
+           for (int j = 0; j < 6; j++) twist.mutable_at(j) = r.twist[j];
+           for (int row = 0; row < 12; row++) for (int c = 0; c < 12; c++) h(row, c) = r.H[c * 12 + row];
+           py::dict out;
+           out["T"] = to_numpy(v.getFinalTransformation().cast<double>());
+           out["twist"] = twist;
+           out["H"] = H;
+           out["nr_iterations"] = r.nr_iterations;
+           out["converged"] = r.converged != 0;
+           out["n_linearize"] = r.n_linearize;
+           out["n_compute_error"] = r.n_compute_error;
+           out["lm_failed"] = r.lm_failed != 0;
+           return out;
+         },
+         py::arg("initial_guess") = identity4f(), py::arg("twist_guess") = filled(6, 0.0), py::arg("twist_prior") = py::none(),
+         py::arg("twist_weight") = filled(1, 1e-6))
     .def("get_fitness_score",
          [](VgicpCuda& v, double max_range) {
            double T[16], score = 0.0;

@@ -77,41 +77,43 @@ inline Iso3d se3_exp(const double* a) {
   return T;
 }
 
-// Solve A x = rhs, A symmetric 6x6 column-major; LDL^T with diagonal pivoting.
-inline void ldlt_solve6(const double* A_in, const double* rhs, double* x) {
-  double A[6][6];
-  int perm[6];
-  for (int r = 0; r < 6; r++) {
+// Solve A x = rhs, A symmetric N x N column-major; LDL^T with diagonal pivoting.  N = 6: the pose step; N = 12: pose and twist
+// (vgicp_align_ct).
+template <int N>
+inline void ldlt_solve(const double* A_in, const double* rhs, double* x) {
+  double A[N][N];
+  int perm[N];
+  for (int r = 0; r < N; r++) {
     perm[r] = r;
-    for (int c = 0; c < 6; c++) A[r][c] = A_in[c * 6 + r];
+    for (int c = 0; c < N; c++) A[r][c] = A_in[c * N + r];
   }
-  for (int k = 0; k < 6; k++) {
+  for (int k = 0; k < N; k++) {
     int p = k;
     double best = fabs(A[k][k]);
-    for (int i = k + 1; i < 6; i++)
+    for (int i = k + 1; i < N; i++)
       if (fabs(A[i][i]) > best) { best = fabs(A[i][i]); p = i; }
     if (p != k) {
-      for (int j = 0; j < 6; j++) { double t = A[k][j]; A[k][j] = A[p][j]; A[p][j] = t; }
-      for (int j = 0; j < 6; j++) { double t = A[j][k]; A[j][k] = A[j][p]; A[j][p] = t; }
+      for (int j = 0; j < N; j++) { double t = A[k][j]; A[k][j] = A[p][j]; A[p][j] = t; }
+      for (int j = 0; j < N; j++) { double t = A[j][k]; A[j][k] = A[j][p]; A[j][p] = t; }
       int t = perm[k]; perm[k] = perm[p]; perm[p] = t;
     }
     const double d = A[k][k];
     if (d == 0.0) continue;
-    for (int i = k + 1; i < 6; i++) A[i][k] /= d;
-    for (int j = k + 1; j < 6; j++)
-      for (int i = j; i < 6; i++) {
+    for (int i = k + 1; i < N; i++) A[i][k] /= d;
+    for (int j = k + 1; j < N; j++)
+      for (int i = j; i < N; i++) {
         A[i][j] -= A[i][k] * d * A[j][k];
         A[j][i] = A[i][j];
       }
   }
-  double y[6];
-  for (int i = 0; i < 6; i++) y[i] = rhs[perm[i]];
-  for (int i = 0; i < 6; i++)
+  double y[N];
+  for (int i = 0; i < N; i++) y[i] = rhs[perm[i]];
+  for (int i = 0; i < N; i++)
     for (int j = 0; j < i; j++) y[i] -= A[i][j] * y[j];
-  for (int i = 0; i < 6; i++) y[i] = (A[i][i] != 0.0) ? y[i] / A[i][i] : 0.0;
-  for (int i = 5; i >= 0; i--)
-    for (int j = i + 1; j < 6; j++) y[i] -= A[j][i] * y[j];
-  for (int i = 0; i < 6; i++) x[perm[i]] = y[i];
+  for (int i = 0; i < N; i++) y[i] = (A[i][i] != 0.0) ? y[i] / A[i][i] : 0.0;
+  for (int i = N - 1; i >= 0; i--)
+    for (int j = i + 1; j < N; j++) y[i] -= A[j][i] * y[j];
+  for (int i = 0; i < N; i++) x[perm[i]] = y[i];
 }
 
 // lsq_registration_impl.hpp:82-91

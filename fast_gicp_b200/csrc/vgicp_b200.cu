@@ -236,6 +236,19 @@ struct vgicp_context {
     uint64_t launches = 0;  // kernel nodes, counted as launches on every replay
     uint64_t prof_launches[VGICP_PROF_NUM_CATEGORIES] = {0};
   } s1;
+
+  // continuous-time registration (vgicp_set_source_timestamps, vgicp_compute_error_ct, vgicp_align_ct): the source's timestamps and
+  // buffers of its own for the evaluation, so that it leaves the single-pose state as it was; allocated at first use
+  bool ct_has_times = false;
+  float ct_tau = 0.0f;    // (float)t_ref
+  double ct_span = 0.0;   // S = max_i |t_i - tau| (float differences)
+  DevBuf<float> ct_times;
+  DevBuf<double> ct_partials;            // [kLinMaxBlocks][kCtStride]
+  unsigned int* d_ct_ticket = nullptr;
+  double* d_ct_out = nullptr;            // [kCtStride] (throughput hint)
+  double* h_ct_out = nullptr;            // pinned + mapped, same shape (latency hint: written by the kernel directly)
+  unsigned long long* h_ct_done = nullptr;  // pinned + mapped completion word
+  unsigned long long ct_seq = 0;
 };
 
 namespace {
@@ -316,6 +329,7 @@ int set_cloud(vgicp_handle h, Cloud& c, const float* xyz, size_t n, size_t strid
     nm.built = false;
     nm.pending = false;
   }
+  if (&c == &h->source) h->ct_has_times = false;  // the timestamps belong to the points they came with
   if (n > 0 && !xyz) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "set_cloud: null points");
   if (stride < 12 || (stride % 4) != 0) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "set_cloud: stride_bytes must be a multiple of 4 and >= 12");
   if (n > (size_t)0x7fffffff / 64) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "set_cloud: too many points");
@@ -673,7 +687,9 @@ struct LinLaunch {
   int G;        // compacted kernels: lanes per source point in the lookup phase
   int grid;     // blocks (per row of a multi-pose launch)
 };
-LinLaunch make_lin_launch(vgicp_handle h) {
+// allow_stream = false: the compacted kernels' shape also where DIRECT1 would stream (the continuous-time evaluation has no
+// streaming kernel)
+LinLaunch make_lin_launch(vgicp_handle h, bool allow_stream = true) {
   Cloud& s = h->source;
   VoxelMap& m = h->problem != 0 ? h->ndt_t : h->map;
   LinLaunch L;
@@ -707,7 +723,7 @@ LinLaunch make_lin_launch(vgicp_handle h) {
   const bool cols = h->offset_mode == 27;
   L.G = !wide ? 1 : (cols ? 3 : (n_off <= 7 ? 4 : 8));
   // DIRECT1 on a large cloud with the direct-mapped index: the bandwidth-bound shape, streamed through shared memory by bulk copies
-  L.stream = h->offset_mode == 1 && a.dense.cells != nullptr && a.n >= 65536 && (reinterpret_cast<uintptr_t>(a.covB) & 15) == 0;
+  L.stream = allow_stream && h->offset_mode == 1 && a.dense.cells != nullptr && a.n >= 65536 && (reinterpret_cast<uintptr_t>(a.covB) & 15) == 0;
   if (L.stream) {
     const int tiles = (a.n + kLinStreamTile - 1) / kLinStreamTile;
     L.grid = tiles < kLinStreamMaxBlocks ? tiles : kLinStreamMaxBlocks;
@@ -981,57 +997,115 @@ int multi_wait(vgicp_handle h, int n_rows, const double** rec) {
 // as a state machine that takes one evaluation record at a time, in host double arithmetic.  vgicp_align drives one with single-pose
 // launches, vgicp_align_multi many with shared multi-pose launches.  The lookup pose of every evaluation is the float image of x0
 // (x0 does not move between a linearisation and its trials); it is evaluated at x0 in phase kLmLinearize, at xi in phase kLmError.
+// N = 6: the pose (vgicp_align, vgicp_align_multi).  N = 12: the pose and the sweep's body twist (vgicp_align_ct): the evaluation
+// record is [err, H (12 x 12), b (12)] and a step d = [d_T; d_xi] moves T <- Exp(d_T) T, xi <- xi + d_xi.
+template <int N>
 struct LmState {
   vgicp_lsq_params p;
   Iso3d x0, xi, delta;  // estimate, LM trial pose, increment of the last step
-  double H[36], b[6], d[6], final_H[36];
+  double tw0[6], twi[6];  // N = 12: twist estimate, LM trial twist
+  double span;            // N = 12: S = max_i |s_i| (the sweep's reach from t_ref)
+  double H[N * N], b[N], d[N], final_H[N * N];
   double y0, lambda, nu;
   int phase;  // kLmLinearize: err, H, b at x0;  kLmError: err at xi over the correspondences of x0;  kLmDone
   int it, lm_j, converged, lm_failed, n_linearize, n_error, nr_iterations;
 };
 enum { kLmLinearize = 0, kLmError = 1, kLmDone = 2 };
 
-LmState lm_init(const double* guess, const vgicp_lsq_params& P) {
-  LmState st;
+template <int N>
+LmState<N> lm_init(const double* guess, const vgicp_lsq_params& P) {
+  LmState<N> st;
   memset(&st, 0, sizeof(st));
   st.p = P;
   memcpy(st.x0.m, guess, sizeof(st.x0.m));
-  for (int j = 0; j < 6; j++) st.final_H[j * 7] = 1.0;  // final_hessian_.setIdentity()
+  for (int j = 0; j < N; j++) st.final_H[j * (N + 1)] = 1.0;  // final_hessian_.setIdentity()
   st.lambda = -1.0;
   st.nu = 2.0;
   st.phase = P.max_iterations > 0 ? kLmLinearize : kLmDone;
   return st;
 }
 
-void lm_propose(LmState* st) {  // solve (H + lambda I) d = -b, delta = exp(d), xi = delta * x0   (:134-139)
-  double Hl[36], nb[6];
+// the rotation of a twist over the sweep, |omega| S, stays within the series of deskew_point
+bool twist_in_series(const double* xi, double span) { return sqrt(xi[0] * xi[0] + xi[1] * xi[1] + xi[2] * xi[2]) * span <= 1.5707963267948966; }
+
+// is_converged(delta) (:65-75); N = 12: and the step's motion of the sweep's end, Exp(S d_xi), as well
+template <int N>
+bool lm_step_converged(const LmState<N>& st) {
+  bool c = is_converged(st.delta, st.p.rotation_epsilon, st.p.transformation_epsilon);
+  if constexpr (N == 12) {
+    double sd[6];
+    for (int j = 0; j < 6; j++) sd[j] = st.span * st.d[6 + j];
+    c = c && is_converged(se3_exp(sd), st.p.rotation_epsilon, st.p.transformation_epsilon);
+  }
+  return c;
+}
+
+template <int N>
+void lm_reject(LmState<N>* st);
+
+template <int N>
+void lm_propose(LmState<N>* st) {  // solve (H + lambda I) d = -b, delta = exp(d), xi = delta * x0   (:134-139)
+  double Hl[N * N], nb[N];
   memcpy(Hl, st->H, sizeof(Hl));
-  for (int q = 0; q < 6; q++) { Hl[q * 7] += st->lambda; nb[q] = -st->b[q]; }
-  ldlt_solve6(Hl, nb, st->d);
+  for (int q = 0; q < N; q++) { Hl[q * (N + 1)] += st->lambda; nb[q] = -st->b[q]; }
+  ldlt_solve<N>(Hl, nb, st->d);
   st->delta = se3_exp(st->d);
   st->xi = iso_mul(st->delta, st->x0);
+  if constexpr (N == 12) {
+    for (int j = 0; j < 6; j++) st->twi[j] = st->tw0[j] + st->d[6 + j];
+    if (!twist_in_series(st->twi, st->span)) {  // outside the series: a rejected step, nothing to evaluate
+      lm_reject(st);
+      return;
+    }
+  }
   st->phase = kLmError;
 }
 
-void lm_finish_outer(LmState* st) {  // end of step_optimize: converged_ = is_converged(delta), next outer iteration (:65-75)
-  st->converged = is_converged(st->delta, st->p.rotation_epsilon, st->p.transformation_epsilon) ? 1 : 0;
+template <int N>
+void lm_finish_outer(LmState<N>* st) {  // end of step_optimize: converged_ = is_converged(delta), next outer iteration (:65-75)
+  st->converged = lm_step_converged(*st) ? 1 : 0;
   st->it++;
   if (st->converged || st->it >= st->p.max_iterations) { st->phase = kLmDone; return; }
   st->nr_iterations = st->it;
   st->phase = kLmLinearize;
 }
 
-void lm_advance(LmState* st, const double* out /*err, H, b*/) {
+template <int N>
+void lm_reject(LmState<N>* st) {  // a trial with rho < 0 (:151-159)
+  if (lm_step_converged(*st)) { lm_finish_outer(st); return; }  // :151-154
+  st->lambda = st->nu * st->lambda;
+  st->nu = 2 * st->nu;
+  st->lm_j++;
+  if (st->lm_j >= st->p.lm_max_iterations) {  // step_lm returns false -> "lm not converged!!" (:69-72)
+    st->lm_failed = 1;
+    st->phase = kLmDone;
+    return;
+  }
+  lm_propose(st);
+}
+
+template <int N>
+void lm_advance(LmState<N>* st, const double* out /*err, H, b*/) {
   if (st->phase == kLmLinearize) {
     st->y0 = out[0];
     memcpy(st->H, out + 1, sizeof(st->H));
-    memcpy(st->b, out + 37, sizeof(st->b));
+    memcpy(st->b, out + 1 + N * N, sizeof(st->b));
     st->n_linearize++;
     if (st->p.use_gauss_newton) {  // step_gn
-      double nb[6];
-      for (int q = 0; q < 6; q++) nb[q] = -st->b[q];
-      ldlt_solve6(st->H, nb, st->d);
+      double nb[N];
+      for (int q = 0; q < N; q++) nb[q] = -st->b[q];
+      ldlt_solve<N>(st->H, nb, st->d);
       st->delta = se3_exp(st->d);
+      if constexpr (N == 12) {
+        double tw[6];
+        for (int j = 0; j < 6; j++) tw[j] = st->tw0[j] + st->d[6 + j];
+        if (!twist_in_series(tw, st->span)) {  // a step outside the series cannot be taken: stop with the last estimate
+          st->lm_failed = 1;
+          st->phase = kLmDone;
+          return;
+        }
+        memcpy(st->tw0, tw, sizeof(tw));
+      }
       st->x0 = iso_mul(st->delta, st->x0);
       memcpy(st->final_H, st->H, sizeof(st->H));
       lm_finish_outer(st);
@@ -1039,7 +1113,7 @@ void lm_advance(LmState* st, const double* out /*err, H, b*/) {
     }
     if (st->lambda < 0.0) {  // :128-130
       double mx = 0.0;
-      for (int j = 0; j < 6; j++) mx = fmax(mx, fabs(st->H[j * 7]));
+      for (int j = 0; j < N; j++) mx = fmax(mx, fabs(st->H[j * (N + 1)]));
       st->lambda = st->p.lm_init_lambda_factor * mx;
     }
     st->nu = 2.0;
@@ -1056,22 +1130,14 @@ void lm_advance(LmState* st, const double* out /*err, H, b*/) {
   const double yi = out[0];
   st->n_error++;
   double den = 0.0;
-  for (int q = 0; q < 6; q++) den += st->d[q] * (st->lambda * st->d[q] - st->b[q]);
+  for (int q = 0; q < N; q++) den += st->d[q] * (st->lambda * st->d[q] - st->b[q]);
   const double rho = (st->y0 - yi) / den;
   if (rho < 0) {
-    if (is_converged(st->delta, st->p.rotation_epsilon, st->p.transformation_epsilon)) { lm_finish_outer(st); return; }  // :151-154
-    st->lambda = st->nu * st->lambda;
-    st->nu = 2 * st->nu;
-    st->lm_j++;
-    if (st->lm_j >= st->p.lm_max_iterations) {  // step_lm returns false -> "lm not converged!!" (:69-72)
-      st->lm_failed = 1;
-      st->phase = kLmDone;
-      return;
-    }
-    lm_propose(st);
+    lm_reject(st);
     return;
   }
   st->x0 = st->xi;  // :161-164
+  if constexpr (N == 12) memcpy(st->tw0, st->twi, sizeof(st->tw0));
   const double f = 1.0 - pow(2.0 * rho - 1.0, 3);
   st->lambda = st->lambda * fmax(1.0 / 3.0, f);
   memcpy(st->final_H, st->H, sizeof(st->H));
@@ -1081,7 +1147,7 @@ void lm_advance(LmState* st, const double* out /*err, H, b*/) {
 // Takes one evaluation record (the single-pose mailbox and a multi-pose row share the layout: err, H, b in [0..42], [43] the trial's
 // error over the current correspondences in a kEvalSpec record).  A speculative record's [43] decides the trial; when the trial is
 // accepted and the optimisation goes on, the linearisation at the trial pose in [0..42] is taken at once.  Returns true in that case.
-bool lm_consume(LmState* st, const double* rec, bool spec) {
+bool lm_consume(LmState<6>* st, const double* rec, bool spec) {
   if (!spec) {
     lm_advance(st, rec);
     return false;
@@ -1092,7 +1158,7 @@ bool lm_consume(LmState* st, const double* rec, bool spec) {
   return true;
 }
 
-void lm_result(const LmState& st, vgicp_align_result* res) {
+void lm_result(const LmState<6>& st, vgicp_align_result* res) {
   memset(res, 0, sizeof(*res));
   memcpy(res->T, st.x0.m, sizeof(res->T));
   memcpy(res->H, st.final_H, sizeof(res->H));
@@ -1101,6 +1167,139 @@ void lm_result(const LmState& st, vgicp_align_result* res) {
   res->n_linearize = st.n_linearize;
   res->n_compute_error = st.n_error;
   res->lm_failed = st.lm_failed;
+}
+
+// ---- continuous-time registration (vgicp_compute_error_ct, vgicp_align_ct) ------------------------------------------------------
+// VGICP on one GPU, with the source's timestamps and the preconditions of vgicp_align
+int ct_check(vgicp_handle h, const char* who) {
+  if (h->problem != 0) return fail(h, VGICP_ERR_UNSUPPORTED, std::string(who) + ": continuous-time registration is defined for the VGICP problem only");
+  if (h->comm_ranks > 1 || h->stage1_sharding || h->shard_end >= 0)
+    return fail(h, VGICP_ERR_UNSUPPORTED, std::string(who) + ": not available with source or stage-1 sharding or in a multi-GPU communicator");
+  if (!h->source.has_pts || !h->source.has_cov) return fail(h, VGICP_ERR_BAD_STATE, std::string(who) + ": source points and covariances required");
+  if (!h->map.built && !h->map.pending) return fail(h, VGICP_ERR_BAD_STATE, std::string(who) + ": target voxel map not built");
+  if (!h->ct_has_times) return fail(h, VGICP_ERR_BAD_STATE, std::string(who) + ": the source has no timestamps (vgicp_set_source_timestamps)");
+  return VGICP_OK;
+}
+
+bool all_finite(const double* v, int n, bool as_float) {
+  for (int j = 0; j < n; j++)
+    if (!(as_float ? std::isfinite((float)v[j]) : std::isfinite(v[j]))) return false;
+  return true;
+}
+
+// fixed-size buffers on first use
+int ct_reserve(vgicp_handle h) {
+  if (!h->h_ct_out) {
+    CU_TRY(h, cudaMalloc(&h->d_ct_ticket, sizeof(unsigned int)));
+    CU_TRY(h, cudaMemsetAsync(h->d_ct_ticket, 0, sizeof(unsigned int), h->stream));
+    CU_TRY(h, cudaMalloc(&h->d_ct_out, kCtStride * sizeof(double)));
+    CU_TRY(h, cudaHostAlloc(&h->h_ct_done, sizeof(unsigned long long), cudaHostAllocMapped));
+    *h->h_ct_done = 0;
+    CU_TRY(h, cudaHostAlloc(&h->h_ct_out, kCtStride * sizeof(double), cudaHostAllocMapped));  // (last: it marks the set as complete)
+  }
+  CU_TRY(h, h->ct_partials.reserve((size_t)kLinMaxBlocks * kCtStride));
+  return VGICP_OK;
+}
+
+// One evaluation at (Te, xe) over the correspondences of (Tl, xl): the compacted kernel and grid make_lin_launch picks (DIRECT1 on
+// large clouds included) with the CT flag.  *raw: kCtValues folded sums (want_H) or err alone, valid until the next one.
+int ct_evaluate(vgicp_handle h, const double* Tl, const double* xl, const double* Te, const double* xe, bool want_H, const double** raw) {
+  LinLaunch L = make_lin_launch(h, false);
+  LinArgs& a = L.a;
+  a.Tlin = to_pose(Tl);
+  a.Teval = to_pose(Te);
+  CtArgs c;
+  c.times = h->ct_times.p;
+  c.tau = h->ct_tau;
+  for (int j = 0; j < 6; j++) {
+    c.xl[j] = (float)xl[j];
+    c.xe[j] = (float)xe[j];
+  }
+  c.partials = h->ct_partials.p;
+  c.ticket = h->d_ct_ticket;
+  const bool direct = h->exec_hint == 0;
+  c.out = direct ? h->h_ct_out : h->d_ct_out;
+  c.done_flag = direct ? h->h_ct_done : nullptr;
+  c.done_seq = ++h->ct_seq;
+  prof_begin(h, want_H ? VGICP_PROF_LINEARIZE : VGICP_PROF_ERROR, h->stream);
+  const bool launched = with_lin_kernel(h->offset_mode, L.G, a.robust, [&](auto mode, auto g, auto rb) {
+    constexpr int MODE = decltype(mode)::value, G = decltype(g)::value;
+    constexpr bool RB = decltype(rb)::value;
+    if (want_H) k_linearize_ct<MODE, true, G, RB><<<L.grid, kLinThreads, 0, h->stream>>>(a, c);
+    else k_linearize_ct<MODE, false, G, RB><<<L.grid, kLinThreads, 0, h->stream>>>(a, c);
+  });
+  prof_end(h, h->stream);
+  if (!launched) return fail(h, VGICP_ERR_UNSUPPORTED, "no evaluation kernel for this offset table and lane split");
+  h->launches++;
+  CU_TRY(h, cudaGetLastError());
+  int rc = wait_records(h, h->h_ct_done, 1, h->ct_seq, h->h_ct_out, h->d_ct_out, want_H ? kCtValues : 1);
+  if (rc) return rc;
+  *raw = h->h_ct_out;
+  return VGICP_OK;
+}
+
+// the unique entries s[1..21] of a 6x6 block in apply_jacobian's order -> column-major 6x6 (lin_unpack's mapping)
+void ct_unpack6(const double* s, double* H) {
+  auto set = [&](int r, int c, double v) { H[c * 6 + r] = v; H[r * 6 + c] = v; };
+  set(0, 0, s[1]); set(0, 1, s[2]); set(0, 2, s[3]); set(1, 1, s[4]); set(1, 2, s[5]); set(2, 2, s[6]);
+  for (int r = 0; r < 3; r++)
+    for (int c = 0; c < 3; c++) set(r, 3 + c, s[7 + r * 3 + c]);
+  set(3, 3, s[16]); set(3, 4, s[17]); set(3, 5, s[18]); set(4, 4, s[19]); set(4, 5, s[20]); set(5, 5, s[21]);
+}
+
+// The 12 x 12 system (column-major) and b12 from the raw sums at T_eval:  H = [[H0, H1 K], [K^T H1, K^T H2 K]], b = [b0; K^T b1],
+// K = [[R, 0], [[t]x R, R]] with (R, t) the float image of T_eval (include/vgicp_b200.h)
+void ct_system(const double* raw, const double* Teval, double* H144, double* b12) {
+  double H0[36], H1[36], H2[36], K[36] = {0};
+  ct_unpack6(raw, H0);
+  ct_unpack6(raw + 27, H1);
+  ct_unpack6(raw + 54, H2);
+  const double* b0 = raw + 22;
+  const double* b1 = raw + 49;
+  const Pose P = to_pose(Teval);
+  double R[3][3], tx[3][3];
+  for (int r = 0; r < 3; r++)
+    for (int c = 0; c < 3; c++) R[r][c] = (double)P.r[r * 3 + c];
+  const double t0 = P.t[0], t1 = P.t[1], t2 = P.t[2];
+  const double S[3][3] = {{0.0, -t2, t1}, {t2, 0.0, -t0}, {-t1, t0, 0.0}};
+  for (int r = 0; r < 3; r++)
+    for (int c = 0; c < 3; c++) tx[r][c] = S[r][0] * R[0][c] + S[r][1] * R[1][c] + S[r][2] * R[2][c];
+  for (int r = 0; r < 3; r++)
+    for (int c = 0; c < 3; c++) {
+      K[c * 6 + r] = R[r][c];
+      K[(3 + c) * 6 + 3 + r] = R[r][c];
+      K[c * 6 + 3 + r] = tx[r][c];
+    }
+  double H1K[36], H2K[36];  // column-major products
+  for (int r = 0; r < 6; r++)
+    for (int c = 0; c < 6; c++) {
+      double u = 0.0, v = 0.0;
+      for (int k = 0; k < 6; k++) {
+        u += H1[k * 6 + r] * K[c * 6 + k];
+        v += H2[k * 6 + r] * K[c * 6 + k];
+      }
+      H1K[c * 6 + r] = u;
+      H2K[c * 6 + r] = v;
+    }
+  for (int r = 0; r < 6; r++)
+    for (int c = 0; c < 6; c++) {
+      H144[c * 12 + r] = H0[c * 6 + r];
+      H144[(6 + c) * 12 + r] = H1K[c * 6 + r];
+      H144[c * 12 + 6 + r] = H1K[r * 6 + c];
+    }
+  for (int r = 0; r < 6; r++)
+    for (int c = r; c < 6; c++) {  // K^T H2 K, symmetric by construction
+      double v = 0.0;
+      for (int k = 0; k < 6; k++) v += K[r * 6 + k] * H2K[c * 6 + k];
+      H144[(6 + c) * 12 + 6 + r] = v;
+      H144[(6 + r) * 12 + 6 + c] = v;
+    }
+  for (int r = 0; r < 6; r++) {
+    b12[r] = b0[r];
+    double v = 0.0;
+    for (int k = 0; k < 6; k++) v += K[r * 6 + k] * b1[k];
+    b12[6 + r] = v;
+  }
 }
 
 }  // namespace
@@ -1195,6 +1394,12 @@ int vgicp_destroy(vgicp_handle h) {
   if (h->d_multi_out) cudaFree(h->d_multi_out);
   if (h->h_multi_out) cudaFreeHost(h->h_multi_out);
   if (h->h_multi_done) cudaFreeHost(h->h_multi_done);
+  h->ct_times.release();
+  h->ct_partials.release();
+  if (h->d_ct_ticket) cudaFree(h->d_ct_ticket);
+  if (h->d_ct_out) cudaFree(h->d_ct_out);
+  if (h->h_ct_out) cudaFreeHost(h->h_ct_out);
+  if (h->h_ct_done) cudaFreeHost(h->h_ct_done);
   for (auto& r : h->prof_pending) { cudaEventDestroy(r.a); cudaEventDestroy(r.b); }
   for (auto e : h->prof_pool) cudaEventDestroy(e);
   for (cudaEvent_t e : {h->ev_copy, h->ev_append, h->ev_deskew, h->target.ready, h->source.ready})
@@ -1307,6 +1512,7 @@ int vgicp_swap_source_and_target(vgicp_handle h) {  // fast_vgicp_cuda.cu:97-107
   CU_TRY(h, cudaStreamSynchronize(h->stream));
   CU_TRY(h, cudaStreamSynchronize(h->stream_b));
   std::swap(h->source, h->target);
+  h->ct_has_times = false;
   h->map.built = false;
   h->map.pending = false;
   // NDT: the reference swaps its two maps (ndt_cuda.cu:90-93); a map that does not exist (P2D never builds the source's) is built by
@@ -1588,7 +1794,7 @@ int vgicp_align(vgicp_handle h, const double guess[16], const vgicp_lsq_params* 
   }
   { int rc = sync_inputs(h); if (rc) return rc; }
   const bool speculate = h->speculate != 0 && !P.use_gauss_newton;
-  LmState st = lm_init(guess, P);
+  LmState<6> st = lm_init<6>(guess, P);
   while (st.phase != kLmDone) {
     const bool lin = st.phase == kLmLinearize;
     const Pose Teval = to_pose(lin ? st.x0.m : st.xi.m);
@@ -1622,8 +1828,8 @@ int vgicp_align_multi(vgicp_handle h, const double* guesses, int n_guesses, cons
   const int B = n_guesses;
   const LinLaunch L = make_lin_launch(h);
   if ((rc = multi_reserve(h, B, L.grid))) return rc;
-  std::vector<LmState> st(B);
-  for (int i = 0; i < B; i++) st[i] = lm_init(guesses + 16 * i, P);
+  std::vector<LmState<6>> st(B);
+  for (int i = 0; i < B; i++) st[i] = lm_init<6>(guesses + 16 * i, P);
   const bool speculate = h->speculate != 0 && !P.use_gauss_newton;
   for (;;) {
     Pose* poses = multi_poses(h);
@@ -1971,34 +2177,49 @@ int vgicp_crop_target(vgicp_handle h, const double center[3], double radius, siz
 }
 
 // ---- motion compensation: deskew the source from per-point timestamps and a constant body twist ----
-int vgicp_deskew_source(vgicp_handle h, const float* t, size_t n, size_t stride_bytes, const double twist[6], double t_ref) {
-  CHECK_HANDLE(h);
-  DeviceGuard g(h->device);
-  if (n > 0 && (!t || !twist)) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "deskew_source: null timestamps or twist");
-  if (stride_bytes < 4 || (stride_bytes % 4) != 0) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "deskew_source: stride_bytes must be a multiple of 4 and >= 4");
-  Cloud& s = h->source;
-  if (!s.has_pts || s.n == 0) return fail(h, VGICP_ERR_BAD_STATE, "deskew_source: no source points");
-  if (n != (size_t)s.n) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "deskew_source: the number of timestamps differs from the number of source points");
-  // the kernel takes every value as a float: a value finite in double but not in float is rejected too
-  const float tau = (float)t_ref;
-  float xi[6];
-  for (int j = 0; j < 6; j++) xi[j] = (float)twist[j];
-  if (!std::isfinite(tau)) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "deskew_source: non-finite t_ref");
-  for (int j = 0; j < 6; j++)
-    if (!std::isfinite(xi[j])) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "deskew_source: non-finite twist");
-  // one pass over the caller's strided array: validate, find the time range, pack contiguously
-  std::vector<float>& packed = h->deskew_times;
+// The checks of a timestamp array that come before the values: stride, a source to match, its size, a t_ref finite as a float
+static int timestamps_check(vgicp_handle h, const char* who, size_t n, size_t stride_bytes, double t_ref) {
+  if (stride_bytes < 4 || (stride_bytes % 4) != 0) return fail(h, VGICP_ERR_INVALID_ARGUMENT, std::string(who) + ": stride_bytes must be a multiple of 4 and >= 4");
+  const Cloud& s = h->source;
+  if (!s.has_pts || s.n == 0) return fail(h, VGICP_ERR_BAD_STATE, std::string(who) + ": no source points");
+  if (n != (size_t)s.n) return fail(h, VGICP_ERR_INVALID_ARGUMENT, std::string(who) + ": the number of timestamps differs from the number of source points");
+  // the kernels take every value as a float: a value finite in double but not in float is rejected too
+  if (!std::isfinite((float)t_ref)) return fail(h, VGICP_ERR_INVALID_ARGUMENT, std::string(who) + ": non-finite t_ref");
+  return VGICP_OK;
+}
+// one pass over the caller's strided array: validate, find the time range, pack contiguously into `packed`
+static int timestamps_pack(vgicp_handle h, const char* who, const float* t, size_t n, size_t stride_bytes, std::vector<float>& packed, float* lo_out, float* hi_out) {
   packed.resize(n);
   const unsigned char* raw = reinterpret_cast<const unsigned char*>(t);
   float lo = 0.0f, hi = 0.0f;
   for (size_t i = 0; i < n; i++) {
     float v;
     memcpy(&v, raw + i * stride_bytes, sizeof(float));
-    if (!std::isfinite(v)) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "deskew_source: non-finite timestamp");
+    if (!std::isfinite(v)) return fail(h, VGICP_ERR_INVALID_ARGUMENT, std::string(who) + ": non-finite timestamp");
     if (i == 0 || v < lo) lo = v;
     if (i == 0 || v > hi) hi = v;
     packed[i] = v;
   }
+  *lo_out = lo;
+  *hi_out = hi;
+  return VGICP_OK;
+}
+
+int vgicp_deskew_source(vgicp_handle h, const float* t, size_t n, size_t stride_bytes, const double twist[6], double t_ref) {
+  CHECK_HANDLE(h);
+  DeviceGuard g(h->device);
+  if (n > 0 && (!t || !twist)) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "deskew_source: null timestamps or twist");
+  int rc = timestamps_check(h, "deskew_source", n, stride_bytes, t_ref);
+  if (rc) return rc;
+  Cloud& s = h->source;
+  const float tau = (float)t_ref;
+  float xi[6];
+  for (int j = 0; j < 6; j++) xi[j] = (float)twist[j];
+  for (int j = 0; j < 6; j++)
+    if (!std::isfinite(xi[j])) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "deskew_source: non-finite twist");
+  std::vector<float>& packed = h->deskew_times;
+  float lo = 0.0f, hi = 0.0f;
+  if ((rc = timestamps_pack(h, "deskew_source", t, n, stride_bytes, packed, &lo, &hi))) return rc;
   const double span = fmax(fabs((double)lo - t_ref), fabs((double)hi - t_ref));
   const double omega = sqrt(twist[0] * twist[0] + twist[1] * twist[1] + twist[2] * twist[2]);
   if (omega * span > 1.5707963267948966)
@@ -2025,6 +2246,104 @@ int vgicp_deskew_source(vgicp_handle h, const float* t, size_t n, size_t stride_
   h->ndt_s.pending = false;
   // the packed timestamps are reused by the next call: the copy out of them must have landed
   CU_TRY(h, cudaEventSynchronize(h->ev_copy));
+  return VGICP_OK;
+}
+
+// ---- continuous-time registration: the sweep's body twist estimated with the pose from per-point timestamps ----
+int vgicp_set_source_timestamps(vgicp_handle h, const float* t, size_t n, size_t stride_bytes, double t_ref) {
+  CHECK_HANDLE(h);
+  DeviceGuard g(h->device);
+  if (n > 0 && !t) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "set_source_timestamps: null timestamps");
+  int rc = timestamps_check(h, "set_source_timestamps", n, stride_bytes, t_ref);
+  if (rc) return rc;
+  std::vector<float> packed;
+  float lo = 0.0f, hi = 0.0f;
+  if ((rc = timestamps_pack(h, "set_source_timestamps", t, n, stride_bytes, packed, &lo, &hi))) return rc;
+  const float tau = (float)t_ref;
+  // S = max |t_i - tau| over the float differences the kernels form (a float subtraction is monotonic in t_i)
+  const double span = fmax(fabs((double)(lo - tau)), fabs((double)(hi - tau)));
+  if (!std::isfinite(span)) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "set_source_timestamps: t_i - t_ref overflows a float");
+  CU_TRY(h, h->ct_times.reserve(n));
+  CU_TRY(h, cudaMemcpyAsync(h->ct_times.p, packed.data(), n * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+  CU_TRY(h, cudaStreamSynchronize(h->stream));  // (`packed` goes out of scope)
+  h->ct_has_times = true;
+  h->ct_tau = tau;
+  h->ct_span = span;
+  return VGICP_OK;
+}
+
+int vgicp_compute_error_ct(vgicp_handle h, const double T_lin[16], const double xi_lin[6], const double T_eval[16], const double xi_eval[6], double* H144, double* b12,
+                           double* err) {
+  CHECK_HANDLE(h);
+  DeviceGuard g(h->device);
+  if (!T_lin || !xi_lin || !T_eval || !xi_eval || (H144 == nullptr) != (b12 == nullptr))
+    return fail(h, VGICP_ERR_INVALID_ARGUMENT, "compute_error_ct: null pose or twist, or H144 without b12 (or b12 without H144)");
+  if (!all_finite(T_lin, 16, false) || !all_finite(T_eval, 16, false) || !all_finite(xi_lin, 6, true) || !all_finite(xi_eval, 6, true))
+    return fail(h, VGICP_ERR_INVALID_ARGUMENT, "compute_error_ct: non-finite pose or twist");
+  int rc = ct_check(h, "compute_error_ct");
+  if (rc) return rc;
+  if (!twist_in_series(xi_lin, h->ct_span) || !twist_in_series(xi_eval, h->ct_span))
+    return fail(h, VGICP_ERR_INVALID_ARGUMENT, "compute_error_ct: the rotation over the sweep (|omega| * max |s_i|) exceeds pi/2, beyond the series");
+  if ((rc = sync_inputs(h))) return rc;
+  if ((rc = ct_reserve(h))) return rc;
+  const bool want_H = H144 != nullptr;
+  const double* raw = nullptr;
+  if ((rc = ct_evaluate(h, T_lin, xi_lin, T_eval, xi_eval, want_H, &raw))) return rc;
+  if (err) *err = raw[0];
+  if (want_H) ct_system(raw, T_eval, H144, b12);
+  return VGICP_OK;
+}
+
+// vgicp_align's state machine with N = 12: every evaluation looks the voxels up at (x0, tw0) and evaluates at (x0, tw0) (linearise)
+// or at the trial (xi, twi) (error only); the prior is added on the host
+int vgicp_align_ct(vgicp_handle h, const double guess[16], const double twist_guess[6], const double twist_prior[6], const double twist_weight[6],
+                   const vgicp_lsq_params* params, vgicp_align_ct_result* res) {
+  CHECK_HANDLE(h);
+  DeviceGuard g(h->device);
+  if (!guess || !twist_guess || !twist_prior || !twist_weight || !res) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "align_ct: null argument");
+  if (!all_finite(guess, 16, false) || !all_finite(twist_guess, 6, true) || !all_finite(twist_prior, 6, false))
+    return fail(h, VGICP_ERR_INVALID_ARGUMENT, "align_ct: non-finite guess, twist guess or prior");
+  for (int j = 0; j < 6; j++)
+    if (!(twist_weight[j] > 0.0 && std::isfinite(twist_weight[j]))) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "align_ct: every twist weight must be finite and > 0");
+  int rc = ct_check(h, "align_ct");
+  if (rc) return rc;
+  if (!twist_in_series(twist_guess, h->ct_span) || !twist_in_series(twist_prior, h->ct_span))
+    return fail(h, VGICP_ERR_INVALID_ARGUMENT, "align_ct: the twist guess or prior rotates more than pi/2 over the sweep (|omega| * max |s_i|), beyond the series");
+  vgicp_lsq_params P;
+  if (params) P = *params; else vgicp_lsq_default_params(&P);
+  if ((rc = sync_inputs(h))) return rc;
+  if ((rc = ct_reserve(h))) return rc;
+  LmState<12> st = lm_init<12>(guess, P);
+  memcpy(st.tw0, twist_guess, sizeof(st.tw0));
+  st.span = h->ct_span;
+  double rec[1 + 144 + 12];
+  while (st.phase != kLmDone) {
+    const bool lin = st.phase == kLmLinearize;
+    const double* Te = lin ? st.x0.m : st.xi.m;
+    const double* xe = lin ? st.tw0 : st.twi;
+    const double* raw = nullptr;
+    if ((rc = ct_evaluate(h, st.x0.m, st.tw0, Te, xe, lin, &raw))) return rc;
+    double prior = 0.0;
+    for (int j = 0; j < 6; j++) prior += twist_weight[j] * (xe[j] - twist_prior[j]) * (xe[j] - twist_prior[j]);
+    rec[0] = raw[0] + prior;
+    if (lin) {
+      ct_system(raw, Te, rec + 1, rec + 145);
+      for (int j = 0; j < 6; j++) {
+        rec[1 + (6 + j) * 13] += twist_weight[j];
+        rec[145 + 6 + j] += twist_weight[j] * (xe[j] - twist_prior[j]);
+      }
+    }
+    lm_advance(&st, rec);
+  }
+  memset(res, 0, sizeof(*res));
+  memcpy(res->T, st.x0.m, sizeof(res->T));
+  memcpy(res->twist, st.tw0, sizeof(res->twist));
+  memcpy(res->H, st.final_H, sizeof(res->H));
+  res->nr_iterations = st.nr_iterations;
+  res->converged = st.converged;
+  res->n_linearize = st.n_linearize;
+  res->n_compute_error = st.n_error;
+  res->lm_failed = st.lm_failed;
   return VGICP_OK;
 }
 

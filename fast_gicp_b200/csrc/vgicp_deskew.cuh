@@ -17,12 +17,9 @@ __device__ __forceinline__ float horner_step(float h, float q, float c) { return
 //   p'_j = ((R_j0 p0 + R_j1 p1) + R_j2 p2) + ((V_j0 u0 + V_j1 u1) + V_j2 u2).
 // The coefficients are the float32 roundings of the series' coefficients; A keeps 7 terms, B and C 6, which keeps the truncation
 // below 2^-24 relative for theta <= pi/2 (the host rejects larger rotations).
-__global__ void k_deskew_points(float4* __restrict__ pts, const float* __restrict__ times, int n, float t_ref, float o0, float o1, float o2, float n0, float n1,
-                                float n2) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const float4 p = pts[i];
-  const float s = __fsub_rn(times[i], t_ref);
+// One point: Exp(s xi) p.  Shared by k_deskew_points and the continuous-time evaluation kernels (vgicp_kernels.cuh), which
+// must place a point exactly where vgicp_deskew_source would store it.
+__device__ __forceinline__ float3 deskew_point(float4 p, float s, float o0, float o1, float o2, float n0, float n1, float n2) {
   const float w[3] = {__fmul_rn(s, o0), __fmul_rn(s, o1), __fmul_rn(s, o2)};
   const float u[3] = {__fmul_rn(s, n0), __fmul_rn(s, n1), __fmul_rn(s, n2)};
   const float q = __fadd_rn(__fadd_rn(__fmul_rn(w[0], w[0]), __fmul_rn(w[1], w[1])), __fmul_rn(w[2], w[2]));
@@ -62,7 +59,17 @@ __global__ void k_deskew_points(float4* __restrict__ pts, const float* __restric
     const float vu = __fadd_rn(__fadd_rn(__fmul_rn(V[0], u[0]), __fmul_rn(V[1], u[1])), __fmul_rn(V[2], u[2]));
     out[j] = __fadd_rn(rp, vu);
   }
-  pts[i] = make_float4(out[0], out[1], out[2], 0.0f);
+  return make_float3(out[0], out[1], out[2]);
+}
+
+__global__ void k_deskew_points(float4* __restrict__ pts, const float* __restrict__ times, int n, float t_ref, float o0, float o1, float o2, float n0, float n1,
+                                float n2) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float4 p = pts[i];
+  const float s = __fsub_rn(times[i], t_ref);
+  const float3 q = deskew_point(p, s, o0, o1, o2, n0, n1, n2);
+  pts[i] = make_float4(q.x, q.y, q.z, 0.0f);
 }
 
 }  // namespace vgicp

@@ -20,6 +20,9 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
+#include "vgicp_deskew.cuh"
 #include "vgicp_sort.cuh"
 #include "vgicp_stage1.cuh"
 
@@ -29,6 +32,9 @@ constexpr int kLinThreads = 128;     // block size of the linearize kernel
 constexpr int kLinMaxBlocks = 4 * kNumSMs;  // 4 blocks per SM: upper bound on partial sums the last block has to fold (more resident warps only thrash L1: measured)
 constexpr int kLinValues = 28;       // 21 unique H + 6 b + 1 err
 constexpr int kLinStride = 32;       // row length of the partial-sum arrays (the speculative evaluation carries 29 values)
+// continuous-time evaluation (k_linearize_ct): the 28 sums above, then 21 H + 6 b weighted by s_i, then 21 H weighted by s_i^2
+constexpr int kCtValues = 76;
+constexpr int kCtStride = 80;        // row length of its partial-sum array
 constexpr int kLinOutCommError = 44; // out[44]: 1.0 when a sharded evaluation timed out waiting for a peer (the sums are then incomplete)
 
 struct Pose {      // float image of an Eigen::Isometry3f: R row-major here, t
@@ -449,6 +455,20 @@ struct LinArgs {
   float robust_d2;
 };
 
+// Continuous-time evaluation (vgicp_compute_error_ct / vgicp_align_ct): source point i is first moved to q_i = Exp(s_i xi) a_i,
+// s_i = times[i] - tau (deskew_point), with xi_lin for the voxel lookup under Tlin and xi_eval for the residual at Teval.  A kernel
+// argument of its own, so that the parameter block of every other evaluation kernel is unchanged.
+struct CtArgs {
+  const float* times;
+  float tau;
+  float xl[6], xe[6];      // xi_lin, xi_eval: rotation first, cast to float
+  double* partials;        // [gridDim.x][kCtStride]
+  unsigned int* ticket;    // zero before the first launch; reset by the last block
+  double* out;             // [kCtValues] raw folded sums; may be mapped pinned host memory
+  volatile unsigned long long* done_flag;  // optional (mapped host memory): set to done_seq once `out` is complete
+  unsigned long long done_seq;
+};
+
 __device__ __forceinline__ int lookup_voxel(const int4* __restrict__ buckets, unsigned mask, int max_scan, uint64_t h, int cx, int cy, int cz) {
   unsigned pos = (unsigned)(h & mask);
   for (int s = 0; s < max_scan; s++) {
@@ -588,10 +608,20 @@ __device__ __forceinline__ int3 fixed_offset(int o) {
 
 // J = [skew(pe) | -I] applied to one correspondence's  wM (symmetric-packed), wMe and w e^T M e, added to the lane's 28 running sums:
 //   B = S*wM (3x3), A = -B*S, with S = skew(pe);  H = [[A, B],[B^T, wM]],  b = [-(pe x wMe); -wMe]
-template <bool WANT_H>
-__device__ __forceinline__ void apply_jacobian(float3 pe, const PointAcc<WANT_H>& acc, float* sum) {
+// CT (continuous time): every H and b term k (1..27) is also added to sum[27 + k] weighted by the point's s, and every H term
+// (1..21) to sum[54 + k] weighted by s^2, after the plain sum: sums 0..27 are formed exactly as without CT.
+template <bool WANT_H, bool CT = false>
+__device__ __forceinline__ void apply_jacobian(float3 pe, const PointAcc<WANT_H>& acc, float* sum, float s = 0.0f) {
   sum[0] += acc.err;
   if (WANT_H) {
+    const float s2 = s * s;
+    auto add = [&](int k, float t) {
+      sum[k] += t;
+      if (CT) {
+        sum[27 + k] += s * t;
+        if (k <= 21) sum[54 + k] += s2 * t;
+      }
+    };
     const float* M = acc.m;  // xx xy xz yy yz zz
     float Mf[9] = {M[0], M[1], M[2], M[1], M[3], M[4], M[2], M[4], M[5]};
     float B[9];
@@ -602,20 +632,20 @@ __device__ __forceinline__ void apply_jacobian(float3 pe, const PointAcc<WANT_H>
       B[2 * 3 + j] = pe.x * Mf[1 * 3 + j] - pe.y * Mf[0 * 3 + j];
     }
     // (B*S)[i][0] = B[i][1]*pz - B[i][2]*py ; [i][1] = -B[i][0]*pz + B[i][2]*px ; [i][2] = B[i][0]*py - B[i][1]*px
-    sum[1] += -(B[1] * pe.z - B[2] * pe.y);
-    sum[2] += -(-B[0] * pe.z + B[2] * pe.x);
-    sum[3] += -(B[0] * pe.y - B[1] * pe.x);
-    sum[4] += -(-B[3] * pe.z + B[5] * pe.x);
-    sum[5] += -(B[3] * pe.y - B[4] * pe.x);
-    sum[6] += -(B[6] * pe.y - B[7] * pe.x);
+    add(1, -(B[1] * pe.z - B[2] * pe.y));
+    add(2, -(-B[0] * pe.z + B[2] * pe.x));
+    add(3, -(B[0] * pe.y - B[1] * pe.x));
+    add(4, -(-B[3] * pe.z + B[5] * pe.x));
+    add(5, -(B[3] * pe.y - B[4] * pe.x));
+    add(6, -(B[6] * pe.y - B[7] * pe.x));
 #pragma unroll
-    for (int j = 0; j < 9; j++) sum[7 + j] += B[j];
+    for (int j = 0; j < 9; j++) add(7 + j, B[j]);
 #pragma unroll
-    for (int j = 0; j < 6; j++) sum[16 + j] += M[j];
-    sum[22] += -(pe.y * acc.v[2] - pe.z * acc.v[1]);
-    sum[23] += -(pe.z * acc.v[0] - pe.x * acc.v[2]);
-    sum[24] += -(pe.x * acc.v[1] - pe.y * acc.v[0]);
-    sum[25] += -acc.v[0]; sum[26] += -acc.v[1]; sum[27] += -acc.v[2];
+    for (int j = 0; j < 6; j++) add(16 + j, M[j]);
+    add(22, -(pe.y * acc.v[2] - pe.z * acc.v[1]));
+    add(23, -(pe.z * acc.v[0] - pe.x * acc.v[2]));
+    add(24, -(pe.x * acc.v[1] - pe.y * acc.v[0]));
+    add(25, -acc.v[0]); add(26, -acc.v[1]); add(27, -acc.v[2]);
   }
 }
 
@@ -626,10 +656,15 @@ struct LinWarpStage {
   float rcr[6][32];   // R C_A R^T, symmetric-packed
   int queue[kLinQueue];
 };
+struct LinWarpStageCt : LinWarpStage {
+  float s[32];        // s_i = t_i - tau of the warp's current points
+};
+template <bool CT>
+using LinStage = std::conditional_t<CT, LinWarpStageCt, LinWarpStage>;
 
 // one correspondence from the queue: entry = slot << 27 | voxel id
-template <bool WANT_H, bool RB>
-__device__ __forceinline__ void lin_process_hit(const LinArgs& a, const LinWarpStage& st, int entry, float* sum) {
+template <bool WANT_H, bool RB, bool CT = false>
+__device__ __forceinline__ void lin_process_hit(const LinArgs& a, const LinStage<CT>& st, int entry, float* sum) {
   const int slot = (int)((unsigned)entry >> 27), id = entry & 0x7ffffff;
   const float4* vr = reinterpret_cast<const float4*>(a.vox + id);
   const float4 mn = __ldg(vr), c0 = __ldg(vr + 1), c1 = __ldg(vr + 2);
@@ -643,7 +678,8 @@ __device__ __forceinline__ void lin_process_hit(const LinArgs& a, const LinWarpS
   acc.v[0] = acc.v[1] = acc.v[2] = 0.f;
   acc.err = 0.f;
   accumulate_voxel<WANT_H, RB>(mn, c0, c1, true, rcr, pe, acc, a.ndt, a.res, a.robust, a.robust_d2);
-  apply_jacobian<WANT_H>(pe, acc, sum);
+  if constexpr (CT) apply_jacobian<WANT_H, true>(pe, acc, sum, st.s[slot]);
+  else apply_jacobian<WANT_H>(pe, acc, sum);
 }
 
 // MODE: 0 = offsets from memory (DIRECT_RADIUS or anything), 1 / 7 / 27 = the reference's fixed tables.
@@ -656,23 +692,26 @@ __device__ __forceinline__ void lin_process_hit(const LinArgs& a, const LinWarpS
 // The per-point terms (evaluation-pose point, R C_A R^T) are computed once per point and staged in shared memory.
 // The running sums are per lane over whatever correspondences the lane drew: the total is a sum over all of them anyway,
 // and the assignment depends only on the data, so the result is reproducible run to run.
-__device__ __forceinline__ LinWarpStage& lin_stage() {
-  __shared__ LinWarpStage stage[kLinThreads / 32];
+template <bool CT = false>
+__device__ __forceinline__ LinStage<CT>& lin_stage() {
+  __shared__ LinStage<CT> stage[kLinThreads / 32];
   return stage[threadIdx.x >> 5];
 }
 
 // COUNT: sum[NV] also counts the (source point, voxel) hits under Tl -- the length of the reference's correspondence list;
-// RB: robust kernel (accumulate_voxel)
-template <int MODE, bool WANT_H, int G, bool DENSE, bool COUNT, bool RB>
-__device__ __forceinline__ void lin_accumulate_impl(const LinArgs& a, const Pose& Tl, const Pose& Te, float* sum) {
-  constexpr int NV = WANT_H ? kLinValues : 1;
+// RB: robust kernel (accumulate_voxel); CT: continuous time (CtArgs): the point is deskewed with xi_lin for the lookup and with
+// xi_eval for the residual, and with WANT_H the sums run to kCtValues (apply_jacobian).  Compile-time flags, not runtime branches:
+// a runtime branch moved the register allocation of the other kernels.
+template <int MODE, bool WANT_H, int G, bool DENSE, bool COUNT, bool RB, bool CT = false>
+__device__ __forceinline__ void lin_accumulate_impl(const LinArgs& a, const Pose& Tl, const Pose& Te, float* sum, const CtArgs* ct = nullptr) {
+  constexpr int NV = WANT_H ? (CT ? kCtValues : kLinValues) : 1;
   constexpr int NOFF = MODE == 0 ? 0 : MODE;
   // MODE 27: a lane walks whole z-columns (3 cells sharing the x,y hash prefix) of a contiguous run of 27/G cells, G in {1, 3, 9}
   constexpr bool COLUMNS = (MODE == 27);
   static_assert(MODE != 27 || G == 1 || G == 3 || G == 9, "DIRECT27 splits its 9 z-columns over 1, 3 or 9 lanes");
   constexpr int CELLS = COLUMNS ? 3 : (MODE == 0 ? 4 : ((NOFF + G - 1) / G < 4 ? (NOFF + G - 1) / G : 4));  // cells per lane per pass (loads in flight)
   constexpr int TPW = (32 / G) * G;  // (point, lane) tasks per warp: whole points only (30 of 32 lanes at G = 3, 27 at G = 9)
-  LinWarpStage& st = lin_stage();
+  LinStage<CT>& st = lin_stage<CT>();
   const int lane = threadIdx.x & 31;
   const unsigned lt_mask = (1u << lane) - 1u;
 #pragma unroll
@@ -690,12 +729,27 @@ __device__ __forceinline__ void lin_accumulate_impl(const LinArgs& a, const Pose
     const int sub = (int)(task % G);
     const int slot = (lane / G) & 31;
     const float4 p = a.pts[i];
-    const float3 pl = transform_point(Tl, p.x, p.y, p.z);
+    float s = 0.0f;
+    float3 pl;
+    if constexpr (CT) {
+      s = __fsub_rn(__ldg(&ct->times[i]), ct->tau);
+      const float3 q = deskew_point(p, s, ct->xl[0], ct->xl[1], ct->xl[2], ct->xl[3], ct->xl[4], ct->xl[5]);
+      pl = transform_point(Tl, q.x, q.y, q.z);
+    } else {
+      pl = transform_point(Tl, p.x, p.y, p.z);
+    }
     __syncwarp();  // the previous set's hits are all consumed before its staging is overwritten
     if (sub == 0) {
       const float4 ca = a.covA[i];
       const float2 cb = a.covB[i];
-      const float3 pe = transform_point(Te, p.x, p.y, p.z);
+      float3 pe;
+      if constexpr (CT) {
+        const float3 q = deskew_point(p, s, ct->xe[0], ct->xe[1], ct->xe[2], ct->xe[3], ct->xe[4], ct->xe[5]);
+        pe = transform_point(Te, q.x, q.y, q.z);
+        st.s[slot] = s;
+      } else {
+        pe = transform_point(Te, p.x, p.y, p.z);
+      }
       st.pe[0][slot] = pe.x; st.pe[1][slot] = pe.y; st.pe[2][slot] = pe.z;
       // RCR = R_lin C_A R_lin^T  (compute_derivatives.cu:75), symmetric-packed
       const float* R = Tl.r;
@@ -784,20 +838,20 @@ __device__ __forceinline__ void lin_accumulate_impl(const LinArgs& a, const Pose
       }
       __syncwarp();
       while (tail - head >= 32u) {  // full batches: one correspondence per lane
-        lin_process_hit<WANT_H, RB>(a, st, st.queue[(head + lane) & (kLinQueue - 1)], sum);
+        lin_process_hit<WANT_H, RB, CT>(a, st, st.queue[(head + lane) & (kLinQueue - 1)], sum);
         head += 32u;
       }
     }
     if (tail != head) {  // the set's last, partial batch
-      if (lane < (int)(tail - head)) lin_process_hit<WANT_H, RB>(a, st, st.queue[(head + lane) & (kLinQueue - 1)], sum);
+      if (lane < (int)(tail - head)) lin_process_hit<WANT_H, RB, CT>(a, st, st.queue[(head + lane) & (kLinQueue - 1)], sum);
     }
   }
 }
 
-template <int MODE, bool WANT_H, int G, bool COUNT, bool RB>
-__device__ __forceinline__ void lin_accumulate(const LinArgs& a, const Pose& Tl, const Pose& Te, float* sum) {
-  if (a.dense.cells) lin_accumulate_impl<MODE, WANT_H, G, true, COUNT, RB>(a, Tl, Te, sum);  // (grid-uniform branch)
-  else lin_accumulate_impl<MODE, WANT_H, G, false, COUNT, RB>(a, Tl, Te, sum);
+template <int MODE, bool WANT_H, int G, bool COUNT, bool RB, bool CT = false>
+__device__ __forceinline__ void lin_accumulate(const LinArgs& a, const Pose& Tl, const Pose& Te, float* sum, const CtArgs* ct = nullptr) {
+  if (a.dense.cells) lin_accumulate_impl<MODE, WANT_H, G, true, COUNT, RB, CT>(a, Tl, Te, sum, ct);  // (grid-uniform branch)
+  else lin_accumulate_impl<MODE, WANT_H, G, false, COUNT, RB, CT>(a, Tl, Te, sum, ct);
 }
 
 // block reduction (warp shuffles in float -> shared in double -> per-block partial), ticket, fixed-order fold by the last
@@ -805,12 +859,13 @@ __device__ __forceinline__ void lin_accumulate(const LinArgs& a, const Pose& Tl,
 // (Tried and dropped: a first-level reduction over distributed shared memory inside 8-block clusters, so that the last block folds
 // grid/8 partials.  It gained little at 17 k points and lost at 1 M points, where the cluster placement constraint left SMs idle
 // at the tail of the single wave.)
-// `partials` ([gridDim.x][kLinStride]) and `ticket` belong to one evaluation: a.partials / a.ticket, or one hypothesis's slice of a
-// multi-pose launch
-template <int NV>
-__device__ __forceinline__ bool lin_reduce(const LinArgs& a, const float* sum, double (*fin)[kLinStride], double* partials, unsigned int* ticket) {
+// `partials` ([gridDim.x][STRIDE]) and `ticket` belong to one evaluation: a.partials / a.ticket, or one hypothesis's slice of a
+// multi-pose launch, or the continuous-time evaluation's own (STRIDE = kCtStride)
+template <int NV, int STRIDE = kLinStride>
+__device__ __forceinline__ bool lin_reduce(const LinArgs& a, const float* sum, double (*fin)[STRIDE], double* partials, unsigned int* ticket) {
+  static_assert(NV <= STRIDE && NV <= kLinThreads, "one partial row holds the sums; one thread per value folds the chains");
   // ---- block reduction: warp shuffles (float) -> shared (double) -> per-block partial ----
-  __shared__ double sh[kLinThreads / 32][kLinStride];
+  __shared__ double sh[kLinThreads / 32][STRIDE];
   __shared__ bool is_last;
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
 #pragma unroll
@@ -825,7 +880,7 @@ __device__ __forceinline__ bool lin_reduce(const LinArgs& a, const float* sum, d
     double s = 0.0;
 #pragma unroll
     for (int w = 0; w < kLinThreads / 32; w++) s += sh[w][threadIdx.x];
-    partials[(size_t)blockIdx.x * kLinStride + threadIdx.x] = s;
+    partials[(size_t)blockIdx.x * STRIDE + threadIdx.x] = s;
   }
   __threadfence();
   __syncthreads();
@@ -838,8 +893,8 @@ __device__ __forceinline__ bool lin_reduce(const LinArgs& a, const float* sum, d
   __threadfence();
   // ---- last block: fold the per-block partials in block order (4 interleaved chains per value) ----
   {
-    const int v = threadIdx.x & 31, chain = threadIdx.x >> 5;  // kLinThreads == 128 -> 4 chains
-    if (v < NV) {
+    const int chain = threadIdx.x >> 5;  // kLinThreads == 128 -> 4 chains
+    auto fold = [&](int v) {
       // ld.global.cg: coherent at L2 (the partials were written by other SMs), 16 independent loads in flight per
       // round -- a dependent load->add chain over hundreds of blocks serialises on L2 latency
       double s = 0.0;
@@ -848,12 +903,18 @@ __device__ __forceinline__ bool lin_reduce(const LinArgs& a, const float* sum, d
       for (; b + 4 * 15 < gridDim.x; b += 4 * 16) {
         double t[16];
 #pragma unroll
-        for (int u = 0; u < 16; u++) t[u] = __ldcg(part + (size_t)(b + 4 * u) * kLinStride);
+        for (int u = 0; u < 16; u++) t[u] = __ldcg(part + (size_t)(b + 4 * u) * STRIDE);
 #pragma unroll
         for (int u = 0; u < 16; u++) s += t[u];
       }
-      for (; b < gridDim.x; b += 4) s += __ldcg(part + (size_t)b * kLinStride);
+      for (; b < gridDim.x; b += 4) s += __ldcg(part + (size_t)b * STRIDE);
       fin[chain][v] = s;
+    };
+    if constexpr (NV <= 32) {
+      const int v = threadIdx.x & 31;
+      if (v < NV) fold(v);
+    } else {
+      for (int v = threadIdx.x & 31; v < NV; v += 32) fold(v);  // (each value in the same chain order as above)
     }
   }
   __syncthreads();
@@ -862,6 +923,7 @@ __device__ __forceinline__ bool lin_reduce(const LinArgs& a, const float* sum, d
     fin[0][threadIdx.x] = s;
   }
   __syncthreads();
+  if constexpr (NV > kLinStride) return true;  // (the mailboxes hold kLinStride values: the continuous-time evaluation is never sharded)
   if (a.comm_ranks > 1) {
     // ---- fused exchange: store this rank's sums into every peer's mailbox over NVLink, publish, wait for the peers,
     // add in rank order (identical doubles in identical order on every rank -> identical LM decisions everywhere) ----
@@ -977,6 +1039,25 @@ __global__ void __launch_bounds__(kLinThreads) k_linearize_spec(const LinArgs a)
     if (a.done_flag) {
       __threadfence_system();
       *a.done_flag = a.done_seq;
+    }
+  }
+}
+
+// Continuous-time evaluation (vgicp_compute_error_ct): the compacted kernel with the CT flag, its own partial-sum stride and
+// result.  c.out[0..kCtValues) (WANT_H) or c.out[0] (error only): the raw folded sums in apply_jacobian's layout.
+template <int MODE, bool WANT_H, int G, bool RB>
+__global__ void __launch_bounds__(kLinThreads) k_linearize_ct(const LinArgs a, const CtArgs c) {
+  constexpr int NV = WANT_H ? kCtValues : 1;
+  __shared__ double fin[4][kCtStride];
+  float sum[NV];
+  lin_accumulate<MODE, WANT_H, G, false, RB, true>(a, a.Tlin, a.Teval, sum, &c);
+  if (!lin_reduce<NV, kCtStride>(a, sum, fin, c.partials, c.ticket)) return;
+  if (threadIdx.x == 0) {
+    for (int j = 0; j < NV; j++) c.out[j] = fin[0][j];
+    *c.ticket = 0u;
+    if (c.done_flag) {
+      __threadfence_system();
+      *c.done_flag = c.done_seq;
     }
   }
 }

@@ -267,6 +267,7 @@ class FastVGICPCuda(LsqRegistration):
         self.vgicp_cuda_ = Core(device)
         self.vgicp_cuda_.set_resolution(self.voxel_resolution_)
         self.vgicp_cuda_.set_kernel_params(0.5, 3.0)  # fast_vgicp_cuda_impl.hpp:31
+        self.final_twist_ = np.zeros(6)
 
     # -- setters (fast_vgicp_cuda_impl.hpp:37-66)
     def setCorrespondenceRandomness(self, k):  # empty in the reference (:38): k stays 20 on the CUDA path
@@ -342,6 +343,42 @@ class FastVGICPCuda(LsqRegistration):
 
     def deskew_source(self, times, twist, t_ref=0.0):
         self.deskewSource(times, twist, t_ref)
+
+    # -- continuous-time registration (an extension): the pose at t_ref and the sweep's body twist estimated together
+    # (vgicp_align_ct).  setInputSource with another cloud and swapSourceAndTarget drop the timestamps; deskewSource keeps them.
+    def setSourceTimestamps(self, times, t_ref=0.0):
+        """One relative timestamp per point of the current source (as deskewSource takes them)."""
+        if self.input_ is None:
+            raise RuntimeError("setSourceTimestamps: input source not set")
+        self.vgicp_cuda_.set_source_timestamps(times, t_ref)
+
+    def alignCT(self, initial_guess=None, twist_guess=None, twist_prior=None, twist_weight=1e-6):
+        """-> dict T (4x4 float32, also getFinalTransformation()), twist (6,), H (12x12), nr_iterations, converged, n_linearize,
+        n_compute_error, lm_failed.  twist_prior None: the twist guess; twist_weight: 6 weights > 0 (a scalar applies to all).
+        The guess is cast to float like align's."""
+        if self.input_ is None or self.target_ is None:
+            raise RuntimeError("alignCT: input source/target not set")
+        guess = np.eye(4) if initial_guess is None else np.asarray(initial_guess, dtype=np.float32).astype(np.float64)
+        self._prelude()
+        self.converged_ = False
+        res = self.vgicp_cuda_.align_ct(guess, twist_guess, twist_prior, np.broadcast_to(np.asarray(twist_weight, dtype=np.float64), (6,)), self._params())
+        if res.lm_failed:
+            print("lm not converged!!")
+        self.nr_iterations_ = res.nr_iterations
+        self.converged_ = bool(res.converged)
+        self.final_transformation_ = _core.pose_from_c(res.T).astype(np.float32)
+        self.final_twist_ = np.array(res.twist)
+        return dict(T=self.final_transformation_, twist=self.final_twist_.copy(), H=np.array(res.H).reshape(12, 12).T.copy(), nr_iterations=res.nr_iterations,
+                    converged=bool(res.converged), n_linearize=res.n_linearize, n_compute_error=res.n_compute_error, lm_failed=bool(res.lm_failed))
+
+    def getFinalTwist(self):
+        return self.final_twist_
+
+    def set_source_timestamps(self, times, t_ref=0.0):
+        self.setSourceTimestamps(times, t_ref)
+
+    def align_ct(self, initial_guess=None, twist_guess=None, twist_prior=None, twist_weight=1e-6):
+        return self.alignCT(initial_guess, twist_guess, twist_prior, twist_weight)
 
     # -- state machine (:69-141)
     def swapSourceAndTarget(self):

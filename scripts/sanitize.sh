@@ -60,6 +60,12 @@ c.deskew_source(cloud["time"], [0.0, 0.0, 0.35, 8.0, 0.0, 0.0], 0.05)
 c.find_source_neighbors(20); c.calculate_source_covariances(3)
 r = c.align()
 print("deskew", c.num_source_points(), "converged", bool(r.converged))
+# continuous time: the timestamps kept by the deskew, the pose and the residual twist estimated together (k_linearize_ct), both hints
+for hint, method in ((0, "DIRECT7"), (1, "DIRECT_RADIUS")):
+    c.set_execution_hint(hint); c.set_neighbor_search_method(method, 1.5)
+    c.set_source_timestamps(cloud["time"], 0.05)
+    r = c.align_ct(np.eye(4), np.zeros(6), np.zeros(6), np.full(6, 1e-3))
+    print("ct", method, "converged", bool(r.converged), "twist", list(r.twist))
 c.close()
 # NDT D2D through the same evaluation kernels
 c = Core(0)
