@@ -47,6 +47,7 @@ EXPORTED_SYMBOLS = [
     "vgicp_align_multi", "vgicp_evaluate_poses", "vgicp_set_robust_kernel",
     "vgicp_append_source_to_target", "vgicp_crop_target", "vgicp_deskew_source",
     "vgicp_set_source_timestamps", "vgicp_compute_error_ct", "vgicp_align_ct",
+    "vgicp_set_source_timestamps_device", "vgicp_deskew_source_stored",
 ]
 PROF_NUM_CATEGORIES = 7
 
@@ -175,6 +176,8 @@ def load_library():
         "vgicp_set_source_timestamps": [hp, C.c_void_p, C.c_size_t, C.c_size_t, C.c_double],
         "vgicp_compute_error_ct": [hp, dp, dp, dp, dp, dp, dp, dp],
         "vgicp_align_ct": [hp, dp, dp, dp, dp, C.POINTER(LsqParams), C.POINTER(AlignCtResult)],
+        "vgicp_set_source_timestamps_device": [hp, C.c_void_p, C.c_size_t, C.c_size_t, C.c_double],
+        "vgicp_deskew_source_stored": [hp, dp],
     }
     for name, argtypes in sig.items():
         fn = getattr(L, name)
@@ -588,6 +591,16 @@ class Core:
         set_source_cloud and swap_source_and_target drop them; deskew_source keeps them."""
         a, stride = self._times(times)
         self._check(self._lib.vgicp_set_source_timestamps(self._h, a.ctypes.data, len(a), stride, float(t_ref)))
+
+    def set_source_timestamps_device(self, dev_ptr, n, stride, t_ref=0.0):
+        """set_source_timestamps with the timestamps already in this GPU's memory (e.g. a torch CUDA tensor's data_ptr(), or the
+        time column of a prep output: data_ptr() + 4 * (3 + j), stride (3 + F) * 4); the same state as the host call."""
+        self._check(self._lib.vgicp_set_source_timestamps_device(self._h, dev_ptr, n, stride, float(t_ref)))
+
+    def deskew_source_stored(self, twist):
+        """deskew_source with the stored timestamps and their t_ref (set_source_timestamps(_device)): no upload; the same points."""
+        xi = np.ascontiguousarray(np.asarray(twist, dtype=np.float64).reshape(6))
+        self._check(self._lib.vgicp_deskew_source_stored(self._h, _dp(xi)))
 
     def compute_error_ct(self, T_lin, xi_lin, T_eval, xi_eval, want_H=True):
         """-> (err, H (12,12) | None, b (12,) | None): the data terms at (T_eval, xi_eval) over the correspondences of

@@ -83,6 +83,13 @@ public:
     sourceCovariances();
     input_ = pcl::make_shared<PointCloudSource>(*input_);
   }
+  // deskewSource with the timestamps and t_ref stored by setSourceTimestamps (no upload): the same points, the same state after
+  void deskewSourceStored(const double twist[6]) {
+    if (!input_) throw std::runtime_error("FastVGICPCuda: deskewSourceStored needs an input source");
+    checkStrict(vgicp_deskew_source_stored(vgicp_cuda_, twist));
+    sourceCovariances();
+    input_ = pcl::make_shared<PointCloudSource>(*input_);
+  }
 
   // Continuous-time registration (an extension): the pose at t_ref and the sweep's body twist estimated together
   // (vgicp_align_ct, include/vgicp_b200.h).  setSourceTimestamps takes one timestamp per point of the current source, as

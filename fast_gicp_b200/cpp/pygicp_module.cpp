@@ -3,8 +3,10 @@
 // accelerated path; asking for them prints the reference's error message and returns identity, main.cpp:117-139).
 #include <pybind11/numpy.h>
 #include <pybind11/pybind11.h>
+#include <pybind11/stl.h>
 
 #include <array>
+#include <cstring>
 #include <iostream>
 #include <limits>
 #include <unordered_map>
@@ -54,9 +56,14 @@ static Cloud::Ptr eigen2pcl(const ArrD& points) {  // main.cpp:36-44 (double -> 
 
 // pcl::ApproximateVoxelGrid<PointXYZ> (main.cpp:46-62,81-91) on the device: include/vgicp_prep_b200.h reproduces the serial
 // filter's output (points and order) bit for bit (tests/test_input_prep.py); no host implementation is kept in the product.
-static Cloud::Ptr approximate_voxel_grid(const Cloud& in, float leaf) {
+static vgicp_prep_handle prep_handle() {
   static vgicp_prep_handle prep = nullptr;  // one per process, device 0 like the registration objects' default
   if (!prep && vgicp_prep_create(0, &prep) != 0) throw std::runtime_error("pygicp: the input-preparation library found no usable CUDA device (sm_90a required)");
+  return prep;
+}
+
+static Cloud::Ptr approximate_voxel_grid(const Cloud& in, float leaf) {
+  vgicp_prep_handle prep = prep_handle();
   auto out = pcl::make_shared<Cloud>();
   const size_t n = in.points.size();
   if (n == 0) return out;
@@ -76,6 +83,27 @@ static ArrD downsample(const ArrD& points, double resolution) {  // main.cpp:46-
   ArrD out({static_cast<py::ssize_t>(filtered->size()), static_cast<py::ssize_t>(3)});
   auto o = out.mutable_unchecked<2>();
   for (size_t i = 0; i < filtered->size(); i++) { o(i, 0) = filtered->at(i).x; o(i, 1) = filtered->at(i).y; o(i, 2) = filtered->at(i).z; }
+  return out;
+}
+
+// the same filter on (n, k) float32 records, averaging the given columns (e.g. time, intensity) per voxel next to x y z
+// (pcl::ApproximateVoxelGrid<PointT>'s default) -> (m, 3 + F) float32: x y z, then the fields in the order given
+static ArrF downsample_fields(const ArrF& points, double resolution, const std::vector<int>& field_columns) {
+  if (points.ndim() != 2 || points.shape(1) < 3) throw std::invalid_argument("points must be (N, K >= 3)");
+  const size_t n = static_cast<size_t>(points.shape(0)), k = static_cast<size_t>(points.shape(1)), F = field_columns.size();
+  std::vector<size_t> offsets;
+  for (int c : field_columns) {
+    if (c < 3 || static_cast<size_t>(c) >= k) throw std::invalid_argument("field columns must lie in 3 ... K-1");
+    offsets.push_back(static_cast<size_t>(c) * sizeof(float));
+  }
+  std::vector<float> records(n * (3 + F));
+  size_t m = 0;
+  vgicp_prep_handle prep = prep_handle();
+  const int rc = vgicp_prep_approximate_voxel_grid_fields(prep, points.data(), n, k * sizeof(float), 0, static_cast<float>(resolution), 0, offsets.data(),
+                                                          static_cast<int>(F), records.data(), n, 0, &m);
+  if (rc != 0) throw std::runtime_error(std::string("pygicp.downsample_fields: ") + vgicp_prep_last_error(prep));
+  ArrF out({static_cast<py::ssize_t>(m), static_cast<py::ssize_t>(3 + F)});
+  if (m > 0) std::memcpy(out.mutable_data(), records.data(), m * (3 + F) * sizeof(float));
   return out;
 }
 
@@ -150,6 +178,8 @@ static py::array_t<double> align_points(const ArrD& target, const ArrD& source, 
 
 PYBIND11_MODULE(pygicp, m) {
   m.def("downsample", &downsample, "downsample points");
+  m.def("downsample_fields", &downsample_fields, "downsample (N, K) float32 records, averaging the field columns per voxel", py::arg("points"), py::arg("resolution"),
+        py::arg("field_columns"));
   m.def("align_points", &align_points, "align two point sets", py::arg("target"), py::arg("source"), py::arg("method") = "GICP", py::arg("downsample_resolution") = -1.0,
         py::arg("k_correspondences") = 15, py::arg("max_correspondence_distance") = std::numeric_limits<double>::max(), py::arg("voxel_resolution") = 1.0,
         py::arg("num_threads") = 0, py::arg("neighbor_search_method") = "DIRECT1", py::arg("neighbor_search_radius") = 1.5, py::arg("initial_guess") = identity4f());
@@ -248,6 +278,13 @@ PYBIND11_MODULE(pygicp, m) {
            v.deskewSource(times.data(), static_cast<size_t>(times.size()), sizeof(float), twist.data(), t_ref);
          },
          py::arg("times"), py::arg("twist"), py::arg("t_ref") = 0.0)
+    // the same with the timestamps and t_ref stored by set_source_timestamps (no upload)
+    .def("deskew_source_stored",
+         [](VgicpCuda& v, const ArrD& twist) {
+           if (twist.size() != 6) throw std::invalid_argument("twist must have 6 elements");
+           v.deskewSourceStored(twist.data());
+         },
+         py::arg("twist"))
     // continuous-time registration (not in the reference binding): pose at t_ref and the sweep's twist together
     .def("set_source_timestamps",
          [](VgicpCuda& v, const ArrF& times, double t_ref) { v.setSourceTimestamps(times.data(), static_cast<size_t>(times.size()), sizeof(float), t_ref); },

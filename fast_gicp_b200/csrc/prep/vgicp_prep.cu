@@ -39,12 +39,34 @@ __global__ void k_prep_keys(const float* __restrict__ xyz, size_t stride_f, int 
   entry[i] = keep ? (unsigned short)(hl & (long long)(kHist - 1)) : kNoEntry;
 }
 
+// Per-point float fields averaged next to x y z (vgicp_prep_approximate_voxel_grid_fields); the kernels below are templates on the
+// field count F, and F = 0 is vgicp_prep_approximate_voxel_grid.  A flushed field centroid goes to flushed[F * i + j], i the index of
+// the flushing point (beside the float4 of its xyz), a held one to tail[F * h + j]; both are read only where the float4 flag is set.
+constexpr int kMaxFields = 8;
+struct FieldArgs {
+  const float* in;  // the input records (device), stride_f floats apart
+  size_t stride_f;
+  int off[kMaxFields];  // offset of field j in floats
+  float* flushed;       // [n][F]
+  float* tail;          // [kHist][F]
+};
+
+template <int F>
+struct FieldSums {
+  float s[F];
+};
+template <>
+struct FieldSums<0> {};
+
+template <int F>
 struct Entry {  // one history entry, in the registers of its thread
   int ix, iy, iz, count;
   float sx, sy, sz;
+  FieldSums<F> f;
 };
 
-__device__ __forceinline__ void entry_step(Entry& e, int i, const float4* __restrict__ pts4, float inv_leaf, float4* __restrict__ flushed) {
+template <int F>
+__device__ __forceinline__ void entry_step(Entry<F>& e, int i, const float4* __restrict__ pts4, float inv_leaf, float4* __restrict__ flushed, const FieldArgs& fa) {
   const float4 p = pts4[i];
   const int ix = (int)floorf(__fmul_rn(p.x, inv_leaf)), iy = (int)floorf(__fmul_rn(p.y, inv_leaf)), iz = (int)floorf(__fmul_rn(p.z, inv_leaf));
   if (e.count && (e.ix != ix || e.iy != iy || e.iz != iz)) {  // another voxel lands on this entry: emit the centroid held so far
@@ -52,21 +74,38 @@ __device__ __forceinline__ void entry_step(Entry& e, int i, const float4* __rest
     flushed[i] = make_float4(__fdiv_rn(e.sx, c), __fdiv_rn(e.sy, c), __fdiv_rn(e.sz, c), 1.f);
     e.count = 0;
     e.sx = e.sy = e.sz = 0.f;
+    if constexpr (F > 0) {
+#pragma unroll
+      for (int j = 0; j < F; j++) {
+        fa.flushed[(size_t)F * i + j] = __fdiv_rn(e.f.s[j], c);
+        e.f.s[j] = 0.f;
+      }
+    }
   }
   e.ix = ix; e.iy = iy; e.iz = iz;
   e.count++;
   e.sx = __fadd_rn(e.sx, p.x); e.sy = __fadd_rn(e.sy, p.y); e.sz = __fadd_rn(e.sz, p.z);
+  if constexpr (F > 0) {
+    const float* r = fa.in + (size_t)i * fa.stride_f;
+#pragma unroll
+    for (int j = 0; j < F; j++) e.f.s[j] = __fadd_rn(e.f.s[j], r[fa.off[j]]);
+  }
 }
 
+template <int F>
 __global__ void __launch_bounds__(kHist) k_prep_walk(const float4* __restrict__ pts4, const unsigned short* __restrict__ entry, int n, float inv_leaf, float4* __restrict__ flushed,
-                                                     float4* __restrict__ tail) {
+                                                     float4* __restrict__ tail, const FieldArgs fa) {
   __shared__ unsigned short sh_entry[kTile];
   __shared__ int cnt[kHist];
   __shared__ unsigned short list[kHist * kCap];
   const int h = threadIdx.x;
-  Entry e;
+  Entry<F> e;
   e.ix = e.iy = e.iz = e.count = 0;
   e.sx = e.sy = e.sz = 0.f;
+  if constexpr (F > 0) {
+#pragma unroll
+    for (int j = 0; j < F; j++) e.f.s[j] = 0.f;
+  }
   for (int base = 0; base < n; base += kTile) {
     cnt[h] = 0;
     __syncthreads();
@@ -89,16 +128,20 @@ __global__ void __launch_bounds__(kHist) k_prep_walk(const float4* __restrict__ 
         while (b >= 0 && mine[b] > v) { mine[b + 1] = mine[b]; b--; }
         mine[b + 1] = v;
       }
-      for (int q = 0; q < c; q++) entry_step(e, base + (int)mine[q], pts4, inv_leaf, flushed);
+      for (int q = 0; q < c; q++) entry_step(e, base + (int)mine[q], pts4, inv_leaf, flushed, fa);
     } else if (c > kCap) {  // a run of points on one entry (e.g. the invalid returns at the origin): walk the staged tile
       for (int j = 0; j < kTile; j++)
-        if (sh_entry[j] == (unsigned short)h) entry_step(e, base + j, pts4, inv_leaf, flushed);
+        if (sh_entry[j] == (unsigned short)h) entry_step(e, base + j, pts4, inv_leaf, flushed, fa);
     }
     __syncthreads();  // the tile's lists are consumed before the next tile overwrites them
   }
   if (e.count) {
     const float c = (float)e.count;
     tail[h] = make_float4(__fdiv_rn(e.sx, c), __fdiv_rn(e.sy, c), __fdiv_rn(e.sz, c), 1.f);
+    if constexpr (F > 0) {
+#pragma unroll
+      for (int j = 0; j < F; j++) fa.tail[F * h + j] = __fdiv_rn(e.f.s[j], c);
+    }
   } else {
     tail[h] = make_float4(0.f, 0.f, 0.f, 0.f);
   }
@@ -106,8 +149,10 @@ __global__ void __launch_bounds__(kHist) k_prep_walk(const float4* __restrict__ 
 
 // rank of every flushed centroid = number of flushes at smaller point indices; one block per 1024 points, decoupled look-back over
 // epoch-tagged block totals (a block only waits for blocks with a smaller index, which were scheduled before it)
+// output records of 3 + F floats: x y z, then the F fields
+template <int F>
 __global__ void __launch_bounds__(1024) k_prep_scatter(const float4* __restrict__ flushed, int n, float* __restrict__ out, size_t cap, unsigned long long* chunk_state,
-                                                       unsigned epoch, int* __restrict__ total) {
+                                                       unsigned epoch, int* __restrict__ total, const float* __restrict__ fflushed) {
   __shared__ int warp_sums[32];
   __shared__ int s_base;
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
@@ -153,12 +198,21 @@ __global__ void __launch_bounds__(1024) k_prep_scatter(const float4* __restrict_
   __syncthreads();
   if (flag) {
     const size_t pos = (size_t)(s_base + (wid > 0 ? warp_sums[wid - 1] : 0) + v - 1);
-    if (pos < cap) { out[3 * pos] = f.x; out[3 * pos + 1] = f.y; out[3 * pos + 2] = f.z; }
+    if (pos < cap) {
+      float* o = out + (3 + F) * pos;
+      o[0] = f.x; o[1] = f.y; o[2] = f.z;
+      if constexpr (F > 0) {
+#pragma unroll
+        for (int j = 0; j < F; j++) o[3 + j] = fflushed[(size_t)F * i + j];
+      }
+    }
   }
 }
 
 // the entries still holding a voxel, in entry order, behind the flushed centroids
-__global__ void __launch_bounds__(kHist) k_prep_tail(const float4* __restrict__ tail, const int* __restrict__ total, float* __restrict__ out, size_t cap, int* __restrict__ n_out) {
+template <int F>
+__global__ void __launch_bounds__(kHist) k_prep_tail(const float4* __restrict__ tail, const int* __restrict__ total, float* __restrict__ out, size_t cap, int* __restrict__ n_out,
+                                                     const float* __restrict__ ftail) {
   __shared__ int warp_sums[kHist / 32];
   const int h = threadIdx.x, lane = h & 31, wid = h >> 5;
   const float4 f = tail[h];
@@ -175,7 +229,14 @@ __global__ void __launch_bounds__(kHist) k_prep_tail(const float4* __restrict__ 
   const int first = *total;
   if (flag) {
     const size_t pos = (size_t)(first + before + __popc(m & ((1u << lane) - 1u)));
-    if (pos < cap) { out[3 * pos] = f.x; out[3 * pos + 1] = f.y; out[3 * pos + 2] = f.z; }
+    if (pos < cap) {
+      float* o = out + (3 + F) * pos;
+      o[0] = f.x; o[1] = f.y; o[2] = f.z;
+      if constexpr (F > 0) {
+#pragma unroll
+        for (int j = 0; j < F; j++) o[3 + j] = ftail[F * h + j];
+      }
+    }
   }
   if (h == 0) *n_out = first + all;
 }
@@ -217,6 +278,8 @@ struct vgicp_prep_context {
   float4* tail = nullptr;  // [kHist]
   int* d_counts = nullptr;  // [0] flushed total, [1] n_out
   int* h_counts = nullptr;  // pinned
+  DevBuf<float> fflushed;  // per-point fields: flushed field centroids [n][F]
+  DevBuf<float> ftail;     // ... and those of the entries still holding a voxel [kHist][F]
 };
 
 namespace {
@@ -263,6 +326,7 @@ void vgicp_prep_destroy(vgicp_prep_handle h) {
     cudaStreamDestroy(h->stream);
   }
   h->staging.release(); h->pts4.release(); h->entry.release(); h->flushed.release(); h->out.release(); h->chunk_state.release();
+  h->fflushed.release(); h->ftail.release();
   if (h->tail) cudaFree(h->tail);
   if (h->d_counts) cudaFree(h->d_counts);
   if (h->h_counts) cudaFreeHost(h->h_counts);
@@ -271,31 +335,53 @@ void vgicp_prep_destroy(vgicp_prep_handle h) {
 
 const char* vgicp_prep_last_error(vgicp_prep_handle h) { return h ? h->err.c_str() : "null handle"; }
 
-int vgicp_prep_approximate_voxel_grid(vgicp_prep_handle h, const float* xyz, size_t n, size_t stride_bytes, int on_device, float leaf, int remove_near_origin, float* out_xyz,
-                                      size_t cap, int out_on_device, size_t* n_out) {
-  if (!h) return 1;
-  if (!n_out) return fail(h, 1, "approximate_voxel_grid: n_out is null");
-  *n_out = 0;
-  if (n == 0) return 0;
-  if (!xyz || !out_xyz) return fail(h, 1, "approximate_voxel_grid: null buffer");
-  if (stride_bytes < 12 || stride_bytes % 4) return fail(h, 1, "approximate_voxel_grid: stride must be >= 12 and a multiple of 4");
-  if (!(leaf > 0.f)) return fail(h, 1, "approximate_voxel_grid: leaf size must be positive");
-  if (n > (size_t)0x7fffffff - 4096) return fail(h, 1, "approximate_voxel_grid: too many points");
+}  // extern "C"
+
+namespace {
+
+template <int F>
+cudaError_t launch_filter(vgicp_prep_handle h, const float* d_in, size_t stride_f, const int* off, int ni, float inv_leaf, int filter, float* d_out, size_t out_cap, int chunks) {
+  FieldArgs fa{};
+  fa.in = d_in;
+  fa.stride_f = stride_f;
+  for (int j = 0; j < F; j++) fa.off[j] = off[j];
+  fa.flushed = h->fflushed.p;
+  fa.tail = h->ftail.p;
+  k_prep_keys<<<(ni + 255) / 256, 256, 0, h->stream>>>(d_in, stride_f, ni, inv_leaf, filter, h->pts4.p, h->entry.p);
+  const cudaError_t e = cudaMemsetAsync(h->flushed.p, 0, (size_t)ni * sizeof(float4), h->stream);
+  if (e != cudaSuccess) return e;
+  k_prep_walk<F><<<1, kHist, 0, h->stream>>>(h->pts4.p, h->entry.p, ni, inv_leaf, h->flushed.p, h->tail, fa);
+  k_prep_scatter<F><<<chunks, 1024, 0, h->stream>>>(h->flushed.p, ni, d_out, out_cap, h->chunk_state.p, h->chunk_epoch, h->d_counts, h->fflushed.p);
+  k_prep_tail<F><<<1, kHist, 0, h->stream>>>(h->tail, h->d_counts, d_out, out_cap, h->d_counts + 1, h->ftail.p);
+  return cudaGetLastError();
+}
+
+// both entry points: F = n_fields per-point fields at float offsets off[] (F = 0: x y z only)
+int run_filter(vgicp_prep_handle h, const char* who, const float* points, size_t n, size_t stride_bytes, int on_device, float leaf, int remove_near_origin, const int* off, int F,
+               float* out, size_t cap, int out_on_device, size_t* n_out) {
+  const std::string w(who);
+  const size_t rec = 3 + (size_t)F;  // output floats per point
+  size_t span = 12;                  // bytes of a record the filter reads
+  for (int j = 0; j < F; j++) span = span > (size_t)off[j] * 4 + 4 ? span : (size_t)off[j] * 4 + 4;
   PREP_TRY(h, cudaSetDevice(h->device));
   const int ni = (int)n;
-  const float* d_in = xyz;
+  const float* d_in = points;
   if (!on_device) {
     PREP_TRY(h, h->staging.reserve(n * stride_bytes));
-    PREP_TRY(h, cudaMemcpyAsync(h->staging.p, xyz, (n - 1) * stride_bytes + 12, cudaMemcpyHostToDevice, h->stream));
+    PREP_TRY(h, cudaMemcpyAsync(h->staging.p, points, (n - 1) * stride_bytes + span, cudaMemcpyHostToDevice, h->stream));
     d_in = reinterpret_cast<const float*>(h->staging.p);
   }
   PREP_TRY(h, h->pts4.reserve(n));
   PREP_TRY(h, h->entry.reserve(n));
   PREP_TRY(h, h->flushed.reserve(n));
-  float* d_out = out_xyz;
+  if (F > 0) {
+    PREP_TRY(h, h->fflushed.reserve(n * F));
+    PREP_TRY(h, h->ftail.reserve((size_t)kHist * F));
+  }
+  float* d_out = out;
   const size_t out_cap = out_on_device ? cap : n;  // the filter never emits more points than it reads
   if (!out_on_device) {
-    PREP_TRY(h, h->out.reserve(3 * n));
+    PREP_TRY(h, h->out.reserve(rec * n));
     d_out = h->out.p;
   }
   const int chunks = (ni + 1023) / 1024;
@@ -312,22 +398,69 @@ int vgicp_prep_approximate_voxel_grid(vgicp_prep_handle h, const float* xyz, siz
     }
   }
   const float inv_leaf = 1.0f / leaf;
-  k_prep_keys<<<(ni + 255) / 256, 256, 0, h->stream>>>(d_in, stride_bytes / 4, ni, inv_leaf, remove_near_origin ? 1 : 0, h->pts4.p, h->entry.p);
-  PREP_TRY(h, cudaMemsetAsync(h->flushed.p, 0, n * sizeof(float4), h->stream));
-  k_prep_walk<<<1, kHist, 0, h->stream>>>(h->pts4.p, h->entry.p, ni, inv_leaf, h->flushed.p, h->tail);
-  k_prep_scatter<<<chunks, 1024, 0, h->stream>>>(h->flushed.p, ni, d_out, out_cap, h->chunk_state.p, h->chunk_epoch, h->d_counts);
-  k_prep_tail<<<1, kHist, 0, h->stream>>>(h->tail, h->d_counts, d_out, out_cap, h->d_counts + 1);
-  PREP_TRY(h, cudaGetLastError());
+  const size_t sf = stride_bytes / 4;
+  const int flt = remove_near_origin ? 1 : 0;
+  switch (F) {
+    case 0: PREP_TRY(h, (launch_filter<0>(h, d_in, sf, off, ni, inv_leaf, flt, d_out, out_cap, chunks))); break;
+    case 1: PREP_TRY(h, (launch_filter<1>(h, d_in, sf, off, ni, inv_leaf, flt, d_out, out_cap, chunks))); break;
+    case 2: PREP_TRY(h, (launch_filter<2>(h, d_in, sf, off, ni, inv_leaf, flt, d_out, out_cap, chunks))); break;
+    case 3: PREP_TRY(h, (launch_filter<3>(h, d_in, sf, off, ni, inv_leaf, flt, d_out, out_cap, chunks))); break;
+    case 4: PREP_TRY(h, (launch_filter<4>(h, d_in, sf, off, ni, inv_leaf, flt, d_out, out_cap, chunks))); break;
+    case 5: PREP_TRY(h, (launch_filter<5>(h, d_in, sf, off, ni, inv_leaf, flt, d_out, out_cap, chunks))); break;
+    case 6: PREP_TRY(h, (launch_filter<6>(h, d_in, sf, off, ni, inv_leaf, flt, d_out, out_cap, chunks))); break;
+    case 7: PREP_TRY(h, (launch_filter<7>(h, d_in, sf, off, ni, inv_leaf, flt, d_out, out_cap, chunks))); break;
+    case 8: PREP_TRY(h, (launch_filter<8>(h, d_in, sf, off, ni, inv_leaf, flt, d_out, out_cap, chunks))); break;
+    default: return fail(h, 1, w + ": unsupported field count");
+  }
   PREP_TRY(h, cudaMemcpyAsync(h->h_counts, h->d_counts, 2 * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
   PREP_TRY(h, cudaStreamSynchronize(h->stream));
   const size_t m = (size_t)h->h_counts[1];
   *n_out = m;
-  if (m > cap) return fail(h, 1, "approximate_voxel_grid: output capacity too small (n points always suffice)");
+  if (m > cap) return fail(h, 1, w + ": output capacity too small (n points always suffice)");
   if (!out_on_device && m > 0) {
-    PREP_TRY(h, cudaMemcpyAsync(out_xyz, d_out, m * 3 * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+    PREP_TRY(h, cudaMemcpyAsync(out, d_out, m * rec * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
     PREP_TRY(h, cudaStreamSynchronize(h->stream));
   }
   return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int vgicp_prep_approximate_voxel_grid(vgicp_prep_handle h, const float* xyz, size_t n, size_t stride_bytes, int on_device, float leaf, int remove_near_origin, float* out_xyz,
+                                      size_t cap, int out_on_device, size_t* n_out) {
+  if (!h) return 1;
+  if (!n_out) return fail(h, 1, "approximate_voxel_grid: n_out is null");
+  *n_out = 0;
+  if (n == 0) return 0;
+  if (!xyz || !out_xyz) return fail(h, 1, "approximate_voxel_grid: null buffer");
+  if (stride_bytes < 12 || stride_bytes % 4) return fail(h, 1, "approximate_voxel_grid: stride must be >= 12 and a multiple of 4");
+  if (!(leaf > 0.f)) return fail(h, 1, "approximate_voxel_grid: leaf size must be positive");
+  if (n > (size_t)0x7fffffff - 4096) return fail(h, 1, "approximate_voxel_grid: too many points");
+  return run_filter(h, "approximate_voxel_grid", xyz, n, stride_bytes, on_device, leaf, remove_near_origin, nullptr, 0, out_xyz, cap, out_on_device, n_out);
+}
+
+int vgicp_prep_approximate_voxel_grid_fields(vgicp_prep_handle h, const float* points, size_t n, size_t stride_bytes, int on_device, float leaf, int remove_near_origin,
+                                             const size_t* field_offsets, int n_fields, float* out, size_t cap, int out_on_device, size_t* n_out) {
+  if (!h) return 1;
+  if (!n_out) return fail(h, 1, "approximate_voxel_grid_fields: n_out is null");
+  *n_out = 0;
+  if (n_fields < 1 || n_fields > kMaxFields) return fail(h, 1, "approximate_voxel_grid_fields: n_fields must be 1 ... 8");
+  if (!field_offsets) return fail(h, 1, "approximate_voxel_grid_fields: null field_offsets");
+  if (stride_bytes < 12 || stride_bytes % 4) return fail(h, 1, "approximate_voxel_grid_fields: stride must be >= 12 and a multiple of 4");
+  int off[kMaxFields];
+  for (int j = 0; j < n_fields; j++) {
+    const size_t o = field_offsets[j];
+    if (o % 4 || o < 12 || o > stride_bytes - 4)
+      return fail(h, 1, "approximate_voxel_grid_fields: a field offset must be a multiple of 4, >= 12 and leave 4 bytes within the stride");
+    off[j] = (int)(o / 4);
+  }
+  if (n == 0) return 0;
+  if (!points || !out) return fail(h, 1, "approximate_voxel_grid_fields: null buffer");
+  if (!(leaf > 0.f)) return fail(h, 1, "approximate_voxel_grid_fields: leaf size must be positive");
+  if (n > (size_t)0x7fffffff - 4096) return fail(h, 1, "approximate_voxel_grid_fields: too many points");
+  return run_filter(h, "approximate_voxel_grid_fields", points, n, stride_bytes, on_device, leaf, remove_near_origin, off, n_fields, out, cap, out_on_device, n_out);
 }
 
 }  // extern "C"

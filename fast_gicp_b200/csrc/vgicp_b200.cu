@@ -249,6 +249,14 @@ struct vgicp_context {
   double* h_ct_out = nullptr;            // pinned + mapped, same shape (latency hint: written by the kernel directly)
   unsigned long long* h_ct_done = nullptr;  // pinned + mapped completion word
   unsigned long long ct_seq = 0;
+
+  // timestamps from device memory and the deskew with the stored ones (vgicp_set_source_timestamps_device,
+  // vgicp_deskew_source_stored): the raw range and t_ref kept with the timestamps, so that the stored deskew applies
+  // vgicp_deskew_source's own bound in double; the spare buffer the device read packs into (swapped with ct_times on success)
+  float ct_lo = 0.0f, ct_hi = 0.0f;
+  double ct_t_ref = 0.0;
+  DevBuf<float> ct_spare;
+  DevBuf<unsigned> ct_stats;  // [3]: k_gather_times' non-finite count, ~key(min), key(max)
 };
 
 namespace {
@@ -1395,6 +1403,8 @@ int vgicp_destroy(vgicp_handle h) {
   if (h->h_multi_out) cudaFreeHost(h->h_multi_out);
   if (h->h_multi_done) cudaFreeHost(h->h_multi_done);
   h->ct_times.release();
+  h->ct_spare.release();
+  h->ct_stats.release();
   h->ct_partials.release();
   if (h->d_ct_ticket) cudaFree(h->d_ct_ticket);
   if (h->d_ct_out) cudaFree(h->d_ct_out);
@@ -2269,6 +2279,92 @@ int vgicp_set_source_timestamps(vgicp_handle h, const float* t, size_t n, size_t
   h->ct_has_times = true;
   h->ct_tau = tau;
   h->ct_span = span;
+  h->ct_lo = lo;
+  h->ct_hi = hi;
+  h->ct_t_ref = t_ref;
+  return VGICP_OK;
+}
+
+// The same state from timestamps already in this GPU's memory: one kernel packs them into the spare buffer, counting the
+// non-finite values and finding min and max in the same pass; one readback; the spare becomes ct_times only when every value passed
+int vgicp_set_source_timestamps_device(vgicp_handle h, const float* d_t, size_t n, size_t stride_bytes, double t_ref) {
+  CHECK_HANDLE(h);
+  DeviceGuard g(h->device);
+  if (n > 0 && !d_t) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "set_source_timestamps_device: null timestamps");
+  int rc = timestamps_check(h, "set_source_timestamps_device", n, stride_bytes, t_ref);
+  if (rc) return rc;
+  // after the source's pending work (a set_source_cloud_device read of the same buffer): the readback below then also tells the
+  // caller that buffer is free
+  const Cloud& s = h->source;
+  if (s.st != h->stream && s.ready) CU_TRY(h, cudaStreamWaitEvent(h->stream, s.ready, 0));
+  CU_TRY(h, h->ct_spare.reserve(n));
+  CU_TRY(h, h->ct_stats.reserve(3));
+  CU_TRY(h, cudaMemsetAsync(h->ct_stats.p, 0, 3 * sizeof(unsigned), h->stream));
+  KLAUNCH(h, VGICP_PROF_OTHER,
+          k_gather_times<<<blocks_for(n, 256), 256, 0, h->stream>>>(reinterpret_cast<const unsigned char*>(d_t), stride_bytes, (int)n, h->ct_spare.p, h->ct_stats.p));
+  CU_TRY(h, cudaGetLastError());
+  unsigned st[3];
+  CU_TRY(h, cudaMemcpyAsync(st, h->ct_stats.p, sizeof(st), cudaMemcpyDeviceToHost, h->stream));
+  CU_TRY(h, cudaStreamSynchronize(h->stream));  // (the caller may reuse d_t after return)
+  if (st[0]) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "set_source_timestamps_device: non-finite timestamp");
+  auto from_key = [](unsigned k) {
+    const unsigned b = (k & 0x80000000u) ? (k & 0x7fffffffu) : ~k;
+    float v;
+    memcpy(&v, &b, sizeof(v));
+    return v;
+  };
+  // min and max are exact in any order (only the sign of a zero can differ from the host pass, which leaves every |t - tau| alike)
+  const float lo = from_key(~st[1]), hi = from_key(st[2]);
+  const float tau = (float)t_ref;
+  const double span = fmax(fabs((double)(lo - tau)), fabs((double)(hi - tau)));
+  if (!std::isfinite(span)) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "set_source_timestamps_device: t_i - t_ref overflows a float");
+  std::swap(h->ct_times, h->ct_spare);
+  h->ct_has_times = true;
+  h->ct_tau = tau;
+  h->ct_span = span;
+  h->ct_lo = lo;
+  h->ct_hi = hi;
+  h->ct_t_ref = t_ref;
+  return VGICP_OK;
+}
+
+// vgicp_deskew_source with the stored timestamps and t_ref: k_deskew_points reads ct_times, nothing is uploaded
+int vgicp_deskew_source_stored(vgicp_handle h, const double twist[6]) {
+  CHECK_HANDLE(h);
+  DeviceGuard g(h->device);
+  if (!twist) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "deskew_source_stored: null twist");
+  if (!h->ct_has_times) return fail(h, VGICP_ERR_BAD_STATE, "deskew_source_stored: the source has no timestamps (vgicp_set_source_timestamps(_device))");
+  Cloud& s = h->source;
+  const size_t n = (size_t)s.n;
+  const double t_ref = h->ct_t_ref;
+  const float tau = (float)t_ref;
+  float xi[6];
+  for (int j = 0; j < 6; j++) xi[j] = (float)twist[j];
+  for (int j = 0; j < 6; j++)
+    if (!std::isfinite(xi[j])) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "deskew_source_stored: non-finite twist");
+  const double span = fmax(fabs((double)h->ct_lo - t_ref), fabs((double)h->ct_hi - t_ref));
+  const double omega = sqrt(twist[0] * twist[0] + twist[1] * twist[1] + twist[2] * twist[2]);
+  if (omega * span > 1.5707963267948966)
+    return fail(h, VGICP_ERR_INVALID_ARGUMENT, "deskew_source_stored: the rotation over the sweep exceeds pi/2 (|omega| * max |t_i - t_ref|), beyond the series");
+  // ordering as vgicp_deskew_source's: after the main stream's reads of the source points and after an append
+  if (s.st != h->stream) {
+    if (!h->ev_deskew) CU_TRY(h, cudaEventCreateWithFlags(&h->ev_deskew, cudaEventDisableTiming));
+    CU_TRY(h, cudaEventRecord(h->ev_deskew, h->stream));
+    CU_TRY(h, cudaStreamWaitEvent(s.st, h->ev_deskew, 0));
+  }
+  if (s.st != h->target.st) CU_TRY(h, cudaStreamWaitEvent(s.st, h->ev_append, 0));
+  KLAUNCH_ST(h, s.st, VGICP_PROF_OTHER,
+             k_deskew_points<<<blocks_for(n, 256), 256, 0, s.st>>>(s.pts.p, h->ct_times.p, (int)n, tau, xi[0], xi[1], xi[2], xi[3], xi[4], xi[5]));
+  CU_TRY(h, cudaGetLastError());
+  CU_TRY(h, cudaEventRecord(s.ready, s.st));
+  // the next write of the timestamp buffers (on the main stream) must not overtake this read of ct_times
+  if (s.st != h->stream) CU_TRY(h, cudaStreamWaitEvent(h->stream, s.ready, 0));
+  // the state vgicp_deskew_source leaves: no neighbour rows, no covariances, the NDT source map reset, the timestamps kept
+  s.k = 0;
+  s.has_cov = false;
+  h->ndt_ready = false;
+  h->ndt_s.built = false;
+  h->ndt_s.pending = false;
   return VGICP_OK;
 }
 

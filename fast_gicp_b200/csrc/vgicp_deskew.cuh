@@ -72,4 +72,34 @@ __global__ void k_deskew_points(float4* __restrict__ pts, const float* __restric
   pts[i] = make_float4(q.x, q.y, q.z, 0.0f);
 }
 
+// vgicp_set_source_timestamps_device: the caller's strided timestamps packed into `times`, with what the host path finds in its
+// pass: stats[0] = the number of non-finite values, stats[1] = ~key(min), stats[2] = key(max) over the finite ones, key() the
+// order-preserving map of a float onto an unsigned (stats zeroed before the launch; min and max are exact in any order)
+__device__ __forceinline__ unsigned time_key(float v) {
+  const unsigned b = __float_as_uint(v);
+  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+__global__ void k_gather_times(const unsigned char* __restrict__ src, size_t stride, int n, float* __restrict__ times, unsigned* __restrict__ stats) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  unsigned bad = 0, nlo = 0, hi = 0;  // neutral values of the three reductions
+  if (i < n) {
+    const float v = *reinterpret_cast<const float*>(src + (size_t)i * stride);
+    times[i] = v;
+    if (isfinite(v)) {
+      nlo = ~time_key(v);
+      hi = time_key(v);
+    } else {
+      bad = 1;
+    }
+  }
+  bad = __reduce_add_sync(0xffffffffu, bad);
+  nlo = __reduce_max_sync(0xffffffffu, nlo);
+  hi = __reduce_max_sync(0xffffffffu, hi);
+  if ((threadIdx.x & 31) == 0) {
+    if (bad) atomicAdd(&stats[0], bad);
+    atomicMax(&stats[1], nlo);
+    atomicMax(&stats[2], hi);
+  }
+}
+
 }  // namespace vgicp

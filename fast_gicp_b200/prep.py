@@ -8,7 +8,8 @@ import os
 import numpy as np
 
 LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), "lib", "libvgicp_prep_b200.so")
-EXPORTED_SYMBOLS = ["vgicp_prep_create", "vgicp_prep_destroy", "vgicp_prep_last_error", "vgicp_prep_approximate_voxel_grid"]
+EXPORTED_SYMBOLS = ["vgicp_prep_create", "vgicp_prep_destroy", "vgicp_prep_last_error", "vgicp_prep_approximate_voxel_grid",
+                    "vgicp_prep_approximate_voxel_grid_fields"]
 _lib = None
 
 
@@ -31,6 +32,8 @@ def load_library():
         L.vgicp_prep_last_error.restype = C.c_char_p
         L.vgicp_prep_approximate_voxel_grid.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_int, C.c_float, C.c_int, C.c_void_p, C.c_size_t, C.c_int,
                                                         C.POINTER(C.c_size_t)]
+        L.vgicp_prep_approximate_voxel_grid_fields.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_int, C.c_float, C.c_int, C.POINTER(C.c_size_t), C.c_int,
+                                                               C.c_void_p, C.c_size_t, C.c_int, C.POINTER(C.c_size_t)]
         _lib = L
     return _lib
 
@@ -71,3 +74,55 @@ class InputPrep:
         if rc:
             raise PrepError(rc, self._lib.vgicp_prep_last_error(self._h).decode())
         return out[: m.value].copy()
+
+    def approximate_voxel_grid_fields(self, points, leaf, fields, remove_near_origin=False):
+        """approximate_voxel_grid that also averages per-point float32 fields over each voxel (pcl::ApproximateVoxelGrid<PointT>'s
+        default, setDownsampleAllData(true)) -> (m, 3 + F) float32 records x y z f_0 ... f_{F-1}.
+          points  a numpy structured array (x, y, z: its first three float32 fields; `fields` name float32 fields), an (n, k)
+                  float32 array (`fields` are column indices >= 3), or an (n, k) float32 torch CUDA tensor on this context's device
+                  (read in place; the result is then an (m, 3 + F) torch CUDA tensor, the layout set_cloud_device reads)."""
+        fields = list(fields)
+        if hasattr(points, "is_cuda") and points.is_cuda:
+            return self._fields_device(points, leaf, fields, remove_near_origin)
+        p = np.asarray(points)
+        if p.dtype.names:
+            names = p.dtype.names
+            if len(names) < 3 or any(p.dtype.fields[k][0] != np.float32 or p.dtype.fields[k][1] != 4 * j for j, k in enumerate(names[:3])):
+                raise ValueError("approximate_voxel_grid_fields: x y z must be the first three float32 fields, at byte offsets 0, 4, 8")
+            offsets = []
+            for f in fields:
+                if p.dtype.fields[f][0] != np.float32:
+                    raise ValueError(f"approximate_voxel_grid_fields: field {f!r} is not float32")
+                offsets.append(p.dtype.fields[f][1])
+            p = np.ascontiguousarray(p)
+            stride = p.dtype.itemsize
+        else:
+            p = np.ascontiguousarray(p, dtype=np.float32)
+            if p.ndim != 2:
+                raise ValueError("approximate_voxel_grid_fields: points must be (n, k) or a structured array")
+            offsets = [4 * int(c) for c in fields]
+            stride = 4 * p.shape[1]
+        n = len(p)
+        out = np.empty((n, 3 + len(fields)), dtype=np.float32)
+        m = self._run_fields(p.ctypes.data, n, stride, 0, leaf, remove_near_origin, offsets, out.ctypes.data, n, 0)
+        return out[:m].copy()
+
+    def _run_fields(self, ptr, n, stride, on_device, leaf, remove_near_origin, offsets, out_ptr, cap, out_on_device):
+        off = (C.c_size_t * max(len(offsets), 1))(*offsets)
+        m = C.c_size_t(0)
+        rc = self._lib.vgicp_prep_approximate_voxel_grid_fields(self._h, ptr, n, stride, int(on_device), C.c_float(leaf), int(bool(remove_near_origin)), off, len(offsets),
+                                                                out_ptr, cap, int(out_on_device), C.byref(m))
+        if rc:
+            raise PrepError(rc, self._lib.vgicp_prep_last_error(self._h).decode())
+        return m.value
+
+    def _fields_device(self, t, leaf, fields, remove_near_origin):
+        import torch
+
+        if t.dtype != torch.float32 or t.dim() != 2 or t.stride(1) != 1:
+            raise ValueError("approximate_voxel_grid_fields: a device input must be an (n, k) float32 tensor with contiguous rows")
+        n, k = t.shape
+        torch.cuda.current_stream(t.device).synchronize()  # the filter runs on this context's own stream: the input must be complete
+        out = torch.empty((n, 3 + len(fields)), dtype=torch.float32, device=t.device)
+        m = self._run_fields(t.data_ptr(), n, 4 * (t.stride(0) if n > 1 else k), 1, leaf, remove_near_origin, [4 * int(c) for c in fields], out.data_ptr(), n, 1)
+        return out[:m]

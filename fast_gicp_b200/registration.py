@@ -344,6 +344,17 @@ class FastVGICPCuda(LsqRegistration):
     def deskew_source(self, times, twist, t_ref=0.0):
         self.deskewSource(times, twist, t_ref)
 
+    def deskewSourceStored(self, twist):
+        """deskewSource with the timestamps and t_ref stored by setSourceTimestamps (no upload): the same points."""
+        if self.input_ is None:
+            raise RuntimeError("deskewSourceStored: input source not set")
+        self.vgicp_cuda_.deskew_source_stored(twist)
+        self._covariances("source")
+        self.input_ = np.array(self.input_, copy=True)
+
+    def deskew_source_stored(self, twist):
+        self.deskewSourceStored(twist)
+
     # -- continuous-time registration (an extension): the pose at t_ref and the sweep's body twist estimated together
     # (vgicp_align_ct).  setInputSource with another cloud and swapSourceAndTarget drop the timestamps; deskewSource keeps them.
     def setSourceTimestamps(self, times, t_ref=0.0):

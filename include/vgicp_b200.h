@@ -285,6 +285,24 @@ VGICP_API int vgicp_deskew_source(vgicp_handle h, const float* t, size_t n, size
  * continuous-time registration of a deskewed scan then estimates the residual twist).  Errors: VGICP_ERR_INVALID_ARGUMENT,
  * VGICP_ERR_BAD_STATE (no source points), before anything is changed. */
 VGICP_API int vgicp_set_source_timestamps(vgicp_handle h, const float* t, size_t n, size_t stride_bytes, double t_ref);
+/* vgicp_set_source_timestamps with the timestamps already in this GPU's memory (device pointer d_t, same n, stride and t_ref
+ * rules): e.g. the time column of vgicp_prep_approximate_voxel_grid_fields' device output, read in place at out + 3 + j with
+ * stride (3 + F) * 4.  Leaves exactly the state vgicp_set_source_timestamps leaves with the same values.  One kernel packs the
+ * values into a spare device buffer, counting the non-finite ones and finding min and max in the same pass; one readback
+ * follows, and the spare buffer replaces the stored timestamps only when every value passed.  The read is stream-ordered on the
+ * handle's stream, after the source's pending work, and the call returns after it: the caller may then reuse d_t, and a buffer
+ * just given to vgicp_set_source_cloud_device as well.  Errors: VGICP_ERR_INVALID_ARGUMENT (null d_t
+ * with n > 0, n other than the source size, a bad stride, a non-finite t_ref, each before any launch; a non-finite timestamp
+ * or t_i - t_ref overflowing a float, found by the kernel: the previous timestamps stay in place), VGICP_ERR_BAD_STATE (no
+ * source points, before any launch). */
+VGICP_API int vgicp_set_source_timestamps_device(vgicp_handle h, const float* d_t, size_t n, size_t stride_bytes, double t_ref);
+/* vgicp_deskew_source with the stored timestamps and their t_ref (vgicp_set_source_timestamps(_device)): no upload, the same
+ * kernel on the stored buffer, so the points are byte for byte those vgicp_deskew_source(h, the same values, ..., twist, the
+ * same t_ref) stores.  The same stream ordering, the same refusal rule (|omega| * max_i |t_i - t_ref| > pi/2 in double, over the
+ * stored raw min and max) and the same state afterwards: no neighbour rows, no covariances, the NDT source map reset, the
+ * timestamps kept.  Errors, all before any launch: VGICP_ERR_INVALID_ARGUMENT (null or non-finite twist, a rotation beyond the
+ * series), VGICP_ERR_BAD_STATE (no stored timestamps). */
+VGICP_API int vgicp_deskew_source_stored(vgicp_handle h, const double twist[6]);
 /* The data terms alone (no prior) at (T_eval, xi_eval) over the correspondences of (T_lin, xi_lin): H144 (12 x 12 column-major)
  * and b12, both given or both NULL (error only), and *err.  Errors as vgicp_align_ct's. */
 VGICP_API int vgicp_compute_error_ct(vgicp_handle h, const double T_lin[16], const double xi_lin[6], const double T_eval[16], const double xi_eval[6], double* H144,

@@ -39,6 +39,21 @@ VGICP_PREP_API const char* vgicp_prep_last_error(vgicp_prep_handle h);
  * *n_out receives the number of points written.  Blocks until the result is in place. */
 VGICP_PREP_API int vgicp_prep_approximate_voxel_grid(vgicp_prep_handle h, const float* xyz, size_t n, size_t stride_bytes, int on_device, float leaf, int remove_near_origin,
                                                      float* out_xyz, size_t cap, int out_on_device, size_t* n_out);
+/* The same filter keeping per-point float fields, as pcl::ApproximateVoxelGrid<PointT> does by default (setDownsampleAllData(true)):
+ * the time and intensity of a PointXYZIT-like point are averaged over the voxel next to x y z.
+ *   points         n records stride_bytes apart (>= 12, a multiple of 4), host (on_device = 0) or device memory; x y z at byte
+ *                  offsets 0, 4, 8 of each record.  A host input is copied up to the last byte of the last record the filter reads.
+ *   field_offsets  n_fields (1 ... 8) byte offsets of float32 fields, each a multiple of 4, >= 12 and offset + 4 <= stride_bytes.
+ *   out            m records of 3 + n_fields floats: x y z f_0 ... f_{F-1}, capacity `cap` records (n always suffices), host
+ *                  (out_on_device = 0) or device memory.  A device output is the layout vgicp_set_source_cloud_device(out, m,
+ *                  (3 + F) * 4) reads, and field j is read in place at out + 3 + j with the same stride (e.g. by
+ *                  vgicp_set_source_timestamps_device).
+ * Arithmetic: each field is summed in float in input order next to x y z and divided once by (float)count (IEEE division), at
+ * the same flushes and in the same output order; x y z are vgicp_prep_approximate_voxel_grid's bytes for the same input.
+ * Blocks until the result is in place. */
+VGICP_PREP_API int vgicp_prep_approximate_voxel_grid_fields(vgicp_prep_handle h, const float* points, size_t n, size_t stride_bytes, int on_device, float leaf,
+                                                            int remove_near_origin, const size_t* field_offsets, int n_fields, float* out, size_t cap, int out_on_device,
+                                                            size_t* n_out);
 #ifdef __cplusplus
 }
 #endif

@@ -67,6 +67,25 @@ for hint, method in ((0, "DIRECT7"), (1, "DIRECT_RADIUS")):
     r = c.align_ct(np.eye(4), np.zeros(6), np.zeros(6), np.full(6, 1e-3))
     print("ct", method, "converged", bool(r.converged), "twist", list(r.twist))
 c.close()
+# timestamped scans on the device: the voxel grid with fields (k_prep_walk / scatter / tail with F = 2, input and output on the
+# device), the source and its timestamps read in place from its output (k_gather_times), the stored deskew, continuous time
+import torch
+from fast_gicp_b200.prep import InputPrep
+p = InputPrep(0)
+rec = np.zeros((len(src), 8), dtype=np.float32)
+rec[:, :3], rec[:, 3], rec[:, 4] = src[:, :3], 50.0, np.linspace(0.0, 0.1, len(src), dtype=np.float32)
+out = p.approximate_voxel_grid_fields(torch.from_numpy(rec).cuda(), 0.25, [4, 3], True)
+m = out.shape[0]
+c = Core(0)
+c.set_neighbor_search_method("DIRECT7")
+c.set_target_cloud(tgt); c.find_target_neighbors(20); c.calculate_target_covariances(3); c.create_target_voxelmap()
+c.set_cloud_device("source", out.data_ptr(), m, 20)
+c.set_source_timestamps_device(out.data_ptr() + 12, m, 20, 0.05)
+c.deskew_source_stored([0.0, 0.0, 0.35, 8.0, 0.0, 0.0])
+c.find_source_neighbors(20); c.calculate_source_covariances(3)
+r = c.align_ct(np.eye(4), np.zeros(6), np.zeros(6), np.full(6, 1e-3))
+print("raw scan", m, "points, ct converged", bool(r.converged))
+c.close(); p.close()
 # NDT D2D through the same evaluation kernels
 c = Core(0)
 c.set_problem(2); c.set_neighbor_search_method("DIRECT7")
