@@ -93,6 +93,13 @@ c.set_target_cloud(tgt); c.set_source_cloud(src); c.ndt_create_voxelmaps()
 r = c.align()
 print("ndt d2d", "converged", bool(r.converged))
 c.close()
+# stage 1, RBF covariances: k_covariance_rbf shares its staged tiles and per-lane partials across a __syncthreads per round of eight
+# blocks; one point (511 padding points), one round plus a padded block, and several rounds with a partial last one
+c = Core(0)
+for n in (1, 513, 4097):
+    c.set_source_cloud(np.ascontiguousarray(d["target"][:n])); c.calculate_source_covariances_rbf(3)
+    print("rbf", n, "finite", bool(np.isfinite(c.get_source_covariances()).all()))
+c.close()
 PY
 for tool in memcheck racecheck synccheck; do
   timeout 900 compute-sanitizer --tool $tool --print-limit 20 python /tmp/san_driver.py > gpurun_out/r02_sanitizer_$tool.log 2>&1
