@@ -74,7 +74,8 @@ PREP_LIB_PATH = os.path.join(LIB_DIR, "libvgicp_prep_b200.so")
 def build_prep(force=False):
     """Input-preparation library (include/vgicp_prep_b200.h): lib/libvgicp_prep_b200.so, independent of libvgicp_b200.so."""
     hdr = os.path.join(ROOT, "include", "vgicp_prep_b200.h")
-    if not force and os.path.exists(PREP_LIB_PATH) and all(os.path.getmtime(d) <= os.path.getmtime(PREP_LIB_PATH) for d in (PREP_SRC, hdr)):
+    deps = (PREP_SRC, hdr, os.path.join(CSRC, "vgicp_sort.cuh"))  # the exact grid uses the library's radix sort
+    if not force and os.path.exists(PREP_LIB_PATH) and all(os.path.getmtime(d) <= os.path.getmtime(PREP_LIB_PATH) for d in deps):
         return PREP_LIB_PATH
     os.makedirs(LIB_DIR, exist_ok=True)
     env = {k: v for k, v in os.environ.items() if k not in ("CC", "CXX")}

@@ -107,6 +107,27 @@ static ArrF downsample_fields(const ArrF& points, double resolution, const std::
   return out;
 }
 
+// pcl::VoxelGrid, the exact grid (vgicp_prep_voxel_grid), on (n, k) float32 records: one centroid per occupied voxel in ascending
+// voxel index, averaging x y z and the given columns -> (m, 3 + F) float32
+static ArrF voxel_grid(const ArrF& points, double resolution, const std::vector<int>& field_columns, unsigned min_points_per_voxel) {
+  if (points.ndim() != 2 || points.shape(1) < 3) throw std::invalid_argument("points must be (N, K >= 3)");
+  const size_t n = static_cast<size_t>(points.shape(0)), k = static_cast<size_t>(points.shape(1)), F = field_columns.size();
+  std::vector<size_t> offsets;
+  for (int c : field_columns) {
+    if (c < 3 || static_cast<size_t>(c) >= k) throw std::invalid_argument("field columns must lie in 3 ... K-1");
+    offsets.push_back(static_cast<size_t>(c) * sizeof(float));
+  }
+  std::vector<float> records(n * (3 + F));
+  size_t m = 0;
+  vgicp_prep_handle prep = prep_handle();
+  const int rc = vgicp_prep_voxel_grid(prep, points.data(), n, k * sizeof(float), 0, static_cast<float>(resolution), 0, offsets.data(), static_cast<int>(F),
+                                       min_points_per_voxel, records.data(), n, 0, &m);
+  if (rc != 0) throw std::runtime_error(std::string("pygicp.voxel_grid: ") + vgicp_prep_last_error(prep));
+  ArrF out({static_cast<py::ssize_t>(m), static_cast<py::ssize_t>(3 + F)});
+  if (m > 0) std::memcpy(out.mutable_data(), records.data(), m * (3 + F) * sizeof(float));
+  return out;
+}
+
 static Eigen::Matrix4f to_mat4f(const ArrF& m) {
   if (m.ndim() != 2 || m.shape(0) != 4 || m.shape(1) != 4) throw std::invalid_argument("initial_guess must be 4x4");
   Eigen::Matrix4f T;
@@ -180,6 +201,8 @@ PYBIND11_MODULE(pygicp, m) {
   m.def("downsample", &downsample, "downsample points");
   m.def("downsample_fields", &downsample_fields, "downsample (N, K) float32 records, averaging the field columns per voxel", py::arg("points"), py::arg("resolution"),
         py::arg("field_columns"));
+  m.def("voxel_grid", &voxel_grid, "pcl::VoxelGrid of (N, K) float32 records: per-voxel centroids of x y z and the field columns, in voxel index order",
+        py::arg("points"), py::arg("resolution"), py::arg("field_columns") = std::vector<int>(), py::arg("min_points_per_voxel") = 0u);
   m.def("align_points", &align_points, "align two point sets", py::arg("target"), py::arg("source"), py::arg("method") = "GICP", py::arg("downsample_resolution") = -1.0,
         py::arg("k_correspondences") = 15, py::arg("max_correspondence_distance") = std::numeric_limits<double>::max(), py::arg("voxel_resolution") = 1.0,
         py::arg("num_threads") = 0, py::arg("neighbor_search_method") = "DIRECT1", py::arg("neighbor_search_radius") = 1.5, py::arg("initial_guess") = identity4f());

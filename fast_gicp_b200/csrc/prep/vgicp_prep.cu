@@ -9,12 +9,16 @@
 // A flushed centroid is stored at the index of the point that flushed it; a scan over those flags (one block per 1024 points,
 // decoupled look-back) gives it the rank the serial filter would have emitted it at, and the entries still holding a voxel at the
 // end follow in entry order.
+//
+// The exact grid (vgicp_prep_voxel_grid, pcl::VoxelGrid) is data-parallel throughout: see "exact grid" below.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <cmath>
 #include <new>
 #include <string>
 
+#include "../vgicp_sort.cuh"
 #include "vgicp_prep_b200.h"
 
 namespace {
@@ -241,6 +245,227 @@ __global__ void __launch_bounds__(kHist) k_prep_tail(const float4* __restrict__ 
   if (h == 0) *n_out = first + all;
 }
 
+// ---------------------------------------------------------------------------------------------------- exact grid (pcl::VoxelGrid)
+// vgicp_prep_voxel_grid: box of the kept points' cells (k_grid_box), one sync to read it back, voxel index keys with their digit
+// histograms (k_grid_keys), the library's stable LSD radix sort carrying x y z and the input index (vgicp_sort.cuh), the voxels that
+// reach the minimum ranked in key order (k_grid_heads), one warp per voxel summing its points in sorted = input order
+// (k_grid_centroids).  Dropped points get the key V = div_x * div_y * div_z, past every voxel, so they sort behind the kept ones.
+constexpr int kGridBoxThreads = 256;
+constexpr int kGridWarps = 4;                  // warps per centroid block
+constexpr int kGridItems = 4;                  // points per lane per round of a centroid warp
+constexpr int kGridChunk = 32 * kGridItems;    // points staged per round
+// box state words: [0..2] ~enc(min g), [3..5] enc(max g) (all reduced with unsigned max, zero = empty), [6] kept count,
+// [7] a kept cell outside the int range, [8] surviving voxels m
+constexpr int kGridState = 9;
+
+__host__ __device__ inline unsigned grid_enc(int g) { return (unsigned)g ^ 0x80000000u; }  // order-preserving int -> unsigned
+__host__ __device__ inline int grid_dec(unsigned u) { return (int)(u ^ 0x80000000u); }
+
+// 0: dropped (non-finite, or near the origin when filtering), 1: kept with cells g, 2: kept but a cell outside the int range
+__device__ __forceinline__ int grid_cell(float x, float y, float z, float inv, int filter, int g[3]) {
+  if (!(isfinite(x) && isfinite(y) && isfinite(z))) return 0;
+  if (filter && __fadd_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)), __fmul_rn(z, z)) < 1e-3f) return 0;
+  const float c[3] = {floorf(__fmul_rn(x, inv)), floorf(__fmul_rn(y, inv)), floorf(__fmul_rn(z, inv))};
+#pragma unroll
+  for (int a = 0; a < 3; a++) {
+    if (!(c[a] >= -2147483648.0f && c[a] < 2147483648.0f)) return 2;
+    g[a] = (int)c[a];
+  }
+  return 1;
+}
+
+__global__ void __launch_bounds__(kGridBoxThreads) k_grid_box(const float* __restrict__ in, size_t stride_f, int n, float inv, int filter, float4* __restrict__ pts4,
+                                                              unsigned* __restrict__ st) {
+  __shared__ unsigned sh[8];
+  if (threadIdx.x < 8) sh[threadIdx.x] = 0;
+  __syncthreads();
+  unsigned mx[6] = {0, 0, 0, 0, 0, 0}, kept = 0, bad = 0;
+  for (int i = blockIdx.x * kGridBoxThreads + threadIdx.x; i < n; i += gridDim.x * kGridBoxThreads) {
+    const float* p = in + (size_t)i * stride_f;
+    const float x = p[0], y = p[1], z = p[2];
+    pts4[i] = make_float4(x, y, z, 0.f);
+    int g[3];
+    const int s = grid_cell(x, y, z, inv, filter, g);
+    kept += s != 0;
+    bad |= s == 2;
+    if (s == 1) {
+#pragma unroll
+      for (int a = 0; a < 3; a++) {
+        mx[a] = max(mx[a], ~grid_enc(g[a]));
+        mx[3 + a] = max(mx[3 + a], grid_enc(g[a]));
+      }
+    }
+  }
+  const unsigned full = 0xffffffffu;
+#pragma unroll
+  for (int a = 0; a < 6; a++) mx[a] = __reduce_max_sync(full, mx[a]);
+  kept = __reduce_add_sync(full, kept);
+  bad = __reduce_or_sync(full, bad);
+  if ((threadIdx.x & 31) == 0) {
+#pragma unroll
+    for (int a = 0; a < 6; a++) atomicMax(&sh[a], mx[a]);
+    atomicAdd(&sh[6], kept);
+    atomicOr(&sh[7], bad);
+  }
+  __syncthreads();
+  if (threadIdx.x < 6) atomicMax(&st[threadIdx.x], sh[threadIdx.x]);
+  else if (threadIdx.x == 6) atomicAdd(&st[6], sh[6]);
+  else if (threadIdx.x == 7) atomicOr(&st[7], sh[7]);
+}
+
+// key of every point (voxel index, or V for a dropped one) and the digit counts of all sort passes
+__global__ void __launch_bounds__(vgicp::kSortThreads) k_grid_keys(const float4* __restrict__ pts4, int n, float inv, int filter, int3 min_b, unsigned div_x, unsigned div_xy,
+                                                                   unsigned dropped_key, int passes, unsigned* __restrict__ keys, unsigned* __restrict__ hist) {
+  using namespace vgicp;
+  __shared__ unsigned sh[kSortMaxPasses * kSortBins];
+  for (int i = threadIdx.x; i < passes * kSortBins; i += kSortThreads) sh[i] = 0;
+  __syncthreads();
+  const int n_round = (n + 31) & ~31;
+  for (int i = blockIdx.x * kSortThreads + threadIdx.x; i < n_round; i += gridDim.x * kSortThreads) {  // warp-uniform trip count
+    const bool valid = i < n;
+    unsigned key = dropped_key;
+    if (valid) {
+      const float4 p = pts4[i];
+      int g[3];
+      if (grid_cell(p.x, p.y, p.z, inv, filter, g) == 1)
+        key = ((unsigned)g[0] - (unsigned)min_b.x) + ((unsigned)g[1] - (unsigned)min_b.y) * div_x + ((unsigned)g[2] - (unsigned)min_b.z) * div_xy;
+      keys[i] = key;
+    }
+    sort_hist_add(sh, passes, valid, key);
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < passes * kSortBins; i += kSortThreads)
+    if (sh[i]) atomicAdd(&hist[i], sh[i]);
+}
+
+// the sorted positions that start a voxel reaching the minimum (the run of equal keys starting at p is at least min_points long iff
+// key[p + min_points - 1] is still p's key), ranked in key order: vstart[rank] = p, st[8] = their number.  One block per 1024 of the
+// kept points' positions, decoupled look-back over epoch-tagged block totals as in k_prep_scatter.
+__global__ void __launch_bounds__(1024) k_grid_heads(const unsigned* __restrict__ keys, int kept, unsigned min_points, unsigned long long* chunk_state, unsigned epoch,
+                                                     int* __restrict__ vstart, unsigned* __restrict__ st) {
+  __shared__ int warp_sums[32];
+  __shared__ int s_base;
+  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  const int p = blockIdx.x * 1024 + tid;
+  int flag = 0;
+  if (p < kept) {
+    const unsigned k = keys[p];
+    flag = p == 0 || keys[p - 1] != k;
+    if (flag && min_points > 1) {
+      const long long q = (long long)p + min_points - 1;
+      flag = q < kept && keys[q] == k;
+    }
+  }
+  int v = flag;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    int t = __shfl_up_sync(0xffffffffu, v, o);
+    if (lane >= o) v += t;
+  }
+  if (lane == 31) warp_sums[wid] = v;
+  __syncthreads();
+  if (wid == 0) {
+    int w = warp_sums[lane];
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      int t = __shfl_up_sync(0xffffffffu, w, o);
+      if (lane >= o) w += t;
+    }
+    warp_sums[lane] = w;
+    const int block_total = __shfl_sync(0xffffffffu, w, 31);
+    volatile unsigned long long* state = chunk_state;
+    if (lane == 0) {
+      state[blockIdx.x] = ((unsigned long long)epoch << 32) | (unsigned)block_total;
+      __threadfence();
+    }
+    int base = 0;
+    for (int b = (int)blockIdx.x - 1 - lane; b >= 0; b -= 32) {
+      unsigned long long sv;
+      while ((unsigned)((sv = state[b]) >> 32) != epoch) {}
+      base += (int)(unsigned)(sv & 0xffffffffULL);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) base += __shfl_xor_sync(0xffffffffu, base, o);
+    if (lane == 0) {
+      s_base = base;
+      if (blockIdx.x == gridDim.x - 1) st[8] = (unsigned)(base + block_total);
+    }
+  }
+  __syncthreads();
+  if (flag) vstart[s_base + (wid > 0 ? warp_sums[wid - 1] : 0) + v - 1] = p;
+}
+
+// One round of a centroid warp: the run's points among sorted positions base ... base + kGridChunk - 1, x y z and the F fields of
+// position base + it * 32 + lane into v[it]; returns how many belong to the run (they are a prefix of the round).
+template <int F>
+__device__ __forceinline__ int grid_round(const unsigned* __restrict__ keys, const float4* __restrict__ sorted4, int kept, unsigned key, int base, const FieldArgs fa,
+                                          float (&v)[kGridItems][3 + F]) {
+  const int lane = threadIdx.x & 31;
+  int cnt = 0;
+#pragma unroll
+  for (int it = 0; it < kGridItems; it++) {
+    const int p = base + it * 32 + lane;
+    const bool in = p < kept && keys[p] == key;
+    cnt += __popc(__ballot_sync(0xffffffffu, in));
+    const float4 q = in ? sorted4[p] : make_float4(0.f, 0.f, 0.f, 0.f);
+    v[it][0] = q.x; v[it][1] = q.y; v[it][2] = q.z;
+    if constexpr (F > 0) {
+      const float* rec = fa.in + (size_t)__float_as_uint(q.w) * fa.stride_f;
+#pragma unroll
+      for (int j = 0; j < F; j++) v[it][3 + j] = in ? rec[fa.off[j]] : 0.f;
+    }
+  }
+  return cnt;
+}
+
+// One warp per surviving voxel (grid-stride over the ranks), in rounds of kGridChunk sorted positions staged point-major in shared
+// memory; lane c < 3 + F adds channel c of the staged points in order while the next round's loads are in flight (a long run is
+// bound by its chain of adds, not by load latency).  The run ends at the first position with another key.  Nothing is written
+// when m > cap.
+template <int F>
+__global__ void __launch_bounds__(kGridWarps * 32, 1) k_grid_centroids(const unsigned* __restrict__ keys, const float4* __restrict__ sorted4, int kept,
+                                                                    const int* __restrict__ vstart, const unsigned* __restrict__ st, const FieldArgs fa,
+                                                                    float* __restrict__ out, size_t cap) {
+  constexpr int R = 3 + F, Row = R | 1;  // odd row length: the lanes' staging stores fall in distinct banks
+  __shared__ float buf[kGridWarps][kGridChunk * Row];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  float* b = buf[w];
+  const int m = (int)st[8];
+  if ((size_t)m > cap) return;
+  for (int r = blockIdx.x * kGridWarps + w; r < m; r += gridDim.x * kGridWarps) {
+    const int start = vstart[r];
+    const unsigned key = keys[start];
+    float v[kGridItems][R];
+    int cnt = grid_round<F>(keys, sorted4, kept, key, start, fa, v);
+    float s = 0.f;
+    int count = 0;
+    for (int base = start;; base += kGridChunk) {
+#pragma unroll
+      for (int it = 0; it < kGridItems; it++) {
+        if (it * 32 + lane < cnt) {
+#pragma unroll
+          for (int c = 0; c < R; c++) b[(it * 32 + lane) * Row + c] = v[it][c];
+        }
+      }
+      __syncwarp();
+      const int cur = cnt;
+      if (cur == kGridChunk) cnt = grid_round<F>(keys, sorted4, kept, key, base + kGridChunk, fa, v);
+      if (lane < R) {
+        if (cur == kGridChunk) {
+#pragma unroll 32
+          for (int q = 0; q < kGridChunk; q++) s = __fadd_rn(s, b[q * Row + lane]);
+        } else {
+          for (int q = 0; q < cur; q++) s = __fadd_rn(s, b[q * Row + lane]);
+        }
+      }
+      count += cur;
+      __syncwarp();
+      if (cur < kGridChunk) break;
+    }
+    if (lane < R) out[(size_t)r * R + lane] = __fdiv_rn(s, (float)count);
+  }
+}
+
 template <typename T>
 struct DevBuf {  // grow-only device array
   T* p = nullptr;
@@ -280,6 +505,13 @@ struct vgicp_prep_context {
   int* h_counts = nullptr;  // pinned
   DevBuf<float> fflushed;  // per-point fields: flushed field centroids [n][F]
   DevBuf<float> ftail;     // ... and those of the entries still holding a voxel [kHist][F]
+  // exact grid: sort keys and values (two buffers each), the sorted float4 payload, the sort scratch, the voxel starts
+  DevBuf<unsigned> gkeys[2], gvals[2];
+  DevBuf<float4> gsorted4;
+  DevBuf<unsigned char> gscratch;
+  DevBuf<int> gvstart;
+  unsigned* d_grid = nullptr;  // [kGridState]
+  unsigned* h_grid = nullptr;  // pinned
 };
 
 namespace {
@@ -310,6 +542,8 @@ int vgicp_prep_create(int device, vgicp_prep_handle* out) {
   ok = ok && cudaMalloc(&h->tail, kHist * sizeof(float4)) == cudaSuccess;
   ok = ok && cudaMalloc(&h->d_counts, 2 * sizeof(int)) == cudaSuccess;
   ok = ok && cudaMallocHost(&h->h_counts, 2 * sizeof(int)) == cudaSuccess;
+  ok = ok && cudaMalloc(&h->d_grid, kGridState * sizeof(unsigned)) == cudaSuccess;
+  ok = ok && cudaMallocHost(&h->h_grid, kGridState * sizeof(unsigned)) == cudaSuccess;
   if (!ok) {
     vgicp_prep_destroy(h);
     return 3;
@@ -327,6 +561,10 @@ void vgicp_prep_destroy(vgicp_prep_handle h) {
   }
   h->staging.release(); h->pts4.release(); h->entry.release(); h->flushed.release(); h->out.release(); h->chunk_state.release();
   h->fflushed.release(); h->ftail.release();
+  for (int k = 0; k < 2; k++) { h->gkeys[k].release(); h->gvals[k].release(); }
+  h->gsorted4.release(); h->gscratch.release(); h->gvstart.release();
+  if (h->d_grid) cudaFree(h->d_grid);
+  if (h->h_grid) cudaFreeHost(h->h_grid);
   if (h->tail) cudaFree(h->tail);
   if (h->d_counts) cudaFree(h->d_counts);
   if (h->h_counts) cudaFreeHost(h->h_counts);
@@ -356,21 +594,43 @@ cudaError_t launch_filter(vgicp_prep_handle h, const float* d_in, size_t stride_
   return cudaGetLastError();
 }
 
+// the device copy of the input: a host input is copied up to the last byte of the last record the filter reads
+cudaError_t stage_input(vgicp_prep_handle h, const float* points, size_t n, size_t stride_bytes, int on_device, const int* off, int F, const float** d_in) {
+  size_t span = 12;
+  for (int j = 0; j < F; j++) span = span > (size_t)off[j] * 4 + 4 ? span : (size_t)off[j] * 4 + 4;
+  *d_in = points;
+  if (on_device) return cudaSuccess;
+  cudaError_t e = h->staging.reserve(n * stride_bytes);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(h->staging.p, points, (n - 1) * stride_bytes + span, cudaMemcpyHostToDevice, h->stream);
+  *d_in = reinterpret_cast<const float*>(h->staging.p);
+  return e;
+}
+
+// a fresh epoch for the look-back state of `chunks` blocks (cleared when newly allocated or when the epoch wraps)
+cudaError_t next_chunk_epoch(vgicp_prep_handle h, int chunks) {
+  const unsigned long long* before = h->chunk_state.p;
+  cudaError_t e = h->chunk_state.reserve((size_t)chunks);
+  if (e != cudaSuccess) return e;
+  if (h->chunk_state.p != before) {  // fresh allocation: no stale epoch may match
+    e = cudaMemsetAsync(h->chunk_state.p, 0, h->chunk_state.cap * sizeof(unsigned long long), h->stream);
+    h->chunk_epoch = 0;
+  }
+  if (e == cudaSuccess && ++h->chunk_epoch == 0) {
+    e = cudaMemsetAsync(h->chunk_state.p, 0, h->chunk_state.cap * sizeof(unsigned long long), h->stream);
+    h->chunk_epoch = 1;
+  }
+  return e;
+}
+
 // both entry points: F = n_fields per-point fields at float offsets off[] (F = 0: x y z only)
 int run_filter(vgicp_prep_handle h, const char* who, const float* points, size_t n, size_t stride_bytes, int on_device, float leaf, int remove_near_origin, const int* off, int F,
                float* out, size_t cap, int out_on_device, size_t* n_out) {
   const std::string w(who);
   const size_t rec = 3 + (size_t)F;  // output floats per point
-  size_t span = 12;                  // bytes of a record the filter reads
-  for (int j = 0; j < F; j++) span = span > (size_t)off[j] * 4 + 4 ? span : (size_t)off[j] * 4 + 4;
   PREP_TRY(h, cudaSetDevice(h->device));
   const int ni = (int)n;
-  const float* d_in = points;
-  if (!on_device) {
-    PREP_TRY(h, h->staging.reserve(n * stride_bytes));
-    PREP_TRY(h, cudaMemcpyAsync(h->staging.p, points, (n - 1) * stride_bytes + span, cudaMemcpyHostToDevice, h->stream));
-    d_in = reinterpret_cast<const float*>(h->staging.p);
-  }
+  const float* d_in = nullptr;
+  PREP_TRY(h, stage_input(h, points, n, stride_bytes, on_device, off, F, &d_in));
   PREP_TRY(h, h->pts4.reserve(n));
   PREP_TRY(h, h->entry.reserve(n));
   PREP_TRY(h, h->flushed.reserve(n));
@@ -385,18 +645,7 @@ int run_filter(vgicp_prep_handle h, const char* who, const float* points, size_t
     d_out = h->out.p;
   }
   const int chunks = (ni + 1023) / 1024;
-  {
-    const unsigned long long* before = h->chunk_state.p;
-    PREP_TRY(h, h->chunk_state.reserve((size_t)chunks));
-    if (h->chunk_state.p != before) {  // fresh allocation: no stale epoch may match
-      PREP_TRY(h, cudaMemsetAsync(h->chunk_state.p, 0, h->chunk_state.cap * sizeof(unsigned long long), h->stream));
-      h->chunk_epoch = 0;
-    }
-    if (++h->chunk_epoch == 0) {
-      PREP_TRY(h, cudaMemsetAsync(h->chunk_state.p, 0, h->chunk_state.cap * sizeof(unsigned long long), h->stream));
-      h->chunk_epoch = 1;
-    }
-  }
+  PREP_TRY(h, next_chunk_epoch(h, chunks));
   const float inv_leaf = 1.0f / leaf;
   const size_t sf = stride_bytes / 4;
   const int flt = remove_near_origin ? 1 : 0;
@@ -417,6 +666,107 @@ int run_filter(vgicp_prep_handle h, const char* who, const float* points, size_t
   const size_t m = (size_t)h->h_counts[1];
   *n_out = m;
   if (m > cap) return fail(h, 1, w + ": output capacity too small (n points always suffice)");
+  if (!out_on_device && m > 0) {
+    PREP_TRY(h, cudaMemcpyAsync(out, d_out, m * rec * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+    PREP_TRY(h, cudaStreamSynchronize(h->stream));
+  }
+  return 0;
+}
+
+template <int F>
+cudaError_t launch_centroids(vgicp_prep_handle h, const float* d_in, size_t stride_f, const int* off, const unsigned* keys, int kept, int blocks, float* d_out, size_t out_cap) {
+  FieldArgs fa{};
+  fa.in = d_in;
+  fa.stride_f = stride_f;
+  for (int j = 0; j < F; j++) fa.off[j] = off[j];
+  k_grid_centroids<F><<<blocks, kGridWarps * 32, 0, h->stream>>>(keys, h->gsorted4.p, kept, h->gvstart.p, h->d_grid, fa, d_out, out_cap);
+  return cudaGetLastError();
+}
+
+int run_voxel_grid(vgicp_prep_handle h, const float* points, size_t n, size_t stride_bytes, int on_device, float leaf, int remove_near_origin, const int* off, int F,
+                   unsigned min_points, float* out, size_t cap, int out_on_device, size_t* n_out) {
+  using namespace vgicp;
+  const size_t rec = 3 + (size_t)F;
+  PREP_TRY(h, cudaSetDevice(h->device));
+  const int ni = (int)n;
+  const float* d_in = nullptr;
+  PREP_TRY(h, stage_input(h, points, n, stride_bytes, on_device, off, F, &d_in));
+  PREP_TRY(h, h->pts4.reserve(n));
+  for (int k = 0; k < 2; k++) {
+    PREP_TRY(h, h->gkeys[k].reserve(n));
+    PREP_TRY(h, h->gvals[k].reserve(n));
+  }
+  PREP_TRY(h, h->gsorted4.reserve(n));
+  const float inv = 1.0f / leaf;
+  const size_t sf = stride_bytes / 4;
+  const int flt = remove_near_origin ? 1 : 0;
+  // 1. the box of the kept points' cells, read back: the one host decision (refusals, key width) before the sort
+  PREP_TRY(h, cudaMemsetAsync(h->d_grid, 0, kGridState * sizeof(unsigned), h->stream));
+  const int bb = (ni + kGridBoxThreads - 1) / kGridBoxThreads;
+  k_grid_box<<<bb < 4 * kNumSMs ? bb : 4 * kNumSMs, kGridBoxThreads, 0, h->stream>>>(d_in, sf, ni, inv, flt, h->pts4.p, h->d_grid);
+  PREP_TRY(h, cudaGetLastError());
+  PREP_TRY(h, cudaMemcpyAsync(h->h_grid, h->d_grid, kGridState * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
+  PREP_TRY(h, cudaStreamSynchronize(h->stream));
+  if (h->h_grid[7]) return fail(h, 1, "voxel_grid: a kept point's cell floor(x / leaf) lies outside the int range");
+  const int kept = (int)h->h_grid[6];
+  if (kept == 0) return 0;
+  int lo[3];
+  long long div[3];
+  for (int a = 0; a < 3; a++) {
+    lo[a] = grid_dec(~h->h_grid[a]);
+    div[a] = (long long)grid_dec(h->h_grid[3 + a]) - lo[a] + 1;
+  }
+  const long long lim = 0x7fffffff;
+  if (div[0] > lim || div[1] > lim / div[0] || div[2] > lim / (div[0] * div[1]))
+    return fail(h, 1, "voxel_grid: the leaf is too small for the extent of the cloud (more than INT32_MAX cells in the box)");
+  const unsigned V = (unsigned)(div[0] * div[1] * div[2]);  // the voxel count, and the key of a dropped point
+  const int key_bits = 32 - __builtin_clz(V);
+  const int passes = sort_num_passes(key_bits);
+  // 2. keys + digit histograms, the sort carrying x y z and the input index
+  const size_t sb = sort_scratch_bytes(ni, passes);
+  PREP_TRY(h, h->gscratch.reserve(sb));
+  PREP_TRY(h, cudaMemsetAsync(h->gscratch.p, 0, sb, h->stream));
+  const int hb = (ni + kSortThreads * 8 - 1) / (kSortThreads * 8);
+  k_grid_keys<<<hb < 4 * kNumSMs ? hb : 4 * kNumSMs, kSortThreads, 0, h->stream>>>(h->pts4.p, ni, inv, flt, make_int3(lo[0], lo[1], lo[2]), (unsigned)div[0],
+                                                                                   (unsigned)(div[0] * div[1]), V, passes, h->gkeys[0].p,
+                                                                                   reinterpret_cast<unsigned*>(h->gscratch.p));
+  PREP_TRY(h, cudaGetLastError());
+  PREP_TRY(h, launch_sort_pairs<unsigned>(h->gkeys[0].p, h->gvals[0].p, h->gkeys[1].p, h->gvals[1].p, ni, key_bits, h->gscratch.p, true, h->pts4.p, h->gsorted4.p, nullptr,
+                                          h->stream));
+  const unsigned* keys = h->gkeys[passes & 1].p;
+  // 3. the voxels that reach the minimum, ranked; 4. their centroids
+  const int chunks = (kept + 1023) / 1024;
+  PREP_TRY(h, next_chunk_epoch(h, chunks));
+  PREP_TRY(h, h->gvstart.reserve((size_t)kept));
+  k_grid_heads<<<chunks, 1024, 0, h->stream>>>(keys, kept, min_points, h->chunk_state.p, h->chunk_epoch, h->gvstart.p, h->d_grid);
+  PREP_TRY(h, cudaGetLastError());
+  float* d_out = out;
+  size_t out_cap = cap;
+  if (!out_on_device) {
+    PREP_TRY(h, h->out.reserve(rec * kept));
+    d_out = h->out.p;
+    out_cap = (size_t)kept;  // m <= kept; the cap itself is checked on the host before anything is copied back
+  }
+  const long long most = (long long)kept / (min_points > 1 ? min_points : 1);  // voxels that can reach the minimum
+  const long long cb = (most < (long long)V ? most : (long long)V) + kGridWarps - 1;
+  const int cblocks = (int)(cb / kGridWarps < 16 * kNumSMs ? (cb / kGridWarps > 0 ? cb / kGridWarps : 1) : 16 * kNumSMs);
+  switch (F) {
+    case 0: PREP_TRY(h, (launch_centroids<0>(h, d_in, sf, off, keys, kept, cblocks, d_out, out_cap))); break;
+    case 1: PREP_TRY(h, (launch_centroids<1>(h, d_in, sf, off, keys, kept, cblocks, d_out, out_cap))); break;
+    case 2: PREP_TRY(h, (launch_centroids<2>(h, d_in, sf, off, keys, kept, cblocks, d_out, out_cap))); break;
+    case 3: PREP_TRY(h, (launch_centroids<3>(h, d_in, sf, off, keys, kept, cblocks, d_out, out_cap))); break;
+    case 4: PREP_TRY(h, (launch_centroids<4>(h, d_in, sf, off, keys, kept, cblocks, d_out, out_cap))); break;
+    case 5: PREP_TRY(h, (launch_centroids<5>(h, d_in, sf, off, keys, kept, cblocks, d_out, out_cap))); break;
+    case 6: PREP_TRY(h, (launch_centroids<6>(h, d_in, sf, off, keys, kept, cblocks, d_out, out_cap))); break;
+    case 7: PREP_TRY(h, (launch_centroids<7>(h, d_in, sf, off, keys, kept, cblocks, d_out, out_cap))); break;
+    case 8: PREP_TRY(h, (launch_centroids<8>(h, d_in, sf, off, keys, kept, cblocks, d_out, out_cap))); break;
+    default: return fail(h, 1, "voxel_grid: unsupported field count");
+  }
+  PREP_TRY(h, cudaMemcpyAsync(h->h_grid + 8, h->d_grid + 8, sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
+  PREP_TRY(h, cudaStreamSynchronize(h->stream));
+  const size_t m = h->h_grid[8];
+  *n_out = m;
+  if (m > cap) return fail(h, 1, "voxel_grid: output capacity too small (n points always suffice)");
   if (!out_on_device && m > 0) {
     PREP_TRY(h, cudaMemcpyAsync(out, d_out, m * rec * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
     PREP_TRY(h, cudaStreamSynchronize(h->stream));
@@ -461,6 +811,28 @@ int vgicp_prep_approximate_voxel_grid_fields(vgicp_prep_handle h, const float* p
   if (!(leaf > 0.f)) return fail(h, 1, "approximate_voxel_grid_fields: leaf size must be positive");
   if (n > (size_t)0x7fffffff - 4096) return fail(h, 1, "approximate_voxel_grid_fields: too many points");
   return run_filter(h, "approximate_voxel_grid_fields", points, n, stride_bytes, on_device, leaf, remove_near_origin, off, n_fields, out, cap, out_on_device, n_out);
+}
+
+int vgicp_prep_voxel_grid(vgicp_prep_handle h, const float* points, size_t n, size_t stride_bytes, int on_device, float leaf, int remove_near_origin, const size_t* field_offsets,
+                          int n_fields, unsigned min_points_per_voxel, float* out, size_t cap, int out_on_device, size_t* n_out) {
+  if (!h) return 1;
+  if (!n_out) return fail(h, 1, "voxel_grid: n_out is null");
+  *n_out = 0;
+  if (n_fields < 0 || n_fields > kMaxFields) return fail(h, 1, "voxel_grid: n_fields must be 0 ... 8");
+  if (n_fields > 0 && !field_offsets) return fail(h, 1, "voxel_grid: null field_offsets");
+  if (stride_bytes < 12 || stride_bytes % 4) return fail(h, 1, "voxel_grid: stride must be >= 12 and a multiple of 4");
+  int off[kMaxFields];
+  for (int j = 0; j < n_fields; j++) {
+    const size_t o = field_offsets[j];
+    if (o % 4 || o < 12 || o > stride_bytes - 4)
+      return fail(h, 1, "voxel_grid: a field offset must be a multiple of 4, >= 12 and leave 4 bytes within the stride");
+    off[j] = (int)(o / 4);
+  }
+  if (!(leaf > 0.f) || !std::isfinite(leaf)) return fail(h, 1, "voxel_grid: leaf size must be finite and positive");
+  if (n == 0) return 0;
+  if (!points || !out) return fail(h, 1, "voxel_grid: null buffer");
+  if (n > (size_t)0x7fffffff - 4096) return fail(h, 1, "voxel_grid: too many points");
+  return run_voxel_grid(h, points, n, stride_bytes, on_device, leaf, remove_near_origin, off, n_fields, min_points_per_voxel, out, cap, out_on_device, n_out);
 }
 
 }  // extern "C"

@@ -54,6 +54,34 @@ VGICP_PREP_API int vgicp_prep_approximate_voxel_grid(vgicp_prep_handle h, const 
 VGICP_PREP_API int vgicp_prep_approximate_voxel_grid_fields(vgicp_prep_handle h, const float* points, size_t n, size_t stride_bytes, int on_device, float leaf,
                                                             int remove_near_origin, const size_t* field_offsets, int n_fields, float* out, size_t cap, int out_on_device,
                                                             size_t* n_out);
+/* pcl::VoxelGrid, the exact grid: one centroid per occupied voxel, x y z and n_fields per-point float fields (0 ... 8) averaged over
+ * the voxel.  Unlike the approximate filter its output does not depend on the order of the input points.
+ *   points, n, stride_bytes, on_device, remove_near_origin, field_offsets, out, cap, out_on_device, n_out: as for
+ *                  vgicp_prep_approximate_voxel_grid_fields (field_offsets may be null when n_fields is 0); the output is m records of
+ *                  3 + n_fields floats, the layout vgicp_set_source_cloud_device and vgicp_set_source_timestamps_device read in place.
+ *   min_points_per_voxel  voxels with fewer points are dropped (pcl::VoxelGrid::setMinimumPointsNumberPerVoxel; 0 and 1 keep all).
+ * Recipe (every float operation one IEEE single operation, no contraction):
+ *   1. kept points: x, y and z finite (a non-dense pcl::VoxelGrid drops the others) and, when remove_near_origin is set, not
+ *      ((x*x + y*y) + z*z) < 1e-3f.  Dropped points neither widen the box nor land in a voxel.
+ *   2. cells: inv = 1.0f / leaf; per axis c = floorf(x * inv) (one multiplication).  A kept c outside [-2^31, 2^31) refuses the
+ *      call; otherwise g = (int)c.
+ *   3. box: min_b, max_b = per-axis min and max of g over the kept points; div = max_b - min_b + 1 in int64.  A cell product
+ *      div_x * div_y * div_z > INT32_MAX refuses the call (pcl::VoxelGrid has the same guard but silently returns its input
+ *      instead; refusing is deliberate).  x * inv is monotone in x, so min_b is PCL's floor(min_p * inv).
+ *   4. voxel index: idx = (g_x - min_b_x) + (g_y - min_b_y) * div_x + (g_z - min_b_z) * div_x * div_y in integers.  PCL subtracts in
+ *      float; the two differ only where |x / leaf| >= 2^24, where PCL's index can be wrong.
+ *   5. a voxel is a run of equal idx; voxels with fewer than min_points_per_voxel points are dropped; the output is in ascending
+ *      idx order (PCL's).
+ *   6. centroids: for x, y, z and each field, s = 0.0f, then s = s + v over the voxel's points in ascending input index, then
+ *      s / (float)count.  This is PCL's Vector4f accumulation with the order inside a voxel, which PCL's std::sort leaves
+ *      unspecified, fixed to input order.  Non-finite field values propagate (a NaN result is a NaN; its payload is not pinned).
+ *   7. no kept point, or no voxel with enough points: status 0 and *n_out = 0.
+ * Status 1 with nothing written to out and *n_out = 0: a null handle, n_out or buffer, a bad stride, offset or field count, a leaf
+ * that is not finite and positive, n > INT32_MAX - 4096, a cell outside the int range or a cell product above INT32_MAX.  Status 1
+ * with *n_out = m (out untouched) when m > cap.  3 on a CUDA error.  Blocks until the result is in place. */
+VGICP_PREP_API int vgicp_prep_voxel_grid(vgicp_prep_handle h, const float* points, size_t n, size_t stride_bytes, int on_device, float leaf,
+                                         int remove_near_origin, const size_t* field_offsets, int n_fields, unsigned min_points_per_voxel,
+                                         float* out, size_t cap, int out_on_device, size_t* n_out);
 #ifdef __cplusplus
 }
 #endif
