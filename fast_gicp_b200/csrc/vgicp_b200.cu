@@ -137,6 +137,54 @@ struct VoxelMap {
   }
 };
 
+// Where the evaluation kernels leave their results: `rows` records of `len` doubles, with the partial sums and tickets of their
+// fixed-order fold.  Latency hint: the kernels write the records to mapped host memory and then set each row's completion word to
+// the launch's sequence number, on which the host spins; throughput hint: the records go to device memory and are copied back.
+struct EvalChannel {
+  int rows = 0;
+  size_t len = 0;
+  DevBuf<double> partials;
+  unsigned int* tickets = nullptr;           // [rows]: zero before the first launch; reset by each row's last block
+  double* d_out = nullptr;                   // [rows][len] (throughput hint)
+  double* h_out = nullptr;                   // pinned + mapped, same shape (latency hint)
+  unsigned long long* h_done = nullptr;      // pinned + mapped per-row completion words
+  unsigned long long seq = 0;                // the current launch's (or round's) sequence number
+  struct Dest {
+    double* out;
+    volatile unsigned long long* done;  // nullptr under the throughput hint
+    unsigned long long seq;
+  };
+
+  // fixed-size buffers at the first call; the partial sums grow
+  cudaError_t open(int n_rows, size_t rec_len, size_t n_partials, cudaStream_t st) {
+    if (!h_out) {
+      rows = n_rows;
+      len = rec_len;
+      cudaError_t e = cudaMalloc(&tickets, rows * sizeof(unsigned int));
+      if (e == cudaSuccess) e = cudaMemsetAsync(tickets, 0, rows * sizeof(unsigned int), st);
+      if (e == cudaSuccess) e = cudaMalloc(&d_out, rows * len * sizeof(double));
+      if (e == cudaSuccess) e = cudaHostAlloc(&h_done, rows * sizeof(unsigned long long), cudaHostAllocMapped);
+      if (e == cudaSuccess) memset(h_done, 0, rows * sizeof(unsigned long long));
+      if (e == cudaSuccess) e = cudaHostAlloc(&h_out, rows * len * sizeof(double), cudaHostAllocMapped);  // (last: it marks the set as complete)
+      if (e != cudaSuccess) return e;
+    }
+    return partials.reserve(n_partials);
+  }
+  void release() {
+    partials.release();
+    if (tickets) cudaFree(tickets);
+    if (d_out) cudaFree(d_out);
+    if (h_out) cudaFreeHost(h_out);
+    if (h_done) cudaFreeHost(h_done);
+    *this = EvalChannel();
+  }
+  // where a launch writes rows [row0, ...) under the execution hint
+  Dest dest(bool direct, int row0 = 0) const {
+    return {(direct ? h_out : d_out) + (size_t)row0 * len, direct ? h_done + row0 : nullptr, seq};
+  }
+  int wait(vgicp_handle h, int n, size_t count);
+};
+
 }  // namespace
 
 struct vgicp_context {
@@ -177,23 +225,14 @@ struct vgicp_context {
   int stage1_sharding = 0;
   int speculate = 1;  // LM trial evaluations also linearise at the trial pose (vgicp_set_speculation)
   int exec_hint = 0;  // 0 = latency (one registration should finish as soon as possible), 1 = throughput (many concurrent handles)
-  DevBuf<double> partials;
   DevBuf<int> corr_ids;
-  unsigned int* d_ticket = nullptr;
-  double* d_out = nullptr;    // 43 doubles
-  double* h_out = nullptr;    // pinned + mapped: in latency mode the kernel's last block writes the result straight here
-  unsigned long long* h_flag = nullptr;  // pinned + mapped completion word
-  unsigned long long eval_seq = 0;
-  // multi-pose evaluations (vgicp_align_multi / vgicp_evaluate_poses) have buffers of their own, so that they leave every piece
-  // of single-pose state (lin, partials, d_out, h_out, eval_seq) as it was; allocated at the first multi-pose call
-  DevBuf<double> multi_partials;            // [rows][grid][kLinStride]
-  unsigned int* d_multi_tickets = nullptr;  // [kMultiMaxHyp]
+  EvalChannel eval;  // single-pose evaluations: one record of 64 doubles (43 used, [44] the sharded exchange's error flag)
+  // multi-pose evaluations (vgicp_align_multi / vgicp_evaluate_poses) have a channel of their own, so that they leave every piece
+  // of single-pose state (lin, eval) as it was; opened at the first multi-pose call: [kMultiMaxHyp][kMultiOut], partials
+  // [rows][grid][kLinStride]
+  EvalChannel multi;
   unsigned char* d_multi_in = nullptr;      // per-launch input: poses [hypotheses][2], then the row -> hypothesis list
   unsigned char* h_multi_in = nullptr;      // pinned staging of d_multi_in
-  double* d_multi_out = nullptr;            // [kMultiMaxHyp][kMultiOut] (throughput hint)
-  double* h_multi_out = nullptr;            // pinned + mapped, same shape (latency hint: written by the kernels directly)
-  unsigned long long* h_multi_done = nullptr;  // pinned + mapped per-row completion words
-  unsigned long long multi_seq = 0;
 
   // NDT (NDTCudaCore, ndt_cuda.cu): 0 = VGICP problem, 1 = NDT point-to-distribution, 2 = NDT distribution-to-distribution
   int problem = 0;
@@ -238,17 +277,13 @@ struct vgicp_context {
   } s1;
 
   // continuous-time registration (vgicp_set_source_timestamps, vgicp_compute_error_ct, vgicp_align_ct): the source's timestamps and
-  // buffers of its own for the evaluation, so that it leaves the single-pose state as it was; allocated at first use
+  // a channel of its own for the evaluation, so that it leaves the single-pose state as it was; opened at first use: one record of
+  // kCtStride doubles, partials [kLinMaxBlocks][kCtStride]
   bool ct_has_times = false;
   float ct_tau = 0.0f;    // (float)t_ref
   double ct_span = 0.0;   // S = max_i |t_i - tau| (float differences)
   DevBuf<float> ct_times;
-  DevBuf<double> ct_partials;            // [kLinMaxBlocks][kCtStride]
-  unsigned int* d_ct_ticket = nullptr;
-  double* d_ct_out = nullptr;            // [kCtStride] (throughput hint)
-  double* h_ct_out = nullptr;            // pinned + mapped, same shape (latency hint: written by the kernel directly)
-  unsigned long long* h_ct_done = nullptr;  // pinned + mapped completion word
-  unsigned long long ct_seq = 0;
+  EvalChannel ct;
 
   // timestamps from device memory and the deskew with the stored ones (vgicp_set_source_timestamps_device,
   // vgicp_deskew_source_stored): the raw range and t_ref kept with the timestamps, so that the stored deskew applies
@@ -720,7 +755,7 @@ LinLaunch make_lin_launch(vgicp_handle h, bool allow_stream = true) {
   if (h->voxel_index_mode != 0) a.dense.cells = nullptr;
   a.offsets = h->d_offsets.p; a.n_off = (int)h->h_offsets.size(); a.res = m.res;
   a.Tlin = h->lin; a.Teval = h->lin;
-  a.partials = h->partials.p; a.ticket = h->d_ticket; a.out = h->d_out;
+  a.partials = h->eval.partials.p; a.ticket = h->eval.tickets; a.out = h->eval.d_out;
   a.done_flag = nullptr; a.done_seq = 0;
   // lanes per source point in the lookup phase: split the neighbour cells of a point over G lanes while the cloud is too small to
   // fill the GPU with one thread per point (latency-bound regime); one lane per point once it is large
@@ -744,67 +779,36 @@ LinLaunch make_lin_launch(vgicp_handle h, bool allow_stream = true) {
   return L;
 }
 
-enum { kEvalLinearize = 0, kEvalError = 1, kEvalSpec = 2 };  // what an evaluation launch computes (every row of a multi-pose one alike)
-
 template <int V>
 using IntC = std::integral_constant<int, V>;
 
-// Calls f(WHAT, RB) with the streaming kernels' WHAT for an evaluation kind (0 error, 1 linearisation, 2 speculative) and RB (robust
-// weights) as compile-time constants.
-template <class F>
-void with_stream_kernel(int kind, bool robust, F&& f) {
-  auto what = [&](auto rb) {
-    if (kind == kEvalSpec) f(IntC<2>{}, rb);
-    else if (kind == kEvalLinearize) f(IntC<1>{}, rb);
-    else f(IntC<0>{}, rb);
-  };
-  if (robust) what(std::true_type{});
-  else what(std::false_type{});
-}
-
 // The compacted evaluation kernels that exist: offset table MODE (1 / 7 / 27, 0 = generic list) with the lanes per point G that
-// make_lin_launch picks for it.  Calls f(MODE, G, RB) as compile-time constants; false when (mode, G) is not in the table.
+// make_lin_launch picks for it.  Calls f(MODE, G) as compile-time constants; false when (mode, G) is not in the table.
 template <int M, int GG>
 struct LinShape { static constexpr int MODE = M, G = GG; };
-template <class F, class RB, class... S>
-bool with_lin_shape(int mode, int G, F& f, RB rb, S...) {
-  return ((S::MODE == mode && S::G == G && (f(IntC<S::MODE>{}, IntC<S::G>{}, rb), true)) || ...);
+template <class F, class... S>
+bool with_shape(int mode, int G, F& f, S...) {
+  return ((S::MODE == mode && S::G == G && (f(IntC<S::MODE>{}, IntC<S::G>{}), true)) || ...);
 }
 template <class F>
-bool with_lin_kernel(int mode, int G, bool robust, F&& f) {
-  auto table = [&](auto rb) {
-    return with_lin_shape(mode, G, f, rb, LinShape<1, 1>{}, LinShape<7, 1>{}, LinShape<7, 4>{}, LinShape<27, 1>{}, LinShape<27, 3>{},
-                          LinShape<0, 1>{}, LinShape<0, 4>{}, LinShape<0, 8>{});
-  };
-  return robust ? table(std::true_type{}) : table(std::false_type{});
+bool with_lin_shape(int mode, int G, F&& f) {
+  return with_shape(mode, G, f, LinShape<1, 1>{}, LinShape<7, 1>{}, LinShape<7, 4>{}, LinShape<27, 1>{}, LinShape<27, 3>{}, LinShape<0, 1>{},
+                    LinShape<0, 4>{}, LinShape<0, 8>{});
 }
 
-// one evaluation: launches the fused lookup+derivative kernel at Teval over the correspondences of h->lin
-int launch_linearize(vgicp_handle h, const Pose& Teval, int kind) {
-  const bool want_H = kind != kEvalError, spec = kind == kEvalSpec;
-  LinLaunch L = make_lin_launch(h);
-  LinArgs& a = L.a;
-  a.Teval = Teval;
-  a.comm_seq = h->comm_seq++;
-  if (h->exec_hint == 0) {  // latency: the result goes straight to mapped host memory (UVA: the pinned pointers are valid on the device)
-    a.out = h->h_out;
-    a.done_flag = h->h_flag;
-    a.done_seq = ++h->eval_seq;
-  }
-  prof_begin(h, want_H ? VGICP_PROF_LINEARIZE : VGICP_PROF_ERROR, h->stream);
-  bool launched = true;
-  if (L.stream)
-    with_stream_kernel(kind, a.robust, [&](auto what, auto rb) {
-      k_linearize_stream<decltype(what)::value, decltype(rb)::value><<<L.grid, kLinThreads, sizeof(LinStreamSmem), h->stream>>>(a);
-    });
-  else
-    launched = with_lin_kernel(h->offset_mode, L.G, a.robust, [&](auto mode, auto g, auto rb) {
-      constexpr int MODE = decltype(mode)::value, G = decltype(g)::value;
-      constexpr bool RB = decltype(rb)::value;
-      if (spec) k_linearize_spec<MODE, G, RB><<<L.grid, kLinThreads, 0, h->stream>>>(a);
-      else if (want_H) k_linearize<MODE, true, G, RB><<<L.grid, kLinThreads, 0, h->stream>>>(a);
-      else k_linearize<MODE, false, G, RB><<<L.grid, kLinThreads, 0, h->stream>>>(a);
-    });
+// Every evaluation launch: profiled under its kind's category and counted.  launch(WHAT, RB) gets the evaluation kind and the
+// robust flag as compile-time constants, launches the kernel and returns false when none exists for the shape.
+template <class F>
+int launch_eval(vgicp_handle h, int kind, bool robust, F&& launch) {
+  prof_begin(h, kind == kEvalError ? VGICP_PROF_ERROR : VGICP_PROF_LINEARIZE, h->stream);
+  bool launched;
+  auto with_kind = [&](auto rb) {
+    if (kind == kEvalSpec) launched = launch(IntC<kEvalSpec>{}, rb);
+    else if (kind == kEvalLinearize) launched = launch(IntC<kEvalLinearize>{}, rb);
+    else launched = launch(IntC<kEvalError>{}, rb);
+  };
+  if (robust) with_kind(std::true_type{});
+  else with_kind(std::false_type{});
   prof_end(h, h->stream);
   if (!launched) return fail(h, VGICP_ERR_UNSUPPORTED, "no evaluation kernel for this offset table and lane split");
   h->launches++;
@@ -812,22 +816,56 @@ int launch_linearize(vgicp_handle h, const Pose& Teval, int kind) {
   return VGICP_OK;
 }
 
-// a robust kind is defined for the VGICP problem only: NDT carries its own Cauchy weight
-int check_robust_problem(vgicp_handle h, const char* who) {
-  if (h->problem != 0 && h->robust_kind != VGICP_ROBUST_NONE)
-    return fail(h, VGICP_ERR_UNSUPPORTED, std::string(who) + ": a robust kernel is set (vgicp_set_robust_kernel) and an NDT problem is selected; NDT has its own weight");
-  return VGICP_OK;
+// one evaluation: launches the fused lookup+derivative kernel at Teval over the correspondences of h->lin
+int launch_linearize(vgicp_handle h, const Pose& Teval, int kind) {
+  LinLaunch L = make_lin_launch(h);
+  LinArgs& a = L.a;
+  a.Teval = Teval;
+  a.comm_seq = h->comm_seq++;
+  h->eval.seq++;
+  // latency hint: the result goes straight to mapped host memory (UVA: the pinned pointers are valid on the device)
+  const EvalChannel::Dest d = h->eval.dest(h->exec_hint == 0);
+  a.out = d.out; a.done_flag = d.done; a.done_seq = d.seq;
+  return launch_eval(h, kind, a.robust, [&](auto what, auto rb) {
+    constexpr int WHAT = decltype(what)::value;
+    constexpr bool RB = decltype(rb)::value;
+    if (L.stream) {
+      k_linearize_stream<WHAT, RB><<<L.grid, kLinThreads, sizeof(LinStreamSmem), h->stream>>>(a);
+      return true;
+    }
+    return with_lin_shape(h->offset_mode, L.G, [&](auto mode, auto g) {
+      k_linearize<decltype(mode)::value, WHAT, decltype(g)::value, RB><<<L.grid, kLinThreads, 0, h->stream>>>(a);
+    });
+  });
 }
 
-int check_ready_for_eval(vgicp_handle h, const char* who) {
+// What an entry point needs before it launches anything.  The conditions are tested in this order, and the first one that does
+// not hold is the error: a robust kind with NDT (kNeedEval) or continuous time with NDT (kNeedCt); a multi-GPU communicator
+// (kNeedOneGpu) or any sharding (kNeedCt); the clouds (VGICP: source points, their covariances with kNeedEval, the voxel map; NDT:
+// source and target points); the linearisation point (kNeedLin); the source's timestamps (kNeedCt).
+enum : unsigned {
+  kNeedEval = 1,    // evaluates residuals: a robust kind must fit the problem (NDT has its own Cauchy weight), covariances (VGICP)
+  kNeedLin = 2,     // the correspondences of vgicp_update_correspondences
+  kNeedOneGpu = 4,  // not in a multi-GPU communicator
+  kNeedCt = 8,      // continuous time: VGICP on one GPU without sharding, with the source's timestamps
+};
+int check_ready(vgicp_handle h, const char* who, unsigned need) {
+  const std::string w(who);
+  if ((need & kNeedCt) && h->problem != 0) return fail(h, VGICP_ERR_UNSUPPORTED, w + ": continuous-time registration is defined for the VGICP problem only");
+  if ((need & kNeedEval) && h->problem != 0 && h->robust_kind != VGICP_ROBUST_NONE)
+    return fail(h, VGICP_ERR_UNSUPPORTED, w + ": a robust kernel is set (vgicp_set_robust_kernel) and an NDT problem is selected; NDT has its own weight");
+  if ((need & kNeedOneGpu) && h->comm_ranks > 1) return fail(h, VGICP_ERR_UNSUPPORTED, w + ": not available on a handle in a multi-GPU communicator");
+  if ((need & kNeedCt) && (h->comm_ranks > 1 || h->stage1_sharding || h->shard_end >= 0))
+    return fail(h, VGICP_ERR_UNSUPPORTED, w + ": not available with source or stage-1 sharding or in a multi-GPU communicator");
   if (h->problem != 0) {
-    if (!h->source.has_pts || !h->target.has_pts) return fail(h, VGICP_ERR_BAD_STATE, std::string(who) + ": NDT needs source and target clouds");
-    if (!h->has_lin) return fail(h, VGICP_ERR_BAD_STATE, std::string(who) + ": update_correspondences has not been called");
-    return VGICP_OK;
+    if (!h->source.has_pts || !h->target.has_pts) return fail(h, VGICP_ERR_BAD_STATE, w + ": NDT needs source and target clouds");
+  } else {
+    if (!h->source.has_pts) return fail(h, VGICP_ERR_BAD_STATE, w + ": source cloud not set");
+    if ((need & kNeedEval) && !h->source.has_cov) return fail(h, VGICP_ERR_BAD_STATE, w + ": source covariances required");
+    if (!h->map.built && !h->map.pending) return fail(h, VGICP_ERR_BAD_STATE, w + ": target voxel map not built");
   }
-  if (!h->source.has_pts || !h->source.has_cov) return fail(h, VGICP_ERR_BAD_STATE, std::string(who) + ": source points and covariances required");
-  if (!h->map.built && !h->map.pending) return fail(h, VGICP_ERR_BAD_STATE, std::string(who) + ": target voxel map not built");
-  if (!h->has_lin) return fail(h, VGICP_ERR_BAD_STATE, std::string(who) + ": update_correspondences has not been called");
+  if ((need & kNeedLin) && !h->has_lin) return fail(h, VGICP_ERR_BAD_STATE, w + ": update_correspondences has not been called");
+  if ((need & kNeedCt) && !h->ct_has_times) return fail(h, VGICP_ERR_BAD_STATE, w + ": the source has no timestamps (vgicp_set_source_timestamps)");
   return VGICP_OK;
 }
 
@@ -876,11 +914,11 @@ int ndt_prepare(vgicp_handle h) {
   return VGICP_OK;
 }
 
-// Waits for the records of the launch just enqueued and leaves them in `host`.  Latency hint: the kernels write them to mapped host
-// memory and then set the completion words done[0, n) to seq, on which the host spins; throughput hint: `count` doubles are copied
-// back from `dev` behind the launch.
-int wait_records(vgicp_handle h, const volatile unsigned long long* done, int n, unsigned long long seq, double* host, const double* dev, size_t count) {
+// Waits for rows [0, n) of the launch (or round) just enqueued and leaves their records in h_out: under the latency hint by spinning
+// on the completion words, under the throughput hint by copying `count` doubles back behind the launch.
+int EvalChannel::wait(vgicp_handle h, int n, size_t count) {
   if (h->exec_hint == 0) {
+    const volatile unsigned long long* done = h_done;
     for (int r = 0; r < n; r++) {
       long spins = 0;
       while (done[r] != seq) {
@@ -894,7 +932,7 @@ int wait_records(vgicp_handle h, const volatile unsigned long long* done, int n,
     }
     __sync_synchronize();
   } else {
-    CU_TRY(h, cudaMemcpyAsync(host, dev, count * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+    CU_TRY(h, cudaMemcpyAsync(h_out, d_out, count * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
     CU_TRY(h, cudaStreamSynchronize(h->stream));
   }
   return VGICP_OK;
@@ -906,40 +944,21 @@ int evaluate(vgicp_handle h, const Pose& Teval, int kind, const double** rec) {
   int rc = launch_linearize(h, Teval, kind);
   if (rc) return rc;
   const size_t count = (h->comm_ranks > 1 || kind == kEvalSpec) ? kLinOutCommError + 1 : (kind == kEvalLinearize ? 43 : 1);
-  if ((rc = wait_records(h, h->h_flag, 1, h->eval_seq, h->h_out, h->d_out, count))) return rc;
-  if (h->comm_ranks > 1 && h->h_out[kLinOutCommError] != 0.0) return fail(h, VGICP_ERR_COMM, "evaluate: a peer rank did not deliver its sums in time (vgicp_comm_error)");
-  *rec = h->h_out;
+  if ((rc = h->eval.wait(h, 1, count))) return rc;
+  if (h->comm_ranks > 1 && h->eval.h_out[kLinOutCommError] != 0.0) return fail(h, VGICP_ERR_COMM, "evaluate: a peer rank did not deliver its sums in time (vgicp_comm_error)");
+  *rec = h->eval.h_out;
   return VGICP_OK;
 }
 
 // ---- multi-pose evaluation (vgicp_align_multi, vgicp_evaluate_poses) -------------------------------------------------------
-// the preconditions of vgicp_align, for the calls that evaluate many poses
-int check_ready_for_multi(vgicp_handle h, const char* who) {
-  if (h->comm_ranks > 1) return fail(h, VGICP_ERR_UNSUPPORTED, std::string(who) + ": not available on a handle in a multi-GPU communicator");
-  if (h->problem == 0) {
-    if (!h->source.has_pts || !h->source.has_cov) return fail(h, VGICP_ERR_BAD_STATE, std::string(who) + ": source points and covariances required");
-    if (!h->map.built && !h->map.pending) return fail(h, VGICP_ERR_BAD_STATE, std::string(who) + ": target voxel map not built");
-  } else if (!h->source.has_pts || !h->target.has_pts) {
-    return fail(h, VGICP_ERR_BAD_STATE, std::string(who) + ": NDT needs source and target clouds");
-  }
-  return VGICP_OK;
-}
-
 // fixed-size buffers on first use; the partial sums grow with rows x grid (256 bytes per block and row)
 int multi_reserve(vgicp_handle h, int rows, int grid) {
-  if (!h->h_multi_out) {
+  if (!h->h_multi_in) {
     const size_t in_bytes = (size_t)kMultiMaxHyp * (2 * sizeof(Pose) + sizeof(int)) + 16;
-    const size_t out_bytes = (size_t)kMultiMaxHyp * kMultiOut * sizeof(double);
-    CU_TRY(h, cudaMalloc(&h->d_multi_tickets, kMultiMaxHyp * sizeof(unsigned int)));
-    CU_TRY(h, cudaMemsetAsync(h->d_multi_tickets, 0, kMultiMaxHyp * sizeof(unsigned int), h->stream));
     CU_TRY(h, cudaMalloc(&h->d_multi_in, in_bytes));
-    CU_TRY(h, cudaMallocHost(&h->h_multi_in, in_bytes));
-    CU_TRY(h, cudaMalloc(&h->d_multi_out, out_bytes));
-    CU_TRY(h, cudaHostAlloc(&h->h_multi_done, kMultiMaxHyp * sizeof(unsigned long long), cudaHostAllocMapped));
-    memset(h->h_multi_done, 0, kMultiMaxHyp * sizeof(unsigned long long));
-    CU_TRY(h, cudaHostAlloc(&h->h_multi_out, out_bytes, cudaHostAllocMapped));  // (last: it marks the set as complete)
+    CU_TRY(h, cudaMallocHost(&h->h_multi_in, in_bytes));  // (last: it marks the pair as complete)
   }
-  CU_TRY(h, h->multi_partials.reserve((size_t)rows * grid * kLinStride));
+  CU_TRY(h, h->multi.open(kMultiMaxHyp, kMultiOut, (size_t)rows * grid * kLinStride, h->stream));
   return VGICP_OK;
 }
 
@@ -957,48 +976,29 @@ int multi_upload(vgicp_handle h, int n_hyp, int n_rows) {
 // of the multi-pose output.  count: also count the hits (kEvalLinearize / kEvalError only).
 int launch_multi(vgicp_handle h, const LinLaunch& L, int n_hyp, int kind, bool count, int row0, int n) {
   const LinArgs& a = L.a;
-  const bool direct = h->exec_hint == 0;
+  const EvalChannel::Dest d = h->multi.dest(h->exec_hint == 0, row0);
   MultiArgs m;
   m.hyp = reinterpret_cast<const int*>(h->d_multi_in + multi_rows_offset(n_hyp)) + row0;
   m.poses = reinterpret_cast<const Pose*>(h->d_multi_in);
-  m.partials = h->multi_partials.p;  // (the launches of a round run one after the other on the stream: slices and tickets are reused)
-  m.tickets = h->d_multi_tickets;
-  m.out = (direct ? h->h_multi_out : h->d_multi_out) + (size_t)row0 * kMultiOut;
-  m.done = direct ? h->h_multi_done + row0 : nullptr;
-  m.done_seq = h->multi_seq;
+  m.partials = h->multi.partials.p;  // (the launches of a round run one after the other on the stream: slices and tickets are reused)
+  m.tickets = h->multi.tickets;
+  m.out = d.out; m.done = d.done; m.done_seq = d.seq;
   const dim3 grid(L.grid, n);
-  prof_begin(h, kind == kEvalError ? VGICP_PROF_ERROR : VGICP_PROF_LINEARIZE, h->stream);
-  bool launched = true;
-  if (L.stream)
-    with_stream_kernel(kind, a.robust, [&](auto what, auto rb) {
-      constexpr int WHAT = decltype(what)::value;
-      constexpr bool RB = decltype(rb)::value;
-      const size_t smem = sizeof(LinStreamSmem);
-      if constexpr (WHAT == 2) k_linearize_stream_multi<2, false, RB><<<grid, kLinThreads, smem, h->stream>>>(a, m);  // (counts no hits)
-      else if (count) k_linearize_stream_multi<WHAT, true, RB><<<grid, kLinThreads, smem, h->stream>>>(a, m);
-      else k_linearize_stream_multi<WHAT, false, RB><<<grid, kLinThreads, smem, h->stream>>>(a, m);
-    });
-  else
-    launched = with_lin_kernel(h->offset_mode, L.G, a.robust, [&](auto mode, auto g, auto rb) {
-      constexpr int MODE = decltype(mode)::value, G = decltype(g)::value;
-      constexpr bool RB = decltype(rb)::value;
-      if (kind == kEvalSpec) k_linearize_spec_multi<MODE, G, RB><<<grid, kLinThreads, 0, h->stream>>>(a, m);
-      else if (kind == kEvalLinearize && count) k_linearize_multi<MODE, true, G, true, RB><<<grid, kLinThreads, 0, h->stream>>>(a, m);
-      else if (kind == kEvalLinearize) k_linearize_multi<MODE, true, G, false, RB><<<grid, kLinThreads, 0, h->stream>>>(a, m);
-      else if (count) k_linearize_multi<MODE, false, G, true, RB><<<grid, kLinThreads, 0, h->stream>>>(a, m);
-      else k_linearize_multi<MODE, false, G, false, RB><<<grid, kLinThreads, 0, h->stream>>>(a, m);
-    });
-  prof_end(h, h->stream);
-  if (!launched) return fail(h, VGICP_ERR_UNSUPPORTED, "no evaluation kernel for this offset table and lane split");
-  h->launches++;
-  CU_TRY(h, cudaGetLastError());
-  return VGICP_OK;
-}
-
-// waits for rows [0, n_rows) of the current round; returns the records (host memory, kMultiOut doubles per row)
-int multi_wait(vgicp_handle h, int n_rows, const double** rec) {
-  *rec = h->h_multi_out;
-  return wait_records(h, h->h_multi_done, n_rows, h->multi_seq, h->h_multi_out, h->d_multi_out, (size_t)n_rows * kMultiOut);
+  return launch_eval(h, kind, a.robust, [&](auto what, auto rb) {
+    constexpr int WHAT = decltype(what)::value;
+    constexpr bool RB = decltype(rb)::value;
+    auto with_count = [&](auto cnt) {
+      constexpr bool COUNT = decltype(cnt)::value && WHAT != kEvalSpec;  // (the speculative evaluation counts no hits)
+      if (L.stream) {
+        k_linearize_stream_multi<WHAT, COUNT, RB><<<grid, kLinThreads, sizeof(LinStreamSmem), h->stream>>>(a, m);
+        return true;
+      }
+      return with_lin_shape(h->offset_mode, L.G, [&](auto mode, auto g) {
+        k_linearize_multi<decltype(mode)::value, WHAT, decltype(g)::value, COUNT, RB><<<grid, kLinThreads, 0, h->stream>>>(a, m);
+      });
+    };
+    return count ? with_count(std::true_type{}) : with_count(std::false_type{});
+  });
 }
 
 // ---- LsqRegistration::computeTransformation (lsq_registration_impl.hpp:53-79) with step_gn (:106-120) / step_lm (:123-168) --------
@@ -1178,35 +1178,10 @@ void lm_result(const LmState<6>& st, vgicp_align_result* res) {
 }
 
 // ---- continuous-time registration (vgicp_compute_error_ct, vgicp_align_ct) ------------------------------------------------------
-// VGICP on one GPU, with the source's timestamps and the preconditions of vgicp_align
-int ct_check(vgicp_handle h, const char* who) {
-  if (h->problem != 0) return fail(h, VGICP_ERR_UNSUPPORTED, std::string(who) + ": continuous-time registration is defined for the VGICP problem only");
-  if (h->comm_ranks > 1 || h->stage1_sharding || h->shard_end >= 0)
-    return fail(h, VGICP_ERR_UNSUPPORTED, std::string(who) + ": not available with source or stage-1 sharding or in a multi-GPU communicator");
-  if (!h->source.has_pts || !h->source.has_cov) return fail(h, VGICP_ERR_BAD_STATE, std::string(who) + ": source points and covariances required");
-  if (!h->map.built && !h->map.pending) return fail(h, VGICP_ERR_BAD_STATE, std::string(who) + ": target voxel map not built");
-  if (!h->ct_has_times) return fail(h, VGICP_ERR_BAD_STATE, std::string(who) + ": the source has no timestamps (vgicp_set_source_timestamps)");
-  return VGICP_OK;
-}
-
 bool all_finite(const double* v, int n, bool as_float) {
   for (int j = 0; j < n; j++)
     if (!(as_float ? std::isfinite((float)v[j]) : std::isfinite(v[j]))) return false;
   return true;
-}
-
-// fixed-size buffers on first use
-int ct_reserve(vgicp_handle h) {
-  if (!h->h_ct_out) {
-    CU_TRY(h, cudaMalloc(&h->d_ct_ticket, sizeof(unsigned int)));
-    CU_TRY(h, cudaMemsetAsync(h->d_ct_ticket, 0, sizeof(unsigned int), h->stream));
-    CU_TRY(h, cudaMalloc(&h->d_ct_out, kCtStride * sizeof(double)));
-    CU_TRY(h, cudaHostAlloc(&h->h_ct_done, sizeof(unsigned long long), cudaHostAllocMapped));
-    *h->h_ct_done = 0;
-    CU_TRY(h, cudaHostAlloc(&h->h_ct_out, kCtStride * sizeof(double), cudaHostAllocMapped));  // (last: it marks the set as complete)
-  }
-  CU_TRY(h, h->ct_partials.reserve((size_t)kLinMaxBlocks * kCtStride));
-  return VGICP_OK;
 }
 
 // One evaluation at (Te, xe) over the correspondences of (Tl, xl): the compacted kernel and grid make_lin_launch picks (DIRECT1 on
@@ -1223,26 +1198,18 @@ int ct_evaluate(vgicp_handle h, const double* Tl, const double* xl, const double
     c.xl[j] = (float)xl[j];
     c.xe[j] = (float)xe[j];
   }
-  c.partials = h->ct_partials.p;
-  c.ticket = h->d_ct_ticket;
-  const bool direct = h->exec_hint == 0;
-  c.out = direct ? h->h_ct_out : h->d_ct_out;
-  c.done_flag = direct ? h->h_ct_done : nullptr;
-  c.done_seq = ++h->ct_seq;
-  prof_begin(h, want_H ? VGICP_PROF_LINEARIZE : VGICP_PROF_ERROR, h->stream);
-  const bool launched = with_lin_kernel(h->offset_mode, L.G, a.robust, [&](auto mode, auto g, auto rb) {
-    constexpr int MODE = decltype(mode)::value, G = decltype(g)::value;
-    constexpr bool RB = decltype(rb)::value;
-    if (want_H) k_linearize_ct<MODE, true, G, RB><<<L.grid, kLinThreads, 0, h->stream>>>(a, c);
-    else k_linearize_ct<MODE, false, G, RB><<<L.grid, kLinThreads, 0, h->stream>>>(a, c);
+  c.partials = h->ct.partials.p;
+  c.ticket = h->ct.tickets;
+  h->ct.seq++;
+  const EvalChannel::Dest d = h->ct.dest(h->exec_hint == 0);
+  c.out = d.out; c.done_flag = d.done; c.done_seq = d.seq;
+  int rc = launch_eval(h, want_H ? kEvalLinearize : kEvalError, a.robust, [&](auto what, auto rb) {
+    return with_lin_shape(h->offset_mode, L.G, [&](auto mode, auto g) {
+      k_linearize_ct<decltype(mode)::value, decltype(what)::value == kEvalLinearize, decltype(g)::value, decltype(rb)::value><<<L.grid, kLinThreads, 0, h->stream>>>(a, c);
+    });
   });
-  prof_end(h, h->stream);
-  if (!launched) return fail(h, VGICP_ERR_UNSUPPORTED, "no evaluation kernel for this offset table and lane split");
-  h->launches++;
-  CU_TRY(h, cudaGetLastError());
-  int rc = wait_records(h, h->h_ct_done, 1, h->ct_seq, h->h_ct_out, h->d_ct_out, want_H ? kCtValues : 1);
-  if (rc) return rc;
-  *raw = h->h_ct_out;
+  if (rc || (rc = h->ct.wait(h, 1, want_H ? kCtValues : 1))) return rc;
+  *raw = h->ct.h_out;
   return VGICP_OK;
 }
 
@@ -1329,7 +1296,7 @@ int vgicp_create(int device, vgicp_handle* out) {
   DeviceGuard g(device);
   // the kernel image is sm_90a only: fail loudly on anything else instead of falling back
   cudaFuncAttributes fa;
-  if (cudaFuncGetAttributes(&fa, k_linearize<1, true, 1, false>) != cudaSuccess) {
+  if (cudaFuncGetAttributes(&fa, k_linearize<1, kEvalLinearize, 1, false>) != cudaSuccess) {
     cudaGetLastError();
     delete h;
     return VGICP_ERR_NO_DEVICE;
@@ -1342,7 +1309,6 @@ int vgicp_create(int device, vgicp_handle* out) {
   ok = ok && cudaEventCreateWithFlags(&h->source.ready, cudaEventDisableTiming) == cudaSuccess;
   h->target.st = h->stream;    // the target (and its voxel map) is built on the main stream, where the evaluations run
   h->source.st = h->stream_b;  // the source's stage 1 overlaps with it
-  ok = ok && cudaMalloc(&h->d_ticket, sizeof(unsigned int)) == cudaSuccess;
   for (VoxelMap* vm : {&h->map, &h->ndt_t, &h->ndt_s}) {
     ok = ok && cudaMalloc(&vm->d_counters, 16 * sizeof(int)) == cudaSuccess;
     ok = ok && cudaMallocHost(&vm->h_counters, 16 * sizeof(int)) == cudaSuccess;
@@ -1350,19 +1316,14 @@ int vgicp_create(int device, vgicp_handle* out) {
     ok = ok && cudaEventCreateWithFlags(&vm->ev_done, cudaEventDisableTiming) == cudaSuccess;
   }
   h->ndt_t.ndt = h->ndt_s.ndt = 1;
-  ok = ok && cudaMalloc(&h->d_out, 64 * sizeof(double)) == cudaSuccess;
-  ok = ok && cudaHostAlloc(&h->h_out, 64 * sizeof(double), cudaHostAllocMapped) == cudaSuccess;
-  ok = ok && cudaHostAlloc(&h->h_flag, 64, cudaHostAllocMapped) == cudaSuccess;
-  if (ok) *h->h_flag = 0;
-  ok = ok && h->partials.reserve((size_t)kLinStreamMaxBlocks * kLinStride) == cudaSuccess;
-  ok = ok && cudaMemsetAsync(h->d_ticket, 0, sizeof(unsigned int), h->stream) == cudaSuccess;
+  ok = ok && h->eval.open(1, 64, (size_t)kLinStreamMaxBlocks * kLinStride, h->stream) == cudaSuccess;
   ok = ok && cudaStreamSynchronize(h->stream) == cudaSuccess;
+  // fast_vgicp_cuda.cu:28-29, with the table on the device as well: the correspondence getter reads it under every method
+  ok = ok && vgicp_set_neighbor_search_method(h, VGICP_DIRECT1, -1.0) == VGICP_OK;
   if (!ok) {
     vgicp_destroy(h);
     return VGICP_ERR_CUDA;
   }
-  h->h_offsets.assign(1, make_int4(0, 0, 0, 0));  // fast_vgicp_cuda.cu:28-29
-  h->offset_mode = 1;
   *out = h;
   return VGICP_OK;
 }
@@ -1379,9 +1340,7 @@ int vgicp_destroy(vgicp_handle h) {
   if (h->comm_ranks > 1) vgicp_comm_shutdown(h);
   if (h->comm_box) cudaFree(h->comm_box);
   if (h->arena) cudaFree(h->arena);
-  h->partials.release();
   h->corr_ids.release();
-  if (h->d_ticket) cudaFree(h->d_ticket);
   for (VoxelMap* vm : {&h->map, &h->ndt_t, &h->ndt_s}) {
     if (vm->d_counters) cudaFree(vm->d_counters);
     if (vm->h_counters) cudaFreeHost(vm->h_counters);
@@ -1392,24 +1351,14 @@ int vgicp_destroy(vgicp_handle h) {
   h->ndt_src_pts.release(); h->ndt_src_covA.release(); h->ndt_src_covB.release();
   h->crop_rank.release(); h->crop_state.release();
   h->spare_pts.release(); h->spare_covA.release(); h->spare_covB.release();
-  if (h->d_out) cudaFree(h->d_out);
-  if (h->h_out) cudaFreeHost(h->h_out);
-  if (h->h_flag) cudaFreeHost(h->h_flag);
-  h->multi_partials.release();
-  if (h->d_multi_tickets) cudaFree(h->d_multi_tickets);
+  h->eval.release();
+  h->multi.release();
   if (h->d_multi_in) cudaFree(h->d_multi_in);
   if (h->h_multi_in) cudaFreeHost(h->h_multi_in);
-  if (h->d_multi_out) cudaFree(h->d_multi_out);
-  if (h->h_multi_out) cudaFreeHost(h->h_multi_out);
-  if (h->h_multi_done) cudaFreeHost(h->h_multi_done);
   h->ct_times.release();
   h->ct_spare.release();
   h->ct_stats.release();
-  h->ct_partials.release();
-  if (h->d_ct_ticket) cudaFree(h->d_ct_ticket);
-  if (h->d_ct_out) cudaFree(h->d_ct_out);
-  if (h->h_ct_out) cudaFreeHost(h->h_ct_out);
-  if (h->h_ct_done) cudaFreeHost(h->h_ct_done);
+  h->ct.release();
   for (auto& r : h->prof_pending) { cudaEventDestroy(r.a); cudaEventDestroy(r.b); }
   for (auto e : h->prof_pool) cudaEventDestroy(e);
   for (cudaEvent_t e : {h->ev_copy, h->ev_append, h->ev_deskew, h->target.ready, h->source.ready})
@@ -1715,9 +1664,7 @@ int vgicp_get_voxel_buckets(vgicp_handle h, int* coords3, int* ids, size_t cap) 
 int vgicp_update_correspondences(vgicp_handle h, const double T[16]) {  // fast_vgicp_cuda.cu:265-274
   CHECK_HANDLE(h);
   if (!T) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "update_correspondences: null pose");
-  if (!h->source.has_pts) return fail(h, VGICP_ERR_BAD_STATE, "update_correspondences: source cloud not set");
-  if (h->problem == 0 && !h->map.built && !h->map.pending) return fail(h, VGICP_ERR_BAD_STATE, "update_correspondences: target voxel map not built");
-  if (h->problem != 0 && !h->target.has_pts) return fail(h, VGICP_ERR_BAD_STATE, "update_correspondences: target cloud not set");
+  if (int rc = check_ready(h, "update_correspondences", 0)) return rc;
   h->lin = to_pose(T);  // linearized_x = trans.cast<float>()
   h->has_lin = true;
   // the lookup itself is fused into the evaluation kernel; the explicit list is only built by the getter
@@ -1727,9 +1674,7 @@ int vgicp_update_correspondences(vgicp_handle h, const double T[16]) {  // fast_
 int vgicp_get_voxel_correspondences(vgicp_handle h, int* pairs, size_t cap, size_t* n_pairs) {
   CHECK_HANDLE(h);
   DeviceGuard g(h->device);
-  if (!h->source.has_pts || (h->problem == 0 && !h->map.built && !h->map.pending) || !h->has_lin)
-    return fail(h, VGICP_ERR_BAD_STATE, "get_voxel_correspondences: update_correspondences has not been called");
-  { int rc = sync_inputs(h); if (rc) return rc; }
+  { int rc = check_ready(h, "get_voxel_correspondences", kNeedLin); if (!rc) rc = sync_inputs(h); if (rc) return rc; }
   const LinLaunch LL = make_lin_launch(h);  // same source array / map as an evaluation (VGICP points, NDT points or voxel means)
   const int n = LL.a.n;
   const int n_off = (int)h->h_offsets.size();
@@ -1760,11 +1705,8 @@ int vgicp_compute_error(vgicp_handle h, const double T[16], double* H36, double*
   CHECK_HANDLE(h);
   DeviceGuard g(h->device);
   if (!T) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "compute_error: null pose");
-  int rc = check_robust_problem(h, "compute_error");
-  if (rc) return rc;
-  rc = check_ready_for_eval(h, "compute_error");
-  if (rc) return rc;
-  if ((rc = sync_inputs(h))) return rc;
+  int rc = check_ready(h, "compute_error", kNeedEval | kNeedLin);
+  if (rc || (rc = sync_inputs(h))) return rc;
   const bool want_H = (H36 != nullptr && b6 != nullptr);  // compute_derivatives.cu:160
   const double* rec = nullptr;
   if ((rc = evaluate(h, to_pose(T), want_H ? kEvalLinearize : kEvalError, &rec))) return rc;
@@ -1793,16 +1735,9 @@ int vgicp_align(vgicp_handle h, const double guess[16], const vgicp_lsq_params* 
   CHECK_HANDLE(h);
   DeviceGuard g(h->device);
   if (!guess || !res) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "align: null argument");
-  { int rc = check_robust_problem(h, "align"); if (rc) return rc; }
+  { int rc = check_ready(h, "align", kNeedEval); if (!rc) rc = sync_inputs(h); if (rc) return rc; }
   vgicp_lsq_params P;
   if (params) P = *params; else vgicp_lsq_default_params(&P);
-  if (h->problem == 0) {
-    if (!h->source.has_pts || !h->source.has_cov) return fail(h, VGICP_ERR_BAD_STATE, "align: source points and covariances required");
-    if (!h->map.built && !h->map.pending) return fail(h, VGICP_ERR_BAD_STATE, "align: target voxel map not built");
-  } else if (!h->source.has_pts || !h->target.has_pts) {
-    return fail(h, VGICP_ERR_BAD_STATE, "align: NDT needs source and target clouds");
-  }
-  { int rc = sync_inputs(h); if (rc) return rc; }
   const bool speculate = h->speculate != 0 && !P.use_gauss_newton;
   LmState<6> st = lm_init<6>(guess, P);
   while (st.phase != kLmDone) {
@@ -1823,16 +1758,13 @@ int vgicp_align(vgicp_handle h, const double guess[16], const vgicp_lsq_params* 
 
 // B registrations from B initial guesses.  Each hypothesis runs vgicp_align's state machine; every round stages the poses of the
 // running hypotheses and evaluates all of them in one launch per evaluation kind.  With LM and speculation every round after the
-// first is one k_linearize_spec_multi launch, whose accepted trials feed their linearisation straight back, as in vgicp_align.
+// first is one k_linearize_multi<kEvalSpec> launch, whose accepted trials feed their linearisation straight back, as in vgicp_align.
 int vgicp_align_multi(vgicp_handle h, const double* guesses, int n_guesses, const vgicp_lsq_params* params, vgicp_align_result* results) {
   CHECK_HANDLE(h);
   DeviceGuard g(h->device);
   if (!guesses || !results || n_guesses < 1 || n_guesses > kMultiMaxHyp) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "align_multi: null argument or n_guesses outside [1, 4096]");
-  int rc = check_robust_problem(h, "align_multi");
-  if (rc) return rc;
-  rc = check_ready_for_multi(h, "align_multi");
-  if (rc) return rc;
-  if ((rc = sync_inputs(h))) return rc;
+  int rc = check_ready(h, "align_multi", kNeedEval | kNeedOneGpu);
+  if (rc || (rc = sync_inputs(h))) return rc;
   vgicp_lsq_params P;
   if (params) P = *params; else vgicp_lsq_default_params(&P);
   const int B = n_guesses;
@@ -1858,12 +1790,12 @@ int vgicp_align_multi(vgicp_handle h, const double* guesses, int n_guesses, cons
         poses[2 * i + 1] = to_pose(st[i].xi.m);
       }
     if (n == 0) break;
-    h->multi_seq++;
+    h->multi.seq++;
     if ((rc = multi_upload(h, B, n))) return rc;
     if (n_lin && (rc = launch_multi(h, L, B, kEvalLinearize, false, 0, n_lin))) return rc;
     if (n > n_lin && (rc = launch_multi(h, L, B, speculate ? kEvalSpec : kEvalError, false, n_lin, n - n_lin))) return rc;
-    const double* rec = nullptr;
-    if ((rc = multi_wait(h, n, &rec))) return rc;
+    if ((rc = h->multi.wait(h, n, (size_t)n * kMultiOut))) return rc;
+    const double* rec = h->multi.h_out;
     for (int r = 0; r < n; r++) lm_consume(&st[rows[r]], rec + (size_t)r * kMultiOut, r >= n_lin && speculate);
   }
   for (int i = 0; i < B; i++) lm_result(st[i], &results[i]);
@@ -1876,11 +1808,8 @@ int vgicp_evaluate_poses(vgicp_handle h, const double* T, int n_poses, double* e
   DeviceGuard g(h->device);
   if (!T || !err || n_poses < 1 || n_poses > kMultiMaxHyp || (H36 == nullptr) != (b6 == nullptr))
     return fail(h, VGICP_ERR_INVALID_ARGUMENT, "evaluate_poses: null argument, H36 without b6 (or b6 without H36), or n_poses outside [1, 4096]");
-  int rc = check_robust_problem(h, "evaluate_poses");
-  if (rc) return rc;
-  rc = check_ready_for_multi(h, "evaluate_poses");
-  if (rc) return rc;
-  if ((rc = sync_inputs(h))) return rc;
+  int rc = check_ready(h, "evaluate_poses", kNeedEval | kNeedOneGpu);
+  if (rc || (rc = sync_inputs(h))) return rc;
   const int B = n_poses;
   const bool want_H = H36 != nullptr;
   const LinLaunch L = make_lin_launch(h);
@@ -1891,11 +1820,11 @@ int vgicp_evaluate_poses(vgicp_handle h, const double* T, int n_poses, double* e
     poses[2 * i] = poses[2 * i + 1] = to_pose(T + 16 * i);  // linearized_x = trans.cast<float>(), evaluated at the same pose
     rows[i] = i;
   }
-  h->multi_seq++;
+  h->multi.seq++;
   if ((rc = multi_upload(h, B, B))) return rc;
   if ((rc = launch_multi(h, L, B, want_H ? kEvalLinearize : kEvalError, true, 0, B))) return rc;
-  const double* rec = nullptr;
-  if ((rc = multi_wait(h, B, &rec))) return rc;
+  if ((rc = h->multi.wait(h, B, (size_t)B * kMultiOut))) return rc;
+  const double* rec = h->multi.h_out;
   for (int i = 0; i < B; i++) {
     const double* o = rec + (size_t)i * kMultiOut;
     err[i] = o[0];
@@ -2376,12 +2305,12 @@ int vgicp_compute_error_ct(vgicp_handle h, const double T_lin[16], const double 
     return fail(h, VGICP_ERR_INVALID_ARGUMENT, "compute_error_ct: null pose or twist, or H144 without b12 (or b12 without H144)");
   if (!all_finite(T_lin, 16, false) || !all_finite(T_eval, 16, false) || !all_finite(xi_lin, 6, true) || !all_finite(xi_eval, 6, true))
     return fail(h, VGICP_ERR_INVALID_ARGUMENT, "compute_error_ct: non-finite pose or twist");
-  int rc = ct_check(h, "compute_error_ct");
+  int rc = check_ready(h, "compute_error_ct", kNeedEval | kNeedCt);
   if (rc) return rc;
   if (!twist_in_series(xi_lin, h->ct_span) || !twist_in_series(xi_eval, h->ct_span))
     return fail(h, VGICP_ERR_INVALID_ARGUMENT, "compute_error_ct: the rotation over the sweep (|omega| * max |s_i|) exceeds pi/2, beyond the series");
   if ((rc = sync_inputs(h))) return rc;
-  if ((rc = ct_reserve(h))) return rc;
+  CU_TRY(h, h->ct.open(1, kCtStride, (size_t)kLinMaxBlocks * kCtStride, h->stream));
   const bool want_H = H144 != nullptr;
   const double* raw = nullptr;
   if ((rc = ct_evaluate(h, T_lin, xi_lin, T_eval, xi_eval, want_H, &raw))) return rc;
@@ -2401,14 +2330,14 @@ int vgicp_align_ct(vgicp_handle h, const double guess[16], const double twist_gu
     return fail(h, VGICP_ERR_INVALID_ARGUMENT, "align_ct: non-finite guess, twist guess or prior");
   for (int j = 0; j < 6; j++)
     if (!(twist_weight[j] > 0.0 && std::isfinite(twist_weight[j]))) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "align_ct: every twist weight must be finite and > 0");
-  int rc = ct_check(h, "align_ct");
+  int rc = check_ready(h, "align_ct", kNeedEval | kNeedCt);
   if (rc) return rc;
   if (!twist_in_series(twist_guess, h->ct_span) || !twist_in_series(twist_prior, h->ct_span))
     return fail(h, VGICP_ERR_INVALID_ARGUMENT, "align_ct: the twist guess or prior rotates more than pi/2 over the sweep (|omega| * max |s_i|), beyond the series");
   vgicp_lsq_params P;
   if (params) P = *params; else vgicp_lsq_default_params(&P);
   if ((rc = sync_inputs(h))) return rc;
-  if ((rc = ct_reserve(h))) return rc;
+  CU_TRY(h, h->ct.open(1, kCtStride, (size_t)kLinMaxBlocks * kCtStride, h->stream));
   LmState<12> st = lm_init<12>(guess, P);
   memcpy(st.tw0, twist_guess, sizeof(st.tw0));
   st.span = h->ct_span;

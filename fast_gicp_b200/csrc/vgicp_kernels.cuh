@@ -455,6 +455,11 @@ struct LinArgs {
   float robust_d2;
 };
 
+// What an evaluation launch computes (every row of a multi-pose one alike): the WHAT parameter of the evaluation kernels.
+//   kEvalError: err;  kEvalLinearize: err, H, b;  kEvalSpec: both, see lin_spec_accumulate
+enum { kEvalError = 0, kEvalLinearize = 1, kEvalSpec = 2 };
+__host__ __device__ constexpr int eval_values(int what) { return what == kEvalError ? 1 : (what == kEvalLinearize ? kLinValues : kLinValues + 1); }
+
 // Continuous-time evaluation (vgicp_compute_error_ct / vgicp_align_ct): source point i is first moved to q_i = Exp(s_i xi) a_i,
 // s_i = times[i] - tau (deskew_point), with xi_lin for the voxel lookup under Tlin and xi_eval for the residual at Teval.  A kernel
 // argument of its own, so that the parameter block of every other evaluation kernel is unchanged.
@@ -985,23 +990,20 @@ __device__ __forceinline__ void lin_unpack(const double* s, double* out) {
   }
 }
 
-// One evaluation (update_correspondences + compute_error fused).  MODE: 0 = offsets from memory (DIRECT_RADIUS or anything),
-// 1 / 7 / 27 = the reference's fixed tables; G = lanes per source point in the lookup phase (see lin_accumulate_impl): at 17k points
-// a one-thread-per-point mapping would leave one warp per scheduler with 27 serial dependent lookups per thread.
-template <int MODE, bool WANT_H, int G, bool RB>
-__global__ void __launch_bounds__(kLinThreads) k_linearize(const LinArgs a) {
-  constexpr int NV = WANT_H ? kLinValues : 1;
-  __shared__ double fin[4][kLinStride];
-  float sum[NV];
-  lin_accumulate<MODE, WANT_H, G, false, RB>(a, a.Tlin, a.Teval, sum);
-  if (!lin_reduce<NV>(a, sum, fin)) return;
-  if (threadIdx.x == 0) {
-    lin_unpack<WANT_H>(fin[0], a.out);
-    *a.ticket = 0u;
-    if (a.done_flag) {  // the host spins on this word instead of waiting for the stream (saves the copy + wake-up latency)
-      __threadfence_system();
-      *a.done_flag = a.done_seq;
-    }
+// the record of an evaluation kind from its folded sums: [0] err, [1..36] H, [37..42] b;  [43] kEvalSpec: err over the old correspondences
+template <int WHAT>
+__device__ __forceinline__ void lin_write_record(const double* s, double* out) {
+  lin_unpack<WHAT != kEvalError>(s, out);
+  if (WHAT == kEvalSpec) out[43] = s[kLinValues];
+}
+
+// thread 0 of the (row's) last block, after the record is written: ready the ticket for the next launch, then publish the record
+// (`done`: the host spins on this word instead of waiting for the stream, which saves the copy and the wake-up latency)
+__device__ __forceinline__ void lin_publish(unsigned int* tickets, volatile unsigned long long* done, unsigned long long seq, int row = 0) {
+  tickets[row] = 0u;
+  if (done) {
+    __threadfence_system();
+    done[row] = seq;
   }
 }
 
@@ -1025,21 +1027,26 @@ __device__ __forceinline__ void lin_spec_accumulate(const LinArgs& a, const Pose
     for (int i = 0; i < kLinValues; i++) sum[i] = lin[i];
   }
 }
-template <int MODE, int G, bool RB>
-__global__ void __launch_bounds__(kLinThreads) k_linearize_spec(const LinArgs a) {
-  constexpr int NV = kLinValues + 1;
+// the sums of an evaluation kind (COUNT: kEvalError / kEvalLinearize only)
+template <int MODE, int WHAT, int G, bool COUNT, bool RB>
+__device__ __forceinline__ void lin_eval_accumulate(const LinArgs& a, const Pose& Tl, const Pose& Te, float* sum) {
+  if constexpr (WHAT == kEvalSpec) lin_spec_accumulate<MODE, G, RB>(a, Tl, Te, sum);
+  else lin_accumulate<MODE, WHAT == kEvalLinearize, G, COUNT, RB>(a, Tl, Te, sum);
+}
+
+// One evaluation (update_correspondences + compute_error fused).  MODE: 0 = offsets from memory (DIRECT_RADIUS or anything),
+// 1 / 7 / 27 = the reference's fixed tables; G = lanes per source point in the lookup phase (see lin_accumulate_impl): at 17k points
+// a one-thread-per-point mapping would leave one warp per scheduler with 27 serial dependent lookups per thread.
+template <int MODE, int WHAT, int G, bool RB>
+__global__ void __launch_bounds__(kLinThreads) k_linearize(const LinArgs a) {
+  constexpr int NV = eval_values(WHAT);
   __shared__ double fin[4][kLinStride];
   float sum[NV];
-  lin_spec_accumulate<MODE, G, RB>(a, a.Tlin, a.Teval, sum);
+  lin_eval_accumulate<MODE, WHAT, G, false, RB>(a, a.Tlin, a.Teval, sum);
   if (!lin_reduce<NV>(a, sum, fin)) return;
   if (threadIdx.x == 0) {
-    lin_unpack<true>(fin[0], a.out);
-    a.out[43] = fin[0][kLinValues];
-    *a.ticket = 0u;
-    if (a.done_flag) {
-      __threadfence_system();
-      *a.done_flag = a.done_seq;
-    }
+    lin_write_record<WHAT>(fin[0], a.out);
+    lin_publish(a.ticket, a.done_flag, a.done_seq);
   }
 }
 
@@ -1054,11 +1061,7 @@ __global__ void __launch_bounds__(kLinThreads) k_linearize_ct(const LinArgs a, c
   if (!lin_reduce<NV, kCtStride>(a, sum, fin, c.partials, c.ticket)) return;
   if (threadIdx.x == 0) {
     for (int j = 0; j < NV; j++) c.out[j] = fin[0][j];
-    *c.ticket = 0u;
-    if (c.done_flag) {
-      __threadfence_system();
-      *c.done_flag = c.done_seq;
-    }
+    lin_publish(c.ticket, c.done_flag, c.done_seq);
   }
 }
 
@@ -1068,8 +1071,8 @@ __global__ void __launch_bounds__(kLinThreads) k_linearize_ct(const LinArgs a, c
 // an elected thread issues cp.async.bulk (global -> shared, completion counted on an mbarrier) for the point, covA and covB slices
 // of the tile kLinStreamStages - 1 tiles ahead, so that the HBM reads of later tiles are in flight while the warps chase the
 // dependent loads of the current one (cell index -> voxel record).  No hit compaction: a lane keeps its own point.
-// SPEC: error over the correspondences of Tlin at Teval (sum[28]) and the full linearisation at Teval (sums 0..27) from one pass
-// over the staged points, like k_linearize_spec.
+// kEvalSpec: error over the correspondences of Tlin at Teval (sum[28]) and the full linearisation at Teval (sums 0..27) from one pass
+// over the staged points, like lin_spec_accumulate.
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int kLinStreamTile = 128;     // points per tile (1 per thread)
 constexpr int kLinStreamStages = 4;
@@ -1139,11 +1142,11 @@ __device__ __forceinline__ void lin_stream_point(const LinArgs& a, const Pose& T
   apply_jacobian<WANT_H>(pe, acc, sum);
 }
 
-// WHAT: 0 = error only, 1 = linearisation (H, b, err), 2 = speculative (both).  COUNT (WHAT 0 / 1): one more slot counts the hits.
+// COUNT (kEvalError / kEvalLinearize): one more slot counts the hits.
 template <int WHAT, bool COUNT, bool RB>
 __device__ __forceinline__ void lin_stream_accumulate(const LinArgs& a, const Pose& Tl, const Pose& Te, float* sum) {
-  constexpr int NV = (WHAT == 0 ? 1 : (WHAT == 1 ? kLinValues : kLinValues + 1)) + (COUNT ? 1 : 0);
-  static_assert(!COUNT || WHAT != 2, "the speculative evaluation does not count hits");
+  constexpr int NV = eval_values(WHAT) + (COUNT ? 1 : 0);
+  static_assert(!COUNT || WHAT != kEvalSpec, "the speculative evaluation does not count hits");
   extern __shared__ __align__(128) unsigned char stream_smem_raw[];
   LinStreamSmem& sm = *reinterpret_cast<LinStreamSmem*>(stream_smem_raw);
   const int tid = threadIdx.x;
@@ -1183,9 +1186,9 @@ __device__ __forceinline__ void lin_stream_accumulate(const LinArgs& a, const Po
       if (first + j < a.n) {
         const float4 p = sm.pts[s][j], ca = sm.covA[s][j];
         const float2 cb = sm.covB[s][j];
-        if (WHAT == 0) {
+        if (WHAT == kEvalError) {
           lin_stream_point<false, COUNT, RB>(a, Tl, Te, p, ca, cb, sum);
-        } else if (WHAT == 1) {
+        } else if (WHAT == kEvalLinearize) {
           lin_stream_point<true, COUNT, RB>(a, Tl, Te, p, ca, cb, sum);
         } else {
           lin_stream_point<false, false, RB>(a, Tl, Te, p, ca, cb, sum + kLinValues);
@@ -1198,24 +1201,14 @@ __device__ __forceinline__ void lin_stream_accumulate(const LinArgs& a, const Po
 }
 template <int WHAT, bool RB>
 __global__ void __launch_bounds__(kLinThreads) k_linearize_stream(const LinArgs a) {
-  constexpr int NV = WHAT == 0 ? 1 : (WHAT == 1 ? kLinValues : kLinValues + 1);
+  constexpr int NV = eval_values(WHAT);
   __shared__ double fin[4][kLinStride];
-  const int tid = threadIdx.x;
   float sum[NV];
   lin_stream_accumulate<WHAT, false, RB>(a, a.Tlin, a.Teval, sum);
   if (!lin_reduce<NV>(a, sum, fin)) return;
-  if (tid == 0) {
-    if (WHAT == 0) {
-      lin_unpack<false>(fin[0], a.out);
-    } else {
-      lin_unpack<true>(fin[0], a.out);
-      if (WHAT == 2) a.out[43] = fin[0][kLinValues];
-    }
-    *a.ticket = 0u;
-    if (a.done_flag) {
-      __threadfence_system();
-      *a.done_flag = a.done_seq;
-    }
+  if (threadIdx.x == 0) {
+    lin_write_record<WHAT>(fin[0], a.out);
+    lin_publish(a.ticket, a.done_flag, a.done_seq);
   }
 }
 
@@ -1254,70 +1247,38 @@ template <int NV>
 __device__ __forceinline__ bool multi_reduce(const LinArgs& a, const MultiArgs& m, int y, const float* sum, double (*fin)[kLinStride]) {
   return lin_reduce<NV>(a, sum, fin, m.partials + (size_t)y * gridDim.x * kLinStride, m.tickets + y);
 }
-// thread 0 of a row's last block, after its record is written
-__device__ __forceinline__ void multi_publish(const MultiArgs& m, int y) {
-  m.tickets[y] = 0u;
-  if (m.done) {
-    __threadfence_system();
-    m.done[y] = m.done_seq;
-  }
+// thread 0 of a row's last block: the row's record, its hit count (COUNT), then the row's ticket and completion word
+template <int WHAT, bool COUNT>
+__device__ __forceinline__ void multi_finish(const MultiArgs& m, int y, const double* fin) {
+  double* rec = m.out + (size_t)y * kMultiOut;
+  lin_write_record<WHAT>(fin, rec);
+  if (COUNT) rec[kMultiOutCount] = fin[eval_values(WHAT)];
+  lin_publish(m.tickets, m.done, m.done_seq, y);
 }
 
-template <int MODE, bool WANT_H, int G, bool COUNT, bool RB>
+template <int MODE, int WHAT, int G, bool COUNT, bool RB>
 __global__ void __launch_bounds__(kLinThreads, 1) k_linearize_multi(const LinArgs a, const MultiArgs m) {
-  constexpr int NV = (WANT_H ? kLinValues : 1) + (COUNT ? 1 : 0);
+  static_assert(!(WHAT == kEvalSpec && COUNT), "the speculative evaluation does not count hits");
+  constexpr int NV = eval_values(WHAT) + (COUNT ? 1 : 0);
   __shared__ double fin[4][kLinStride];
   __shared__ Pose sp[2];
   const int y = multi_row(m, sp);
   float sum[NV];
-  lin_accumulate<MODE, WANT_H, G, COUNT, RB>(a, sp[0], sp[1], sum);
+  lin_eval_accumulate<MODE, WHAT, G, COUNT, RB>(a, sp[0], sp[1], sum);
   if (!multi_reduce<NV>(a, m, y, sum, fin)) return;
-  if (threadIdx.x == 0) {
-    double* rec = m.out + (size_t)y * kMultiOut;
-    lin_unpack<WANT_H>(fin[0], rec);
-    if (COUNT) rec[kMultiOutCount] = fin[0][NV - 1];
-    multi_publish(m, y);
-  }
-}
-
-template <int MODE, int G, bool RB>
-__global__ void __launch_bounds__(kLinThreads, 1) k_linearize_spec_multi(const LinArgs a, const MultiArgs m) {
-  constexpr int NV = kLinValues + 1;
-  __shared__ double fin[4][kLinStride];
-  __shared__ Pose sp[2];
-  const int y = multi_row(m, sp);
-  float sum[NV];
-  lin_spec_accumulate<MODE, G, RB>(a, sp[0], sp[1], sum);
-  if (!multi_reduce<NV>(a, m, y, sum, fin)) return;
-  if (threadIdx.x == 0) {
-    double* rec = m.out + (size_t)y * kMultiOut;
-    lin_unpack<true>(fin[0], rec);
-    rec[43] = fin[0][kLinValues];
-    multi_publish(m, y);
-  }
+  if (threadIdx.x == 0) multi_finish<WHAT, COUNT>(m, y, fin[0]);
 }
 
 template <int WHAT, bool COUNT, bool RB>
 __global__ void __launch_bounds__(kLinThreads, 1) k_linearize_stream_multi(const LinArgs a, const MultiArgs m) {
-  constexpr int NB = WHAT == 0 ? 1 : (WHAT == 1 ? kLinValues : kLinValues + 1);
-  constexpr int NV = NB + (COUNT ? 1 : 0);
+  constexpr int NV = eval_values(WHAT) + (COUNT ? 1 : 0);
   __shared__ double fin[4][kLinStride];
   __shared__ Pose sp[2];
   const int y = multi_row(m, sp);
   float sum[NV];
   lin_stream_accumulate<WHAT, COUNT, RB>(a, sp[0], sp[1], sum);
   if (!multi_reduce<NV>(a, m, y, sum, fin)) return;
-  if (threadIdx.x == 0) {
-    double* rec = m.out + (size_t)y * kMultiOut;
-    if (WHAT == 0) {
-      lin_unpack<false>(fin[0], rec);
-    } else {
-      lin_unpack<true>(fin[0], rec);
-      if (WHAT == 2) rec[43] = fin[0][kLinValues];
-    }
-    if (COUNT) rec[kMultiOutCount] = fin[0][NB];
-    multi_publish(m, y);
-  }
+  if (threadIdx.x == 0) multi_finish<WHAT, COUNT>(m, y, fin[0]);
 }
 
 // Materialise the reference's correspondence list for the getter (fast_vgicp_cuda.cu:221-225): dense [n_off][n] voxel ids,

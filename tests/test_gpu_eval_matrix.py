@@ -3,7 +3,7 @@
 make_lin_launch (csrc/vgicp_b200.cu) picks the kernel from the source size n, the offset table and the voxel index alone, so the
 cases below reach each variant through input sizes: one generated target and exact-size prefixes of one generated source.
 selected_kernel() restates that rule as data and test_case_table_reaches_every_kernel checks that the cases reach every shape of
-with_lin_kernel and the streaming kernel, with robust weights on and off, under both voxel indexes.
+with_lin_shape and the streaming kernel, with robust weights on and off, under both voxel indexes.
 
 Per case, with T_lin != T_eval (update_correspondences(T), then compute_error(T @ small perturbation)) at the identity and near
 the ground truth, for every robust kind:
@@ -43,7 +43,7 @@ pytestmark = pytest.mark.gpu
 TAU = 1e-5
 TAU_PLANE = 1e-4
 
-# with_lin_kernel's table: (MODE, G), MODE = 1 / 7 / 27 fixed tables, 0 = generic offset list
+# with_lin_shape's table: (MODE, G), MODE = 1 / 7 / 27 fixed tables, 0 = generic offset list
 LIN_SHAPES = {(1, 1), (7, 1), (7, 4), (27, 1), (27, 3), (0, 1), (0, 4), (0, 8)}
 MODE_OF = {O.DIRECT1: 1, O.DIRECT7: 7, O.DIRECT27: 27, O.DIRECT_RADIUS: 0}
 METHODS = {"d1": (O.DIRECT1, -1.0), "d7": (O.DIRECT7, -1.0), "d27": (O.DIRECT27, -1.0), "r0.5": (O.DIRECT_RADIUS, 0.5),
@@ -97,7 +97,7 @@ def claimed_cells(pair_n):
 
 
 def test_case_table_reaches_every_kernel(pair02):
-    """The cases reach every (MODE, G) of with_lin_kernel with RB on and off under both indexes, the streaming kernel (dense index
+    """The cases reach every (MODE, G) of with_lin_shape with RB on and off under both indexes, the streaming kernel (dense index
     only) with RB on and off and with NDT weights, every robust kind at every shape, and wide kernels with >= 3 sets per warp."""
     n_of = case_sizes(len(pair02[1]))
     cells = claimed_cells(len(pair02[1]))
@@ -317,7 +317,7 @@ def test_speculation_and_multi_hypothesis_are_bit_identical(pair02, relative_pos
 
 # ---- the kernels the table claims are the ones that run ---------------------------------------------------------------------
 
-_LIN = re.compile(r"k_linearize<(\d+), (true|false), (\d+), (true|false)>")
+_LIN = re.compile(r"k_linearize<(\d+), (\d+), (\d+), (true|false)>")
 _STREAM = re.compile(r"k_linearize_stream<(\d+), (true|false)>")
 
 
@@ -355,7 +355,7 @@ def test_profiler_sees_every_claimed_kernel(pair02, relative_pose, big):
     names = {e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA}
     if not names:
         pytest.skip("torch.profiler recorded no device kernel events on this machine")
-    seen = {(int(g[0]), int(g[2]), g[3] == "true") for g in (_LIN.search(s).groups() for s in names if _LIN.search(s)) if g[1] == "true"}
+    seen = {(int(g[0]), int(g[2]), g[3] == "true") for g in (_LIN.search(s).groups() for s in names if _LIN.search(s)) if g[1] == "1"}  # WHAT == kEvalLinearize
     seen |= {("stream", g[1] == "true") for g in (_STREAM.search(s).groups() for s in names if _STREAM.search(s)) if g[0] == "1"}
     want = {(k[0], k[1], rb) for size, m in VGICP_CASES if size in handles for k in [selected_kernel(n_of[size], *METHODS[m], d) for d in (True, False)]
             if k != "stream" for rb in (False, True)}
