@@ -47,7 +47,7 @@ EXPORTED_SYMBOLS = [
     "vgicp_align_multi", "vgicp_evaluate_poses", "vgicp_set_robust_kernel",
     "vgicp_append_source_to_target", "vgicp_crop_target", "vgicp_deskew_source",
     "vgicp_set_source_timestamps", "vgicp_compute_error_ct", "vgicp_align_ct",
-    "vgicp_set_source_timestamps_device", "vgicp_deskew_source_stored",
+    "vgicp_set_source_timestamps_device", "vgicp_deskew_source_stored", "vgicp_align_sources",
 ]
 PROF_NUM_CATEGORIES = 7
 
@@ -178,6 +178,8 @@ def load_library():
         "vgicp_align_ct": [hp, dp, dp, dp, dp, C.POINTER(LsqParams), C.POINTER(AlignCtResult)],
         "vgicp_set_source_timestamps_device": [hp, C.c_void_p, C.c_size_t, C.c_size_t, C.c_double],
         "vgicp_deskew_source_stored": [hp, dp],
+        "vgicp_align_sources": [hp, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.c_size_t, C.c_int, C.c_int, C.c_int, dp, C.c_int, C.POINTER(LsqParams),
+                                C.POINTER(AlignResult)],
     }
     for name, argtypes in sig.items():
         fn = getattr(L, name)
@@ -524,6 +526,34 @@ class Core:
         params = params or default_params()
         res = (AlignResult * max(B, 1))()
         self._check(self._lib.vgicp_align_multi(self._h, _dp(g), B, C.byref(params), res))
+        return list(res)[:B]
+
+    def align_sources(self, sources, guesses=None, k=20, reg=REG_PLANE, params=None):
+        """Register each of the B source clouds ((N_i, >=3) arrays) against the current target map, the optimisers' evaluations
+        shared across sources -> list of AlignResult.  Result i equals set_source_cloud(sources[i]) + find_source_neighbors(k) +
+        calculate_source_covariances(reg) + align(guesses[i], params) bit for bit; the handle's own source is left as it was.
+        guesses: (B, 4, 4), None = identity for every source."""
+        clouds = [self._cloud(s) for s in sources]
+        if len({st for _, _, st in clouds}) > 1:  # one stride for all: repack to xyz
+            clouds = [self._cloud(np.ascontiguousarray(np.asarray(a, dtype=np.float32)[:, :3])) for a, _, _ in clouds]
+        ptrs = [a.ctypes.data for a, _, _ in clouds]
+        ns = [n for _, n, _ in clouds]
+        return self.align_sources_raw(ptrs, ns, clouds[0][2] if clouds else 12, False, k, reg, guesses, params)
+
+    def align_sources_raw(self, ptrs, ns, stride=12, on_device=False, k=20, reg=REG_PLANE, guesses=None, params=None):
+        """vgicp_align_sources with the B point pointers (host, or device when on_device) and sizes straight through."""
+        B = len(ptrs)
+        P = (C.c_void_p * max(B, 1))(*[int(p) for p in ptrs])
+        N = (C.c_size_t * max(B, 1))(*[int(n) for n in ns])
+        g = None
+        if guesses is not None:
+            g = self._poses_to_c(guesses)
+            if len(g) != 16 * B:
+                raise ValueError("guesses must be (B, 4, 4) with one pose per source")
+        params = params or default_params()
+        res = (AlignResult * max(B, 1))()
+        self._check(self._lib.vgicp_align_sources(self._h, P, N, int(stride), int(bool(on_device)), int(k), int(reg), _dp(g) if g is not None else None, B,
+                                                  C.byref(params), res))
         return list(res)[:B]
 
     def evaluate_poses(self, poses, want_H=False):

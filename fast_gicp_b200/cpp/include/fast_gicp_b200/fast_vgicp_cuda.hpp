@@ -118,6 +118,45 @@ public:
   }
   const double* getFinalTwist() const { return final_twist_; }
 
+  // Multi-source alignment (an extension): each source registered against the current target with this object's k and
+  // regularisation, the optimisers' evaluations sharing launches (vgicp_align_sources).  T_out[i] and converged_out[i] are what
+  // setInputSource(sources[i]) + align(output, guesses[i]) would give (guesses empty: identity); the input source,
+  // getFinalTransformation(), hasConverged() and the final Hessian are left alone.  RBF covariances are not batched: with
+  // GPU_RBF_KERNEL selected this throws.
+  void alignSources(const std::vector<PointCloudSourceConstPtr>& sources, const std::vector<Matrix4>& guesses, std::vector<Matrix4>& T_out, std::vector<bool>& converged_out) {
+    T_out.clear();
+    converged_out.clear();
+    if (!target_) throw std::runtime_error("FastVGICPCuda: alignSources needs an input target");
+    if (neighbor_search_method_ == NearestNeighborMethod::GPU_RBF_KERNEL)
+      throw std::runtime_error("FastVGICPCuda: alignSources computes k-NN covariances; GPU_RBF_KERNEL is not available here");
+    if (!guesses.empty() && guesses.size() != sources.size()) throw std::invalid_argument("FastVGICPCuda: alignSources needs one guess per source");
+    if (sources.empty()) return;
+    multiPrelude();
+    const int n = static_cast<int>(sources.size());
+    std::vector<const float*> xyz(sources.size());
+    std::vector<size_t> sizes(sources.size());
+    for (int i = 0; i < n; i++) {
+      xyz[i] = sources[i]->empty() ? nullptr : &sources[i]->points[0].x;
+      sizes[i] = sources[i]->size();
+    }
+    std::vector<double> g;
+    if (!guesses.empty()) {
+      g.resize(16 * guesses.size());
+      for (int i = 0; i < n; i++)
+        for (int k = 0; k < 16; k++) g[16 * i + k] = static_cast<double>(guesses[i].v[k]);
+    }
+    const vgicp_lsq_params P = this->lsqParams();
+    std::vector<vgicp_align_result> r(sources.size());
+    checkStrict(vgicp_align_sources(vgicp_cuda_, xyz.data(), sizes.data(), sizeof(PointSource), 0, k_correspondences_, static_cast<int>(regularization_method_),
+                                    g.empty() ? nullptr : g.data(), n, &P, r.data()));
+    T_out.resize(sources.size());
+    converged_out.resize(sources.size());
+    for (int i = 0; i < n; i++) {
+      for (int k = 0; k < 16; k++) T_out[i].v[k] = static_cast<float>(r[i].T[k]);
+      converged_out[i] = r[i].converged != 0;
+    }
+  }
+
   virtual void swapSourceAndTarget() override {  // impl:69-72
     check(vgicp_swap_source_and_target(vgicp_cuda_));
     input_.swap(target_);

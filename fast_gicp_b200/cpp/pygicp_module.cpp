@@ -350,6 +350,38 @@ PYBIND11_MODULE(pygicp, m) {
          },
          py::arg("initial_guess") = identity4f(), py::arg("twist_guess") = filled(6, 0.0), py::arg("twist_prior") = py::none(),
          py::arg("twist_weight") = filled(1, 1e-6))
+    // multi-source alignment (not in the reference binding): B (N_i, 3) sources against the current target, (B,4,4) guesses or None
+    // -> (T (B,4,4) float32, converged (B,) bool)
+    .def("align_sources",
+         [](VgicpCuda& v, const std::vector<ArrD>& sources, py::object initial_guesses) {
+           std::vector<VgicpCuda::PointCloudSourceConstPtr> clouds;
+           for (const ArrD& s : sources) clouds.push_back(eigen2pcl(s));
+           std::vector<Eigen::Matrix4f> guesses, T;
+           if (!initial_guesses.is_none()) {
+             ArrF g = initial_guesses.cast<ArrF>();
+             if (g.ndim() != 3 || g.shape(1) != 4 || g.shape(2) != 4) throw std::invalid_argument("initial_guesses must be (B, 4, 4)");
+             auto a = g.unchecked<3>();
+             guesses.resize(g.shape(0));
+             for (py::ssize_t i = 0; i < g.shape(0); i++)
+               for (int r = 0; r < 4; r++) for (int c = 0; c < 4; c++) guesses[i](r, c) = a(i, r, c);
+           }
+           std::vector<bool> converged;
+           {
+             py::gil_scoped_release release;
+             v.alignSources(clouds, guesses, T, converged);
+           }
+           const py::ssize_t n = static_cast<py::ssize_t>(T.size());
+           py::array_t<float> T_out({n, static_cast<py::ssize_t>(4), static_cast<py::ssize_t>(4)});
+           py::array_t<bool> conv_out(n);
+           auto t = T_out.mutable_unchecked<3>();
+           auto cv = conv_out.mutable_unchecked<1>();
+           for (py::ssize_t i = 0; i < n; i++) {
+             for (int r = 0; r < 4; r++) for (int c = 0; c < 4; c++) t(i, r, c) = T[i](r, c);
+             cv(i) = converged[i];
+           }
+           return py::make_tuple(T_out, conv_out);
+         },
+         py::arg("sources"), py::arg("initial_guesses") = py::none())
     .def("get_fitness_score",
          [](VgicpCuda& v, double max_range) {
            double T[16], score = 0.0;

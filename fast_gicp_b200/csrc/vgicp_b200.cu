@@ -292,6 +292,14 @@ struct vgicp_context {
   double ct_t_ref = 0.0;
   DevBuf<float> ct_spare;
   DevBuf<unsigned> ct_stats;  // [3]: k_gather_times' non-finite count, ~key(min), key(max)
+
+  // multi-source alignment (vgicp_align_sources): the sources' points and covariances back to back in one grow-only pool; stage 1
+  // runs source by source on `srcs`, a cloud whose point and covariance arrays are views into the pool and whose neighbour rows and
+  // k-NN scratch are reused from source to source; `src_rows` is the evaluation kernels' row descriptor table
+  DevBuf<float4> src_pts, src_covA;
+  DevBuf<float2> src_covB;
+  Cloud srcs;
+  DevBuf<SourceRow> src_rows;
 };
 
 namespace {
@@ -365,9 +373,10 @@ Pose to_pose(const double* T) {  // Eigen::Isometry3d (column-major) -> float im
 }
 
 int set_cloud(vgicp_handle h, Cloud& c, const float* xyz, size_t n, size_t stride, bool on_device = false) {
-  // NDT: set_{source,target}_cloud resets that cloud's voxel map only (ndt_cuda.cu:104,114); it is rebuilt by the next create_voxelmaps
-  h->ndt_ready = false;
-  {
+  // NDT: set_{source,target}_cloud resets that cloud's voxel map only (ndt_cuda.cu:104,114); it is rebuilt by the next create_voxelmaps.
+  // (The multi-source pool's cloud belongs to neither.)
+  if (&c == &h->source || &c == &h->target) {
+    h->ndt_ready = false;
     VoxelMap& nm = (&c == &h->target) ? h->ndt_t : h->ndt_s;
     nm.built = false;
     nm.pending = false;
@@ -730,24 +739,17 @@ struct LinLaunch {
   int G;        // compacted kernels: lanes per source point in the lookup phase
   int grid;     // blocks (per row of a multi-pose launch)
 };
-// allow_stream = false: the compacted kernels' shape also where DIRECT1 would stream (the continuous-time evaluation has no
-// streaming kernel)
-LinLaunch make_lin_launch(vgicp_handle h, bool allow_stream = true) {
-  Cloud& s = h->source;
+// The evaluation of the source (pts, covA, covB, n): arguments, kernel and grid.  Every evaluation takes its shape from here -- the
+// handle's source (below) and each source of vgicp_align_sources alike.  allow_stream = false: the compacted kernels' shape also where
+// DIRECT1 would stream (the continuous-time evaluation has no streaming kernel)
+LinLaunch make_lin_launch(vgicp_handle h, const float4* pts, const float4* covA, const float2* covB, int n, bool allow_stream = true) {
   VoxelMap& m = h->problem != 0 ? h->ndt_t : h->map;
   LinLaunch L;
   LinArgs& a = L.a;
   a.ndt = h->problem != 0 ? 1 : 0;
   a.robust = h->problem == 0 ? h->robust_kind : 0;  // (the NDT entry points refuse a robust kind before they get here)
   a.robust_d2 = a.robust ? (float)(h->robust_scale * h->robust_scale) : 0.0f;
-  if (h->problem != 0) {  // NDT: target map = ndt_t; source = points + zero covariances (P2D) or source voxel Gaussians (D2D)
-    a.pts = h->problem == 2 ? h->ndt_src_pts.p : s.pts.p;
-    a.covA = h->ndt_src_covA.p; a.covB = h->ndt_src_covB.p; a.n = h->ndt_src_n;
-  } else {
-    const int sb = h->shard_end >= 0 ? h->shard_begin : 0;
-    const int se = h->shard_end >= 0 ? (h->shard_end < s.n ? h->shard_end : s.n) : s.n;
-    a.pts = s.pts.p + sb; a.covA = s.covA.p + sb; a.covB = s.covB.p + sb; a.n = se > sb ? se - sb : 0;
-  }
+  a.pts = pts; a.covA = covA; a.covB = covB; a.n = n;
   a.comm_ranks = h->comm_ranks; a.comm_rank = h->comm_rank; a.comm_seq = 0;
   for (int r = 0; r < kCommMaxRanks; r++) a.comm_peers[r] = h->comm_peers[r];
   a.buckets = m.buckets.p; a.mask = (unsigned)(m.num_buckets - 1); a.max_scan = m.max_scan; a.vox = m.vox.p;
@@ -777,6 +779,15 @@ LinLaunch make_lin_launch(vgicp_handle h, bool allow_stream = true) {
     L.grid = (int)(grid > kLinMaxBlocks ? kLinMaxBlocks : grid);
   }
   return L;
+}
+// the handle's source: VGICP points and covariances (the shard's slice under source sharding), NDT points + zero covariances (P2D)
+// or the source's voxel Gaussians (D2D)
+LinLaunch make_lin_launch(vgicp_handle h, bool allow_stream = true) {
+  Cloud& s = h->source;
+  if (h->problem != 0) return make_lin_launch(h, h->problem == 2 ? h->ndt_src_pts.p : s.pts.p, h->ndt_src_covA.p, h->ndt_src_covB.p, h->ndt_src_n, allow_stream);
+  const int sb = h->shard_end >= 0 ? h->shard_begin : 0;
+  const int se = h->shard_end >= 0 ? (h->shard_end < s.n ? h->shard_end : s.n) : s.n;
+  return make_lin_launch(h, s.pts.p + sb, s.covA.p + sb, s.covB.p + sb, se > sb ? se - sb : 0, allow_stream);
 }
 
 template <int V>
@@ -973,8 +984,9 @@ int multi_upload(vgicp_handle h, int n_hyp, int n_rows) {
 }
 
 // one launch over rows [row0, row0 + n) of the staged row list, all computing `kind`; the records land in rows [row0, row0 + n)
-// of the multi-pose output.  count: also count the hits (kEvalLinearize / kEvalError only).
-int launch_multi(vgicp_handle h, const LinLaunch& L, int n_hyp, int kind, bool count, int row0, int n) {
+// of the multi-pose output.  count: also count the hits (kEvalLinearize / kEvalError only).  src: the multi-source kernels, each
+// row on its own source and grid from this descriptor table (L: the launch class's kernel, grid = the largest of its rows)
+int launch_multi(vgicp_handle h, const LinLaunch& L, int n_hyp, int kind, bool count, int row0, int n, const SourceRow* src = nullptr) {
   const LinArgs& a = L.a;
   const EvalChannel::Dest d = h->multi.dest(h->exec_hint == 0, row0);
   MultiArgs m;
@@ -990,11 +1002,13 @@ int launch_multi(vgicp_handle h, const LinLaunch& L, int n_hyp, int kind, bool c
     auto with_count = [&](auto cnt) {
       constexpr bool COUNT = decltype(cnt)::value && WHAT != kEvalSpec;  // (the speculative evaluation counts no hits)
       if (L.stream) {
-        k_linearize_stream_multi<WHAT, COUNT, RB><<<grid, kLinThreads, sizeof(LinStreamSmem), h->stream>>>(a, m);
+        if (src) k_linearize_stream_multi_src<WHAT, RB><<<grid, kLinThreads, sizeof(LinStreamSmem), h->stream>>>(a, m, src);
+        else k_linearize_stream_multi<WHAT, COUNT, RB><<<grid, kLinThreads, sizeof(LinStreamSmem), h->stream>>>(a, m);
         return true;
       }
       return with_lin_shape(h->offset_mode, L.G, [&](auto mode, auto g) {
-        k_linearize_multi<decltype(mode)::value, WHAT, decltype(g)::value, COUNT, RB><<<grid, kLinThreads, 0, h->stream>>>(a, m);
+        if (src) k_linearize_multi_src<decltype(mode)::value, WHAT, decltype(g)::value, RB><<<grid, kLinThreads, 0, h->stream>>>(a, m, src);
+        else k_linearize_multi<decltype(mode)::value, WHAT, decltype(g)::value, COUNT, RB><<<grid, kLinThreads, 0, h->stream>>>(a, m);
       });
     };
     return count ? with_count(std::true_type{}) : with_count(std::false_type{});
@@ -1359,9 +1373,12 @@ int vgicp_destroy(vgicp_handle h) {
   h->ct_spare.release();
   h->ct_stats.release();
   h->ct.release();
+  h->srcs.release();  // (the views into the pool are not freed here)
+  h->src_pts.release(); h->src_covA.release(); h->src_covB.release();
+  h->src_rows.release();
   for (auto& r : h->prof_pending) { cudaEventDestroy(r.a); cudaEventDestroy(r.b); }
   for (auto e : h->prof_pool) cudaEventDestroy(e);
-  for (cudaEvent_t e : {h->ev_copy, h->ev_append, h->ev_deskew, h->target.ready, h->source.ready})
+  for (cudaEvent_t e : {h->ev_copy, h->ev_append, h->ev_deskew, h->target.ready, h->source.ready, h->srcs.ready})
     if (e) cudaEventDestroy(e);
   if (h->s1.exec) cudaGraphExecDestroy(h->s1.exec);
   if (h->stream_b) cudaStreamDestroy(h->stream_b);
@@ -1834,6 +1851,129 @@ int vgicp_evaluate_poses(vgicp_handle h, const double* T, int n_poses, double* e
     }
     if (n_corr) n_corr[i] = (int64_t)o[kMultiOutCount];
   }
+  return VGICP_OK;
+}
+
+// B source clouds against the current map.  Stage 1 of each source is the handle's own set_cloud / find_neighbors / calc_covariances
+// on a cloud whose arrays are views into the source pool; the optimisers then run as in vgicp_align_multi, one row per source.  The
+// rows of a round are grouped by launch class (streaming or compacted kernel and lanes per point G; the offset table is the
+// handle's): one launch per class and evaluation kind, with the largest grid of its rows.
+int vgicp_align_sources(vgicp_handle h, const float* const* xyz, const size_t* n, size_t stride_bytes, int on_device, int k, int regularization_method,
+                        const double* guesses, int n_sources, const vgicp_lsq_params* params, vgicp_align_result* results) {
+  CHECK_HANDLE(h);
+  DeviceGuard g(h->device);
+  if (!xyz || !n || !results || n_sources < 1 || n_sources > kMultiMaxHyp) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "align_sources: null argument or n_sources outside [1, 4096]");
+  if (stride_bytes < 12 || (stride_bytes % 4) != 0) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "align_sources: stride_bytes must be a multiple of 4 and >= 12");
+  if (k < 1 || k > kMaxK) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "align_sources: need 1 <= k <= 64");
+  if (regularization_method < 0 || regularization_method > 4) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "align_sources: bad regularization method");
+  const int B = n_sources;
+  for (int i = 0; i < B; i++) {
+    if (!xyz[i]) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "align_sources: null points for source " + std::to_string(i));
+    if (n[i] < (size_t)k || n[i] > (size_t)0x7fffffff / 64)
+      return fail(h, VGICP_ERR_INVALID_ARGUMENT, "align_sources: source " + std::to_string(i) + " needs k <= num_points <= 2^31 / 64");
+  }
+  if (h->problem != 0) return fail(h, VGICP_ERR_UNSUPPORTED, "align_sources: defined for the VGICP problem only");
+  if (h->comm_ranks > 1 || h->stage1_sharding || h->shard_end >= 0)
+    return fail(h, VGICP_ERR_UNSUPPORTED, "align_sources: not available with source or stage-1 sharding or in a multi-GPU communicator");
+  if (!h->map.built && !h->map.pending) return fail(h, VGICP_ERR_BAD_STATE, "align_sources: target voxel map not built");
+  int rc = sync_inputs(h);
+  if (rc) return rc;
+  vgicp_lsq_params P;
+  if (params) P = *params; else vgicp_lsq_default_params(&P);
+
+  // pool slots: at least one spare element per source (the streaming kernel reads covB in whole 16-byte units) and an even start,
+  // so that every source's covB is 16-byte aligned like a cloud of its own
+  std::vector<size_t> off(B + 1, 0);
+  size_t n_max = 0;
+  for (int i = 0; i < B; i++) {
+    off[i + 1] = off[i] + ((n[i] + 32) & ~(size_t)31);
+    n_max = n[i] > n_max ? n[i] : n_max;
+  }
+  CU_TRY(h, h->src_pts.reserve(off[B]));
+  CU_TRY(h, h->src_covA.reserve(off[B]));
+  CU_TRY(h, h->src_covB.reserve(off[B]));
+  CU_TRY(h, h->src_rows.reserve(B));
+  Cloud& c = h->srcs;
+  if (!c.ready) {
+    CU_TRY(h, cudaEventCreateWithFlags(&c.ready, cudaEventDisableTiming));
+    c.st = h->stream_b;
+  }
+  CU_TRY(h, c.nbr.reserve(n_max * k));  // (find_neighbors reserves as well; this keeps the buffers from growing source by source)
+  CU_TRY(h, c.knn_scratch.reserve(knn_grid_scratch_bytes((int)n_max, nullptr, nullptr)));
+  // the pool is rewritten on the cloud stream only after everything already enqueued on the main stream (which may read it)
+  CU_TRY(h, cudaEventRecord(c.ready, h->stream));
+  CU_TRY(h, cudaStreamWaitEvent(c.st, c.ready, 0));
+
+  // stage 1, source by source, and each source's launch shape
+  std::vector<SourceRow> desc(B);
+  std::vector<LinLaunch> shape(B);
+  for (int i = 0; i < B; i++) {
+    const size_t cap = off[i + 1] - off[i];
+    c.pts.attach(h->src_pts.p + off[i], cap);
+    c.covA.attach(h->src_covA.p + off[i], cap);
+    c.covB.attach(h->src_covB.p + off[i], cap);
+    c.k = 0;
+    c.has_cov = false;
+    if ((rc = set_cloud(h, c, xyz[i], n[i], stride_bytes, on_device != 0))) return rc;
+    if ((rc = find_neighbors(h, c, k))) return rc;
+    rc = calc_covariances(h, c, regularization_method);
+    if (rc && !(rc == VGICP_ERR_UNSUPPORTED && regularization_method == VGICP_REG_NORMALIZED_MIN_EIG)) return rc;  // (raw covariances, as vgicp_register)
+    shape[i] = make_lin_launch(h, c.pts.p, c.covA.p, c.covB.p, c.n);
+    desc[i] = SourceRow{c.pts.p, c.covA.p, c.covB.p, c.n, shape[i].grid};
+  }
+  CU_TRY(h, cudaMemcpyAsync(h->src_rows.p, desc.data(), sizeof(SourceRow) * B, cudaMemcpyHostToDevice, h->stream));
+  CU_TRY(h, cudaStreamWaitEvent(h->stream, c.ready, 0));
+
+  // launch classes: sources that share a kernel share the launches
+  std::vector<int> cls(B), rep;  // class of each source; rep[c]: a source of class c (its kernel and arguments)
+  int grid_max = 0;
+  for (int i = 0; i < B; i++) {
+    int q = 0;
+    while (q < (int)rep.size() && !(shape[rep[q]].stream == shape[i].stream && shape[rep[q]].G == shape[i].G)) q++;
+    if (q == (int)rep.size()) rep.push_back(i);
+    cls[i] = q;
+    grid_max = shape[i].grid > grid_max ? shape[i].grid : grid_max;
+  }
+  if ((rc = multi_reserve(h, B, grid_max))) return rc;
+  std::vector<LmState<6>> st(B);
+  const double I[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+  for (int i = 0; i < B; i++) st[i] = lm_init<6>(guesses ? guesses + 16 * i : I, P);
+  const bool speculate = h->speculate != 0 && !P.use_gauss_newton;
+  struct Group { int row0, n, cls, grid; bool lin; };
+  std::vector<Group> groups;
+  for (;;) {
+    Pose* poses = multi_poses(h);
+    int* rows = multi_rows(h, B);
+    int nr = 0, n_lin = 0;
+    groups.clear();
+    for (int lin = 1; lin >= 0; lin--) {  // the linearisations first, then the trials; class by class within each
+      for (int q = 0; q < (int)rep.size(); q++) {
+        const int row0 = nr;
+        int grid = 0;
+        for (int i = 0; i < B; i++) {
+          if (cls[i] != q || st[i].phase != (lin ? kLmLinearize : kLmError)) continue;
+          rows[nr++] = i;
+          poses[2 * i] = to_pose(st[i].x0.m);
+          poses[2 * i + 1] = to_pose(lin ? st[i].x0.m : st[i].xi.m);
+          grid = desc[i].grid > grid ? desc[i].grid : grid;
+        }
+        if (nr > row0) groups.push_back(Group{row0, nr - row0, q, grid, lin != 0});
+      }
+      if (lin) n_lin = nr;
+    }
+    if (nr == 0) break;
+    h->multi.seq++;
+    if ((rc = multi_upload(h, B, nr))) return rc;
+    for (const Group& gr : groups) {
+      LinLaunch L = shape[rep[gr.cls]];
+      L.grid = gr.grid;
+      if ((rc = launch_multi(h, L, B, gr.lin ? kEvalLinearize : (speculate ? kEvalSpec : kEvalError), false, gr.row0, gr.n, h->src_rows.p))) return rc;
+    }
+    if ((rc = h->multi.wait(h, nr, (size_t)nr * kMultiOut))) return rc;
+    const double* rec = h->multi.h_out;
+    for (int r = 0; r < nr; r++) lm_consume(&st[rows[r]], rec + (size_t)r * kMultiOut, r >= n_lin && speculate);
+  }
+  for (int i = 0; i < B; i++) lm_result(st[i], &results[i]);
   return VGICP_OK;
 }
 

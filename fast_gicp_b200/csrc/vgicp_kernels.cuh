@@ -654,6 +654,10 @@ __device__ __forceinline__ void apply_jacobian(float3 pe, const PointAcc<WANT_H>
   }
 }
 
+// Blocks of one evaluation: nblk, or gridDim.x when nblk == 0.  A multi-source row passes its own grid (its launch has the largest
+// grid of its rows); every other kernel passes 0, which folds to gridDim.x read where it is used.
+__device__ __forceinline__ unsigned lin_blocks(unsigned nblk) { return nblk ? nblk : gridDim.x; }
+
 // per-warp staging for the compacted evaluation (below)
 constexpr int kLinQueue = 256;  // ring of pending (slot, voxel) hits: a pass adds at most 4*32, a batch of 32 is drained whenever one is full
 struct LinWarpStage {
@@ -708,7 +712,7 @@ __device__ __forceinline__ LinStage<CT>& lin_stage() {
 // xi_eval for the residual, and with WANT_H the sums run to kCtValues (apply_jacobian).  Compile-time flags, not runtime branches:
 // a runtime branch moved the register allocation of the other kernels.
 template <int MODE, bool WANT_H, int G, bool DENSE, bool COUNT, bool RB, bool CT = false>
-__device__ __forceinline__ void lin_accumulate_impl(const LinArgs& a, const Pose& Tl, const Pose& Te, float* sum, const CtArgs* ct = nullptr) {
+__device__ __forceinline__ void lin_accumulate_impl(const LinArgs& a, const Pose& Tl, const Pose& Te, float* sum, unsigned nblk, const CtArgs* ct = nullptr) {
   constexpr int NV = WANT_H ? (CT ? kCtValues : kLinValues) : 1;
   constexpr int NOFF = MODE == 0 ? 0 : MODE;
   // MODE 27: a lane walks whole z-columns (3 cells sharing the x,y hash prefix) of a contiguous run of 27/G cells, G in {1, 3, 9}
@@ -726,7 +730,7 @@ __device__ __forceinline__ void lin_accumulate_impl(const LinArgs& a, const Pose
   const long long n_tasks = (long long)a.n * G;
   constexpr int kWarps = kLinThreads / 32;
   // warp-uniform trip count (the body uses warp votes): lanes past the end are clamped onto the last task and masked out
-  for (long long base = ((long long)blockIdx.x * kWarps + (threadIdx.x >> 5)) * TPW; base < n_tasks; base += (long long)gridDim.x * kWarps * TPW) {
+  for (long long base = ((long long)blockIdx.x * kWarps + (threadIdx.x >> 5)) * TPW; base < n_tasks; base += (long long)lin_blocks(nblk) * kWarps * TPW) {
     const long long task_raw = base + lane;
     const bool active = lane < TPW && task_raw < n_tasks;
     const long long task = active ? task_raw : n_tasks - 1;
@@ -854,9 +858,9 @@ __device__ __forceinline__ void lin_accumulate_impl(const LinArgs& a, const Pose
 }
 
 template <int MODE, bool WANT_H, int G, bool COUNT, bool RB, bool CT = false>
-__device__ __forceinline__ void lin_accumulate(const LinArgs& a, const Pose& Tl, const Pose& Te, float* sum, const CtArgs* ct = nullptr) {
-  if (a.dense.cells) lin_accumulate_impl<MODE, WANT_H, G, true, COUNT, RB, CT>(a, Tl, Te, sum, ct);  // (grid-uniform branch)
-  else lin_accumulate_impl<MODE, WANT_H, G, false, COUNT, RB, CT>(a, Tl, Te, sum, ct);
+__device__ __forceinline__ void lin_accumulate(const LinArgs& a, const Pose& Tl, const Pose& Te, float* sum, unsigned nblk, const CtArgs* ct = nullptr) {
+  if (a.dense.cells) lin_accumulate_impl<MODE, WANT_H, G, true, COUNT, RB, CT>(a, Tl, Te, sum, nblk, ct);  // (grid-uniform branch)
+  else lin_accumulate_impl<MODE, WANT_H, G, false, COUNT, RB, CT>(a, Tl, Te, sum, nblk, ct);
 }
 
 // block reduction (warp shuffles in float -> shared in double -> per-block partial), ticket, fixed-order fold by the last
@@ -864,10 +868,11 @@ __device__ __forceinline__ void lin_accumulate(const LinArgs& a, const Pose& Tl,
 // (Tried and dropped: a first-level reduction over distributed shared memory inside 8-block clusters, so that the last block folds
 // grid/8 partials.  It gained little at 17 k points and lost at 1 M points, where the cluster placement constraint left SMs idle
 // at the tail of the single wave.)
-// `partials` ([gridDim.x][STRIDE]) and `ticket` belong to one evaluation: a.partials / a.ticket, or one hypothesis's slice of a
-// multi-pose launch, or the continuous-time evaluation's own (STRIDE = kCtStride)
+// `partials` ([nblk][STRIDE]) and `ticket` belong to one evaluation: a.partials / a.ticket, or one hypothesis's slice of a
+// multi-pose launch, or the continuous-time evaluation's own (STRIDE = kCtStride).  nblk: the evaluation's block count -- gridDim.x,
+// or a multi-source row's own grid (the blocks past it have left before they get here); 0 = gridDim.x (lin_blocks)
 template <int NV, int STRIDE = kLinStride>
-__device__ __forceinline__ bool lin_reduce(const LinArgs& a, const float* sum, double (*fin)[STRIDE], double* partials, unsigned int* ticket) {
+__device__ __forceinline__ bool lin_reduce(const LinArgs& a, const float* sum, double (*fin)[STRIDE], double* partials, unsigned int* ticket, unsigned nblk) {
   static_assert(NV <= STRIDE && NV <= kLinThreads, "one partial row holds the sums; one thread per value folds the chains");
   // ---- block reduction: warp shuffles (float) -> shared (double) -> per-block partial ----
   __shared__ double sh[kLinThreads / 32][STRIDE];
@@ -891,7 +896,7 @@ __device__ __forceinline__ bool lin_reduce(const LinArgs& a, const float* sum, d
   __syncthreads();
   if (threadIdx.x == 0) {
     unsigned t = atomicAdd(ticket, 1u);
-    is_last = (t == gridDim.x - 1);
+    is_last = (t == lin_blocks(nblk) - 1);
   }
   __syncthreads();
   if (!is_last) return false;
@@ -905,14 +910,14 @@ __device__ __forceinline__ bool lin_reduce(const LinArgs& a, const float* sum, d
       double s = 0.0;
       const double* part = partials + v;
       unsigned b = chain;
-      for (; b + 4 * 15 < gridDim.x; b += 4 * 16) {
+      for (; b + 4 * 15 < lin_blocks(nblk); b += 4 * 16) {
         double t[16];
 #pragma unroll
         for (int u = 0; u < 16; u++) t[u] = __ldcg(part + (size_t)(b + 4 * u) * STRIDE);
 #pragma unroll
         for (int u = 0; u < 16; u++) s += t[u];
       }
-      for (; b < gridDim.x; b += 4) s += __ldcg(part + (size_t)b * STRIDE);
+      for (; b < lin_blocks(nblk); b += 4) s += __ldcg(part + (size_t)b * STRIDE);
       fin[chain][v] = s;
     };
     if constexpr (NV <= 32) {
@@ -964,7 +969,7 @@ __device__ __forceinline__ bool lin_reduce(const LinArgs& a, const float* sum, d
 }
 template <int NV>
 __device__ __forceinline__ bool lin_reduce(const LinArgs& a, const float* sum, double (*fin)[kLinStride]) {
-  return lin_reduce<NV>(a, sum, fin, a.partials, a.ticket);
+  return lin_reduce<NV>(a, sum, fin, a.partials, a.ticket, 0);
 }
 
 // unpack the folded sums into err, H (36, column-major), b (6)
@@ -1014,24 +1019,24 @@ __device__ __forceinline__ void lin_publish(unsigned int* tickets, volatile unsi
 // an accepted step saves a launch and a host round trip, a rejected one discards the second half.
 //   out[0..42] = err, H, b at xi (linearised at xi);  out[43] = err at xi over the old correspondences
 template <int MODE, int G, bool RB>
-__device__ __forceinline__ void lin_spec_accumulate(const LinArgs& a, const Pose& Tl, const Pose& Te, float* sum) {  // sum[kLinValues + 1]
+__device__ __forceinline__ void lin_spec_accumulate(const LinArgs& a, const Pose& Tl, const Pose& Te, float* sum, unsigned nblk) {  // sum[kLinValues + 1]
   {
     float e_old[1];
-    lin_accumulate<MODE, false, G, false, RB>(a, Tl, Te, e_old);
+    lin_accumulate<MODE, false, G, false, RB>(a, Tl, Te, e_old, nblk);
     sum[kLinValues] = e_old[0];
   }
   {
     float lin[kLinValues];
-    lin_accumulate<MODE, true, G, false, RB>(a, Te, Te, lin);
+    lin_accumulate<MODE, true, G, false, RB>(a, Te, Te, lin, nblk);
 #pragma unroll
     for (int i = 0; i < kLinValues; i++) sum[i] = lin[i];
   }
 }
 // the sums of an evaluation kind (COUNT: kEvalError / kEvalLinearize only)
 template <int MODE, int WHAT, int G, bool COUNT, bool RB>
-__device__ __forceinline__ void lin_eval_accumulate(const LinArgs& a, const Pose& Tl, const Pose& Te, float* sum) {
-  if constexpr (WHAT == kEvalSpec) lin_spec_accumulate<MODE, G, RB>(a, Tl, Te, sum);
-  else lin_accumulate<MODE, WHAT == kEvalLinearize, G, COUNT, RB>(a, Tl, Te, sum);
+__device__ __forceinline__ void lin_eval_accumulate(const LinArgs& a, const Pose& Tl, const Pose& Te, float* sum, unsigned nblk) {
+  if constexpr (WHAT == kEvalSpec) lin_spec_accumulate<MODE, G, RB>(a, Tl, Te, sum, nblk);
+  else lin_accumulate<MODE, WHAT == kEvalLinearize, G, COUNT, RB>(a, Tl, Te, sum, nblk);
 }
 
 // One evaluation (update_correspondences + compute_error fused).  MODE: 0 = offsets from memory (DIRECT_RADIUS or anything),
@@ -1042,7 +1047,7 @@ __global__ void __launch_bounds__(kLinThreads) k_linearize(const LinArgs a) {
   constexpr int NV = eval_values(WHAT);
   __shared__ double fin[4][kLinStride];
   float sum[NV];
-  lin_eval_accumulate<MODE, WHAT, G, false, RB>(a, a.Tlin, a.Teval, sum);
+  lin_eval_accumulate<MODE, WHAT, G, false, RB>(a, a.Tlin, a.Teval, sum, 0);
   if (!lin_reduce<NV>(a, sum, fin)) return;
   if (threadIdx.x == 0) {
     lin_write_record<WHAT>(fin[0], a.out);
@@ -1057,8 +1062,8 @@ __global__ void __launch_bounds__(kLinThreads) k_linearize_ct(const LinArgs a, c
   constexpr int NV = WANT_H ? kCtValues : 1;
   __shared__ double fin[4][kCtStride];
   float sum[NV];
-  lin_accumulate<MODE, WANT_H, G, false, RB, true>(a, a.Tlin, a.Teval, sum, &c);
-  if (!lin_reduce<NV, kCtStride>(a, sum, fin, c.partials, c.ticket)) return;
+  lin_accumulate<MODE, WANT_H, G, false, RB, true>(a, a.Tlin, a.Teval, sum, 0, &c);
+  if (!lin_reduce<NV, kCtStride>(a, sum, fin, c.partials, c.ticket, 0)) return;
   if (threadIdx.x == 0) {
     for (int j = 0; j < NV; j++) c.out[j] = fin[0][j];
     lin_publish(c.ticket, c.done_flag, c.done_seq);
@@ -1144,7 +1149,7 @@ __device__ __forceinline__ void lin_stream_point(const LinArgs& a, const Pose& T
 
 // COUNT (kEvalError / kEvalLinearize): one more slot counts the hits.
 template <int WHAT, bool COUNT, bool RB>
-__device__ __forceinline__ void lin_stream_accumulate(const LinArgs& a, const Pose& Tl, const Pose& Te, float* sum) {
+__device__ __forceinline__ void lin_stream_accumulate(const LinArgs& a, const Pose& Tl, const Pose& Te, float* sum, unsigned nblk) {
   constexpr int NV = eval_values(WHAT) + (COUNT ? 1 : 0);
   static_assert(!COUNT || WHAT != kEvalSpec, "the speculative evaluation does not count hits");
   extern __shared__ __align__(128) unsigned char stream_smem_raw[];
@@ -1158,7 +1163,7 @@ __device__ __forceinline__ void lin_stream_accumulate(const LinArgs& a, const Po
   __syncthreads();
   const int n_tiles = (a.n + kLinStreamTile - 1) / kLinStreamTile;
   auto issue = [&](int it) {  // tile number it of this block -> stage it % kLinStreamStages
-    const long long tile = (long long)blockIdx.x + (long long)it * gridDim.x;
+    const long long tile = (long long)blockIdx.x + (long long)it * lin_blocks(nblk);
     if (tile >= n_tiles) return;
     const int s = it % kLinStreamStages;
     const int first = (int)tile * kLinStreamTile;
@@ -1174,7 +1179,7 @@ __device__ __forceinline__ void lin_stream_accumulate(const LinArgs& a, const Po
 #pragma unroll
   for (int i = 0; i < NV; i++) sum[i] = 0.f;
   for (int it = 0;; it++) {
-    const long long tile = (long long)blockIdx.x + (long long)it * gridDim.x;
+    const long long tile = (long long)blockIdx.x + (long long)it * lin_blocks(nblk);
     if (tile >= n_tiles) break;
     const int s = it % kLinStreamStages;
     if (tid == 0) issue(it + kLinStreamStages - 1);  // refills the stage read in iteration it - 1 (all threads are past its barrier)
@@ -1204,7 +1209,7 @@ __global__ void __launch_bounds__(kLinThreads) k_linearize_stream(const LinArgs 
   constexpr int NV = eval_values(WHAT);
   __shared__ double fin[4][kLinStride];
   float sum[NV];
-  lin_stream_accumulate<WHAT, false, RB>(a, a.Tlin, a.Teval, sum);
+  lin_stream_accumulate<WHAT, false, RB>(a, a.Tlin, a.Teval, sum, 0);
   if (!lin_reduce<NV>(a, sum, fin)) return;
   if (threadIdx.x == 0) {
     lin_write_record<WHAT>(fin[0], a.out);
@@ -1245,7 +1250,7 @@ __device__ __forceinline__ int multi_row(const MultiArgs& m, Pose* sp) {
 }
 template <int NV>
 __device__ __forceinline__ bool multi_reduce(const LinArgs& a, const MultiArgs& m, int y, const float* sum, double (*fin)[kLinStride]) {
-  return lin_reduce<NV>(a, sum, fin, m.partials + (size_t)y * gridDim.x * kLinStride, m.tickets + y);
+  return lin_reduce<NV>(a, sum, fin, m.partials + (size_t)y * gridDim.x * kLinStride, m.tickets + y, 0);
 }
 // thread 0 of a row's last block: the row's record, its hit count (COUNT), then the row's ticket and completion word
 template <int WHAT, bool COUNT>
@@ -1264,7 +1269,7 @@ __global__ void __launch_bounds__(kLinThreads, 1) k_linearize_multi(const LinArg
   __shared__ Pose sp[2];
   const int y = multi_row(m, sp);
   float sum[NV];
-  lin_eval_accumulate<MODE, WHAT, G, COUNT, RB>(a, sp[0], sp[1], sum);
+  lin_eval_accumulate<MODE, WHAT, G, COUNT, RB>(a, sp[0], sp[1], sum, 0);
   if (!multi_reduce<NV>(a, m, y, sum, fin)) return;
   if (threadIdx.x == 0) multi_finish<WHAT, COUNT>(m, y, fin[0]);
 }
@@ -1276,9 +1281,61 @@ __global__ void __launch_bounds__(kLinThreads, 1) k_linearize_stream_multi(const
   __shared__ Pose sp[2];
   const int y = multi_row(m, sp);
   float sum[NV];
-  lin_stream_accumulate<WHAT, COUNT, RB>(a, sp[0], sp[1], sum);
+  lin_stream_accumulate<WHAT, COUNT, RB>(a, sp[0], sp[1], sum, 0);
   if (!multi_reduce<NV>(a, m, y, sum, fin)) return;
   if (threadIdx.x == 0) multi_finish<WHAT, COUNT>(m, y, fin[0]);
+}
+
+// Multi-source evaluation (vgicp_align_sources): many source clouds against the same map.  m.hyp[y] names row y's source, which is
+// both its pose pair in m.poses and its entry in the descriptor table: the source's arrays, its size and the grid of its
+// single-pose launch.  The launch has the largest grid of its rows; a row's blocks past its own grid leave at once, and the others
+// split the tasks and fold the partials over the row's grid, not gridDim.x, so each row's sums are its single-pose sums bit for bit.
+struct SourceRow {
+  const float4* pts;
+  const float4* covA;
+  const float2* covB;
+  int n;
+  int grid;
+};
+
+// the row's source and grid, or false in the blocks past the row's grid (before any barrier, shared store or partial)
+__device__ __forceinline__ bool source_row(const MultiArgs& m, const SourceRow* src, SourceRow& s) {
+  s = src[__ldg(&m.hyp[blockIdx.y])];
+  return blockIdx.x < (unsigned)s.grid;
+}
+// the single-pose arguments with the row's source in place of the handle's
+__device__ __forceinline__ LinArgs source_args(const LinArgs& a, const SourceRow& s) {
+  LinArgs r = a;
+  r.pts = s.pts; r.covA = s.covA; r.covB = s.covB; r.n = s.n;
+  return r;
+}
+
+template <int MODE, int WHAT, int G, bool RB>
+__global__ void __launch_bounds__(kLinThreads, 1) k_linearize_multi_src(const LinArgs a, const MultiArgs m, const SourceRow* __restrict__ src) {
+  constexpr int NV = eval_values(WHAT);
+  __shared__ double fin[4][kLinStride];
+  __shared__ Pose sp[2];
+  SourceRow s;
+  if (!source_row(m, src, s)) return;
+  const int y = multi_row(m, sp);
+  float sum[NV];
+  lin_eval_accumulate<MODE, WHAT, G, false, RB>(source_args(a, s), sp[0], sp[1], sum, (unsigned)s.grid);
+  if (!lin_reduce<NV>(a, sum, fin, m.partials + (size_t)y * gridDim.x * kLinStride, m.tickets + y, (unsigned)s.grid)) return;
+  if (threadIdx.x == 0) multi_finish<WHAT, false>(m, y, fin[0]);
+}
+
+template <int WHAT, bool RB>
+__global__ void __launch_bounds__(kLinThreads, 1) k_linearize_stream_multi_src(const LinArgs a, const MultiArgs m, const SourceRow* __restrict__ src) {
+  constexpr int NV = eval_values(WHAT);
+  __shared__ double fin[4][kLinStride];
+  __shared__ Pose sp[2];
+  SourceRow s;
+  if (!source_row(m, src, s)) return;
+  const int y = multi_row(m, sp);
+  float sum[NV];
+  lin_stream_accumulate<WHAT, false, RB>(source_args(a, s), sp[0], sp[1], sum, (unsigned)s.grid);
+  if (!lin_reduce<NV>(a, sum, fin, m.partials + (size_t)y * gridDim.x * kLinStride, m.tickets + y, (unsigned)s.grid)) return;
+  if (threadIdx.x == 0) multi_finish<WHAT, false>(m, y, fin[0]);
 }
 
 // Materialise the reference's correspondence list for the getter (fast_vgicp_cuda.cu:221-225): dense [n_off][n] voxel ids,

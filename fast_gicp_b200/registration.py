@@ -469,6 +469,31 @@ class FastVGICPCuda(LsqRegistration):
             return self.final_transformation_, self.vgicp_cuda_.transform_source(self.final_transformation_.astype(np.float64))[:, :3]
         return self.final_transformation_
 
+    def alignSources(self, sources, initial_guesses=None):
+        """Register each of the B source clouds against the current target, the optimisers' evaluations sharing launches
+        (vgicp_align_sources), with this object's k and regularisation.
+
+        Returns (T (B, 4, 4) float32, converged (B,) bool); T[i] equals what setInputSource(sources[i]) + align(initial_guesses[i])
+        returns.  initial_guesses: (B, 4, 4), None = identity.  The input source and the state of the single registration
+        (getFinalTransformation, hasConverged, the final Hessian) are left alone.  RBF covariances are not batched: with
+        GPU_RBF_KERNEL selected this raises."""
+        if self.target_ is None:
+            raise RuntimeError("alignSources: input target not set")
+        if self.neighbor_search_method_ == NearestNeighborMethod.GPU_RBF_KERNEL:
+            raise RuntimeError("alignSources: GPU_RBF_KERNEL covariances are not available here; use the k-NN methods or a loop of align")
+        G = None
+        if initial_guesses is not None:
+            G = np.asarray(initial_guesses, dtype=np.float32).astype(np.float64)  # cast like align's guess
+            if G.ndim != 3 or G.shape[1:] != (4, 4) or len(G) != len(sources):
+                raise ValueError("initial_guesses must be (B, 4, 4), one per source")
+        self._prelude()
+        res = self.vgicp_cuda_.align_sources(sources, G, self.k_correspondences_, int(self.regularization_method_), self._params())
+        T = np.stack([_core.pose_from_c(r.T) for r in res]).astype(np.float32)
+        return T, np.array([bool(r.converged) for r in res])
+
+    def align_sources(self, sources, initial_guesses=None):
+        return self.alignSources(sources, initial_guesses)
+
     def getFitnessScore(self, max_range=float("inf")):
         """pcl::Registration::getFitnessScore: mean squared nearest-neighbour distance of the aligned source to the target."""
         return self.vgicp_cuda_.fitness_score(self.final_transformation_.astype(np.float64), max_range)

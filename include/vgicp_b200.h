@@ -171,6 +171,29 @@ VGICP_API int vgicp_align_multi(vgicp_handle h, const double* guesses, int n_gue
  * correspondences, so rank hypotheses by err normalised with n_corr, not by err alone.  Handle state unchanged; 1 <= n_poses <= 4096;
  * errors as vgicp_align_multi. */
 VGICP_API int vgicp_evaluate_poses(vgicp_handle h, const double* T, int n_poses, double* err, double* H36, double* b6, int64_t* n_corr);
+/* ---- multi-source alignment (multi-LiDAR rigs, keyframes against one submap, a recorded log against a prebuilt map) ----------
+ * B source clouds registered against the current target map in one call.  Source i is xyz[i] with n[i] points, stride_bytes apart
+ * (one stride for all), host pointers or device pointers when on_device != 0; guesses: B x 16 doubles (column-major), NULL = the
+ * identity for every source.  Stage 1 runs source by source on the library's k-NN and covariance kernels (k neighbours,
+ * regularization_method); the optimisers of all sources then share their evaluation launches, as in vgicp_align_multi: each round
+ * groups the running sources by launch class (streaming or compacted kernel, lanes per point; sources of different sizes can fall in
+ * different classes, e.g. DIRECT1 streams from 65 536 points with the direct index) and issues one launch per class and evaluation
+ * kind, each source a row of blocks with the grid of its own single-pose launch.
+ * results[i] equals, bit for bit (T, H, nr_iterations, converged, n_linearize, n_compute_error, lm_failed), what the same handle
+ * returns for vgicp_set_source_cloud(xyz[i], n[i], stride_bytes) (or _device) + vgicp_find_source_neighbors(k) +
+ * vgicp_calculate_source_covariances(regularization_method) + vgicp_align(guesses + 16 i, params), under either execution hint and
+ * speculation setting, with every neighbour search, voxel index and robust kind.  NORMALIZED_MIN_EIG behaves as in vgicp_register:
+ * the raw covariances are used and the call registers.
+ * The handle's own source (points, neighbour rows, covariances, timestamps), its linearisation point and the rest of its
+ * single-pose state are left as they were; so are the target and its map.  1 <= n_sources <= 4096, 1 <= k <= min(n[i], 64).
+ * Working memory, grow-only: the sources live in one pool of about 40 bytes per point (float4 point, float4 + float2 covariance);
+ * neighbour rows are not kept (one table of the largest source's rows is reused), plus vgicp_align_multi's 256 bytes per evaluation
+ * block and source.
+ * Errors, every one returned before anything is launched or modified: VGICP_ERR_INVALID_ARGUMENT (null handle or pointer, n_sources
+ * out of range, a bad k, size, stride or regularization method), VGICP_ERR_BAD_STATE (no target voxel map), VGICP_ERR_UNSUPPORTED
+ * (an NDT problem, source or stage-1 sharding, a multi-GPU communicator). */
+VGICP_API int vgicp_align_sources(vgicp_handle h, const float* const* xyz, const size_t* n, size_t stride_bytes, int on_device, int k, int regularization_method,
+                                  const double* guesses /* B x 16, NULL = identity */, int n_sources, const vgicp_lsq_params* params, vgicp_align_result* results);
 /* One whole registration: clearTarget/clearSource + setInputTarget + setInputSource + align (the body of the reference's
  * benchmark loop, src/align.cpp:72-81) with GPU k-NN covariances.  xyz are host pointers, or device pointers when on_device != 0. */
 VGICP_API int vgicp_register(vgicp_handle h, const float* target_xyz, size_t n_target, const float* source_xyz, size_t n_source, size_t stride_bytes, int on_device, int k,
