@@ -45,7 +45,7 @@ EXPORTED_SYMBOLS = [
     "vgicp_comm_export", "vgicp_comm_init", "vgicp_comm_shutdown", "vgicp_comm_error", "vgicp_set_source_shard", "vgicp_clear_source_shard",
     "vgicp_comm_export_arena", "vgicp_comm_init_arena", "vgicp_set_stage1_sharding", "vgicp_set_source_covariances", "vgicp_set_target_covariances",
     "vgicp_align_multi", "vgicp_evaluate_poses", "vgicp_set_robust_kernel",
-    "vgicp_append_source_to_target", "vgicp_crop_target", "vgicp_deskew_source",
+    "vgicp_append_source_to_target", "vgicp_crop_target", "vgicp_thin_target", "vgicp_deskew_source",
     "vgicp_set_source_timestamps", "vgicp_compute_error_ct", "vgicp_align_ct",
     "vgicp_set_source_timestamps_device", "vgicp_deskew_source_stored", "vgicp_align_sources",
 ]
@@ -172,6 +172,7 @@ def load_library():
         "vgicp_get_profile": [hp, dp, C.POINTER(C.c_uint64), C.c_int],
         "vgicp_append_source_to_target": [hp, dp],
         "vgicp_crop_target": [hp, dp, C.c_double, C.c_size_t],
+        "vgicp_thin_target": [hp, C.c_double, C.c_int],
         "vgicp_deskew_source": [hp, C.c_void_p, C.c_size_t, C.c_size_t, dp, C.c_double],
         "vgicp_set_source_timestamps": [hp, C.c_void_p, C.c_size_t, C.c_size_t, C.c_double],
         "vgicp_compute_error_ct": [hp, dp, dp, dp, dp, dp, dp, dp],
@@ -596,6 +597,11 @@ class Core:
         (0 = no cap); rebuild the voxel map.  A crop that would leave no points raises and changes nothing."""
         c = np.ascontiguousarray(np.asarray(center, dtype=np.float64).reshape(3))
         self._check(self._lib.vgicp_crop_target(self._h, _dp(c), float(radius), int(max_points)))
+
+    def thin_target(self, leaf_size, max_points_per_voxel):
+        """Keep at most max_points_per_voxel target points per cell floor(p * (1 / leaf_size)) (float32), the oldest in array
+        order; rebuild the voxel map.  Kept rows are unchanged and stay in order.  Errors raise and change nothing."""
+        self._check(self._lib.vgicp_thin_target(self._h, float(leaf_size), int(max_points_per_voxel)))
 
     # ---- motion compensation
     def deskew_source(self, times, twist, t_ref=0.0):

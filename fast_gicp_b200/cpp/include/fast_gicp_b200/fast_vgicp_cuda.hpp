@@ -71,6 +71,11 @@ public:
     checkStrict(vgicp_crop_target(vgicp_cuda_, center, radius, max_points));
     target_ = pcl::make_shared<PointCloudTarget>();
   }
+  // keep at most `max_points_per_voxel` target points per cell of a `leaf_size` grid, the oldest (call after appendSourceToTarget)
+  void thinTarget(double leaf_size, int max_points_per_voxel) {
+    checkStrict(vgicp_thin_target(vgicp_cuda_, leaf_size, max_points_per_voxel));
+    target_ = pcl::make_shared<PointCloudTarget>();
+  }
 
   // Motion compensation (an extension): every source point becomes Exp((t_i - t_ref) twist) p_i, the point in the sensor frame at
   // t_ref (include/vgicp_b200.h), then the source covariances are recomputed as setInputSource computes them.  t: n float

@@ -294,6 +294,7 @@ PYBIND11_MODULE(pygicp, m) {
            v.cropTarget(center.data(), radius, max_points);
          },
          py::arg("center"), py::arg("radius"), py::arg("max_points") = 0)
+    .def("thin_target", &VgicpCuda::thinTarget, py::arg("leaf_size"), py::arg("max_points_per_voxel"))
     // motion compensation (not in the reference binding): one relative timestamp per source point, twist = [omega, v]
     .def("deskew_source",
          [](VgicpCuda& v, const ArrF& times, const ArrD& twist, double t_ref) {

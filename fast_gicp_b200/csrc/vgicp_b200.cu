@@ -300,6 +300,14 @@ struct vgicp_context {
   DevBuf<float2> src_covB;
   Cloud srcs;
   DevBuf<SourceRow> src_rows;
+
+  // voxel-capped thinning of the local map (vgicp_thin_target): u64 cell keys and original indices sorted stably (vgicp_sort.cuh),
+  // the sort's scratch, the per-point keep mask k_crop_rank reads, and the box pass's words
+  DevBuf<unsigned long long> thin_keys[2];
+  DevBuf<unsigned> thin_vals[2];
+  DevBuf<unsigned char> thin_scratch;
+  DevBuf<unsigned char> thin_keep;
+  DevBuf<unsigned> thin_box;
 };
 
 namespace {
@@ -1365,6 +1373,8 @@ int vgicp_destroy(vgicp_handle h) {
   h->ndt_src_pts.release(); h->ndt_src_covA.release(); h->ndt_src_covB.release();
   h->crop_rank.release(); h->crop_state.release();
   h->spare_pts.release(); h->spare_covA.release(); h->spare_covB.release();
+  for (int j = 0; j < 2; j++) { h->thin_keys[j].release(); h->thin_vals[j].release(); }
+  h->thin_scratch.release(); h->thin_keep.release(); h->thin_box.release();
   h->eval.release();
   h->multi.release();
   if (h->d_multi_in) cudaFree(h->d_multi_in);
@@ -2206,16 +2216,11 @@ int vgicp_append_source_to_target(vgicp_handle h, const double T[16]) {
   return local_map_rebuild(h);
 }
 
-int vgicp_crop_target(vgicp_handle h, const double center[3], double radius, size_t max_points) {
-  CHECK_HANDLE(h);
-  DeviceGuard g(h->device);
-  if (!center) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "crop_target: null center");
-  if (!(radius >= 0.0)) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "crop_target: radius must be >= 0 (NaN is rejected; +inf keeps every point)");
-  int rc = local_map_check(h, "crop_target");
-  if (rc) return rc;
+// k_crop_rank over the target (keep: the optional per-point mask) and the read-back of the number of passing points, the one
+// synchronisation of a crop and the second of a thinning; also sizes the spare arrays k_crop_scatter compacts into
+static int local_map_rank(vgicp_handle h, const unsigned char* keep, float cx, float cy, float cz, float r2, size_t* passed) {
   Cloud& t = h->target;
   const int n = t.n;
-  if (n == 0) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "crop_target: the crop would leave no points");
   const int blocks = blocks_for(n, kCropThreads);
   CU_TRY(h, h->crop_rank.reserve(n));
   {
@@ -2235,24 +2240,117 @@ int vgicp_crop_target(vgicp_handle h, const double center[3], double radius, siz
   CU_TRY(h, h->spare_covB.reserve(n));
   int* d_count = h->map.d_counters + 10;
   KLAUNCH_ST(h, t.st, VGICP_PROF_OTHER,
-             k_crop_rank<<<blocks, kCropThreads, 0, t.st>>>(t.pts.p, n, (float)center[0], (float)center[1], (float)center[2], (float)(radius * radius), h->crop_rank.p, d_count,
-                                                            h->crop_state.p, h->crop_epoch));
+             k_crop_rank<<<blocks, kCropThreads, 0, t.st>>>(t.pts.p, keep, n, cx, cy, cz, r2, h->crop_rank.p, d_count, h->crop_state.p, h->crop_epoch));
   CU_TRY(h, cudaGetLastError());
-  // the host needs the new size (and must refuse an empty result before anything is modified): one synchronisation
+  // the host needs the new size (and must refuse an empty result before anything is modified)
   CU_TRY(h, cudaMemcpyAsync(h->map.h_counters + 10, d_count, sizeof(int), cudaMemcpyDeviceToHost, t.st));
   CU_TRY(h, cudaStreamSynchronize(t.st));
-  const size_t passed = (size_t)h->map.h_counters[10];
-  const size_t first = (max_points > 0 && passed > max_points) ? passed - max_points : 0;
-  const int kept = (int)(passed - first);
-  if (kept == 0) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "crop_target: the crop would leave no points");
+  *passed = (size_t)h->map.h_counters[10];
+  return VGICP_OK;
+}
+
+// rows with rank >= first go to the spare arrays, which become the target's; then the map is rebuilt
+static int local_map_compact(vgicp_handle h, int first, int kept) {
+  Cloud& t = h->target;
+  const int n = t.n;
   KLAUNCH_ST(h, t.st, VGICP_PROF_OTHER,
-             k_crop_scatter<<<blocks_for(n, 256), 256, 0, t.st>>>(t.pts.p, t.covA.p, t.covB.p, h->crop_rank.p, n, (int)first, h->spare_pts.p, h->spare_covA.p, h->spare_covB.p));
+             k_crop_scatter<<<blocks_for(n, 256), 256, 0, t.st>>>(t.pts.p, t.covA.p, t.covB.p, h->crop_rank.p, n, first, h->spare_pts.p, h->spare_covA.p, h->spare_covB.p));
   CU_TRY(h, cudaGetLastError());
   std::swap(t.pts, h->spare_pts);
   std::swap(t.covA, h->spare_covA);
   std::swap(t.covB, h->spare_covB);
   t.n = kept;
   return local_map_rebuild(h);
+}
+
+int vgicp_crop_target(vgicp_handle h, const double center[3], double radius, size_t max_points) {
+  CHECK_HANDLE(h);
+  DeviceGuard g(h->device);
+  if (!center) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "crop_target: null center");
+  if (!(radius >= 0.0)) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "crop_target: radius must be >= 0 (NaN is rejected; +inf keeps every point)");
+  int rc = local_map_check(h, "crop_target");
+  if (rc) return rc;
+  if (h->target.n == 0) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "crop_target: the crop would leave no points");
+  size_t passed = 0;
+  if ((rc = local_map_rank(h, nullptr, (float)center[0], (float)center[1], (float)center[2], (float)(radius * radius), &passed))) return rc;
+  const size_t first = (max_points > 0 && passed > max_points) ? passed - max_points : 0;
+  const int kept = (int)(passed - first);
+  if (kept == 0) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "crop_target: the crop would leave no points");
+  return local_map_compact(h, (int)first, kept);
+}
+
+// Thinning: the cells' box and the refusals the points decide (sync 1), u64 cell keys of the box's width with their digit
+// histograms, the stable radix sort, the keep mask from the run test, then the crop's rank (sync 2: the new size) and scatter
+int vgicp_thin_target(vgicp_handle h, double leaf_size, int max_points_per_voxel) {
+  CHECK_HANDLE(h);
+  DeviceGuard g(h->device);
+  if (!std::isfinite(leaf_size) || !(leaf_size > 0.0)) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "thin_target: leaf_size must be finite and > 0");
+  const float l = (float)leaf_size;
+  const float inv = 1.0f / l;
+  if (!(std::isfinite(l) && l > 0.0f && std::isfinite(inv) && inv > 0.0f))
+    return fail(h, VGICP_ERR_INVALID_ARGUMENT, "thin_target: (float)leaf_size and its reciprocal must be finite and > 0");
+  if (max_points_per_voxel < 1) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "thin_target: max_points_per_voxel must be >= 1");
+  int rc = local_map_check(h, "thin_target");
+  if (rc) return rc;
+  Cloud& t = h->target;
+  const int n = t.n;
+  if (n == 0) return fail(h, VGICP_ERR_BAD_STATE, "thin_target: the target has no points");
+  // 1. the box of the cells, read back: the refusals and the key width are decided before anything is modified
+  CU_TRY(h, h->thin_box.reserve(kThinBoxWords));
+  CU_TRY(h, cudaMemsetAsync(h->thin_box.p, 0, kThinBoxWords * sizeof(unsigned), t.st));
+  const int bb = blocks_for(n, kThinBoxThreads);
+  KLAUNCH_ST(h, t.st, VGICP_PROF_OTHER, k_thin_box<<<bb < 4 * kNumSMs ? bb : 4 * kNumSMs, kThinBoxThreads, 0, t.st>>>(t.pts.p, n, inv, h->thin_box.p));
+  CU_TRY(h, cudaGetLastError());
+  unsigned box[kThinBoxWords];
+  CU_TRY(h, cudaMemcpyAsync(box, h->thin_box.p, sizeof(box), cudaMemcpyDeviceToHost, t.st));
+  CU_TRY(h, cudaStreamSynchronize(t.st));
+  if (box[6]) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "thin_target: a target point has a non-finite coordinate");
+  if (box[7]) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "thin_target: a cell floor(p * (1 / leaf)) lies outside [-2^31, 2^31)");
+  int lo[3], bits[3];
+  for (int a = 0; a < 3; a++) {
+    lo[a] = thin_dec(~box[a]);
+    const unsigned span = box[3 + a] - ~box[a];  // max - min
+    bits[a] = span ? 32 - __builtin_clz(span) : 0;
+  }
+  const int key_bits = bits[0] + bits[1] + bits[2];
+  if (key_bits > 64) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "thin_target: the cell key would be wider than 64 bits (leaf too small for the map's extent)");
+  // 2. keys and digit histograms; 3. the sort (nothing to sort when every point is in one cell)
+  const int passes = key_bits ? sort_num_passes(key_bits) : 0;
+  for (int j = 0; j < 2; j++) {
+    CU_TRY(h, h->thin_keys[j].reserve(n));
+    CU_TRY(h, h->thin_vals[j].reserve(n));
+  }
+  CU_TRY(h, h->thin_keep.reserve(n));
+  if (passes) {
+    const size_t sb = sort_scratch_bytes(n, passes);
+    CU_TRY(h, h->thin_scratch.reserve(sb));
+    CU_TRY(h, cudaMemsetAsync(h->thin_scratch.p, 0, sb, t.st));
+  }
+  unsigned* hist = reinterpret_cast<unsigned*>(h->thin_scratch.p);
+  const int kb = blocks_for(n, kSortThreads);
+  KLAUNCH_ST(h, t.st, VGICP_PROF_OTHER,
+             k_thin_keys<<<kb < 4 * kNumSMs ? kb : 4 * kNumSMs, kSortThreads, 0, t.st>>>(t.pts.p, n, inv, make_int3(lo[0], lo[1], lo[2]), bits[0], bits[0] + bits[1], passes,
+                                                                                         h->thin_keys[0].p, hist));
+  CU_TRY(h, cudaGetLastError());
+  const unsigned long long* skeys = h->thin_keys[0].p;
+  const unsigned* svals = nullptr;
+  if (passes) {
+    int nl = 0;
+    cudaError_t se = cudaSuccess;
+    KLAUNCH_ST(h, t.st, VGICP_PROF_OTHER,
+               se = launch_sort_pairs<unsigned long long>(h->thin_keys[0].p, h->thin_vals[0].p, h->thin_keys[1].p, h->thin_vals[1].p, n, key_bits, h->thin_scratch.p, true,
+                                                          nullptr, nullptr, &nl, t.st));
+    CU_TRY(h, se);
+    h->launches += nl > 0 ? nl - 1 : 0;
+    skeys = h->thin_keys[passes & 1].p;
+    svals = h->thin_vals[passes & 1].p;
+  }
+  // 4. the keep mask; 5. the crop's compaction with it (every point passes r^2 = +inf: the coordinates are finite)
+  KLAUNCH_ST(h, t.st, VGICP_PROF_OTHER, k_thin_keep<<<blocks_for(n, 256), 256, 0, t.st>>>(skeys, svals, n, max_points_per_voxel, h->thin_keep.p));
+  CU_TRY(h, cudaGetLastError());
+  size_t kept = 0;
+  if ((rc = local_map_rank(h, h->thin_keep.p, 0.0f, 0.0f, 0.0f, std::numeric_limits<float>::infinity(), &kept))) return rc;
+  return local_map_compact(h, 0, (int)kept);
 }
 
 // ---- motion compensation: deskew the source from per-point timestamps and a constant body twist ----

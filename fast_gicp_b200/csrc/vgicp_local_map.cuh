@@ -1,7 +1,8 @@
-// vgicp_local_map.cuh -- kernels of the local-map operations (vgicp_append_source_to_target, vgicp_crop_target): the target
-// cloud grows by the registered source and is compacted by a crop, both in place on the device, so that scan-to-map odometry
-// never moves the map over PCIe.  Included after vgicp_kernels.cuh (Pose, transform_point).  The arithmetic the header
-// documents is spelled as IEEE single operations (__f*_rn): this unit is compiled with contraction on.
+// vgicp_local_map.cuh -- kernels of the local-map operations (vgicp_append_source_to_target, vgicp_thin_target,
+// vgicp_crop_target): the target cloud grows by the registered source and is compacted by a voxel cap and a crop, all in place on
+// the device, so that scan-to-map odometry never moves the map over PCIe.  Included after vgicp_kernels.cuh (Pose,
+// transform_point, vgicp_sort.cuh).  The arithmetic the header documents is spelled as IEEE single operations (__f*_rn): this
+// unit is compiled with contraction on.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -36,12 +37,13 @@ __global__ void k_append_transformed(const float4* __restrict__ src_pts, const f
   dst_covB[i] = make_float2(__fmul_rn(0.5f, __fadd_rn(N[5], N[7])), N[8]);
 }
 
-// Crop, pass 1: point i passes when d^2 = (dx dx + dy dy) + dz dz <= r2 (dx = p.x - c.x, ...); rank[i] = number of passing points
-// before i, or -1.  The total lands in *count.  Block scan, then the decoupled look-back of k_table_assign_ids over the totals
-// the preceding blocks publish in `state` (epoch << 32 | total; the epoch changes every launch, so the array never needs clearing).
-// A block only ever waits for blocks with a smaller index, which the hardware scheduled before it.
-__global__ void __launch_bounds__(kCropThreads) k_crop_rank(const float4* __restrict__ pts, int n, float cx, float cy, float cz, float r2, int* __restrict__ rank,
-                                                            int* __restrict__ count, unsigned long long* state_words, unsigned epoch) {
+// Crop, pass 1: point i passes when d^2 = (dx dx + dy dy) + dz dz <= r2 (dx = p.x - c.x, ...) and, when `keep` is given,
+// keep[i] != 0; rank[i] = number of passing points before i, or -1.  The total lands in *count.  Block scan, then the decoupled
+// look-back of k_table_assign_ids over the totals the preceding blocks publish in `state` (epoch << 32 | total; the epoch changes
+// every launch, so the array never needs clearing).  A block only ever waits for blocks with a smaller index, which the hardware
+// scheduled before it.
+__global__ void __launch_bounds__(kCropThreads) k_crop_rank(const float4* __restrict__ pts, const unsigned char* __restrict__ keep, int n, float cx, float cy, float cz,
+                                                            float r2, int* __restrict__ rank, int* __restrict__ count, unsigned long long* state_words, unsigned epoch) {
   __shared__ int warp_sums[32];
   __shared__ int s_base;
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
@@ -51,7 +53,7 @@ __global__ void __launch_bounds__(kCropThreads) k_crop_rank(const float4* __rest
     const float4 p = pts[i];
     const float dx = __fsub_rn(p.x, cx), dy = __fsub_rn(p.y, cy), dz = __fsub_rn(p.z, cz);
     const float d2 = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
-    flag = d2 <= r2 ? 1 : 0;
+    flag = d2 <= r2 && (!keep || keep[i]) ? 1 : 0;
   }
   int v = flag;
 #pragma unroll
@@ -103,6 +105,99 @@ __global__ void k_crop_scatter(const float4* __restrict__ pts, const float4* __r
   out_pts[r - first] = pts[i];
   out_covA[r - first] = covA[i];
   out_covB[r - first] = covB[i];
+}
+
+// Thinning (vgicp_thin_target): row i is kept iff fewer than M earlier rows share its cell c_a = floorf(p_a * inv).  The rows are
+// sorted stably by a u64 cell key, so the rows of one cell are contiguous and in array order; sorted position j is then kept iff
+// j < M or key[j - M] != key[j].  k_crop_rank with the resulting mask (and r2 = +inf) and k_crop_scatter compact the target.
+constexpr int kThinBoxThreads = 256;
+// box words: [0..2] ~enc(min c), [3..5] enc(max c) (unsigned max reductions, zero = empty), [6] a non-finite coordinate,
+// [7] a cell outside [-2^31, 2^31)
+constexpr int kThinBoxWords = 8;
+
+__host__ __device__ inline unsigned thin_enc(int c) { return (unsigned)c ^ 0x80000000u; }  // order-preserving int -> unsigned
+__host__ __device__ inline int thin_dec(unsigned u) { return (int)(u ^ 0x80000000u); }
+
+// 0: a coordinate is not finite, 1: cells in c, 2: a cell outside the int range
+__device__ __forceinline__ int thin_cell(float4 p, float inv, int c[3]) {
+  if (!(isfinite(p.x) && isfinite(p.y) && isfinite(p.z))) return 0;
+  const float f[3] = {floorf(__fmul_rn(p.x, inv)), floorf(__fmul_rn(p.y, inv)), floorf(__fmul_rn(p.z, inv))};
+#pragma unroll
+  for (int a = 0; a < 3; a++) {
+    if (!(f[a] >= -2147483648.0f && f[a] < 2147483648.0f)) return 2;
+    c[a] = (int)f[a];
+  }
+  return 1;
+}
+
+// one pass over the target: the cells' bounding box and the two refusal flags (st zeroed by the caller)
+__global__ void __launch_bounds__(kThinBoxThreads) k_thin_box(const float4* __restrict__ pts, int n, float inv, unsigned* __restrict__ st) {
+  __shared__ unsigned sh[kThinBoxWords];
+  if (threadIdx.x < kThinBoxWords) sh[threadIdx.x] = 0;
+  __syncthreads();
+  unsigned mx[6] = {0, 0, 0, 0, 0, 0}, nonfinite = 0, range = 0;
+  for (int i = blockIdx.x * kThinBoxThreads + threadIdx.x; i < n; i += gridDim.x * kThinBoxThreads) {
+    int c[3];
+    const int s = thin_cell(pts[i], inv, c);
+    nonfinite |= s == 0;
+    range |= s == 2;
+    if (s == 1) {
+#pragma unroll
+      for (int a = 0; a < 3; a++) {
+        mx[a] = max(mx[a], ~thin_enc(c[a]));
+        mx[3 + a] = max(mx[3 + a], thin_enc(c[a]));
+      }
+    }
+  }
+  const unsigned full = 0xffffffffu;
+#pragma unroll
+  for (int a = 0; a < 6; a++) mx[a] = __reduce_max_sync(full, mx[a]);
+  nonfinite = __reduce_or_sync(full, nonfinite);
+  range = __reduce_or_sync(full, range);
+  if ((threadIdx.x & 31) == 0) {
+#pragma unroll
+    for (int a = 0; a < 6; a++) atomicMax(&sh[a], mx[a]);
+    atomicOr(&sh[6], nonfinite);
+    atomicOr(&sh[7], range);
+  }
+  __syncthreads();
+  if (threadIdx.x < 6) atomicMax(&st[threadIdx.x], sh[threadIdx.x]);
+  else if (threadIdx.x < kThinBoxWords) atomicOr(&st[threadIdx.x], sh[threadIdx.x]);
+}
+
+// key of every point, (c_x - min_x) | (c_y - min_y) << b_x | (c_z - min_z) << (b_x + b_y), and the digit counts of all sort passes
+// (every cell is valid: the box pass refused the target otherwise).  sh_x / sh_z: the shifts of the y and z fields; a field of
+// width 0 is always 0, which also covers a shift of 64.
+__global__ void __launch_bounds__(kSortThreads) k_thin_keys(const float4* __restrict__ pts, int n, float inv, int3 lo, int sh_y, int sh_z, int passes,
+                                                            unsigned long long* __restrict__ keys, unsigned* __restrict__ hist) {
+  __shared__ unsigned sh[kSortMaxPasses * kSortBins];
+  for (int i = threadIdx.x; i < passes * kSortBins; i += kSortThreads) sh[i] = 0;
+  __syncthreads();
+  const int n_round = (n + 31) & ~31;
+  for (int i = blockIdx.x * kSortThreads + threadIdx.x; i < n_round; i += gridDim.x * kSortThreads) {  // warp-uniform trip count
+    const bool valid = i < n;
+    unsigned long long key = 0;
+    if (valid) {
+      int c[3];
+      thin_cell(pts[i], inv, c);
+      const unsigned long long dy = (unsigned)c[1] - (unsigned)lo.y, dz = (unsigned)c[2] - (unsigned)lo.z;
+      key = (unsigned long long)((unsigned)c[0] - (unsigned)lo.x) | (dy ? dy << sh_y : 0ull) | (dz ? dz << sh_z : 0ull);
+      keys[i] = key;
+    }
+    sort_hist_add(sh, passes, valid, key);
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < passes * kSortBins; i += kSortThreads)
+    if (sh[i]) atomicAdd(&hist[i], sh[i]);
+}
+
+// sorted position j is kept iff j < M or key[j - M] != key[j]; the flag goes to the point's original index (vals == nullptr: the
+// keys were not sorted, sorted position = original index)
+__global__ void k_thin_keep(const unsigned long long* __restrict__ keys, const unsigned* __restrict__ vals, int n, int M, unsigned char* __restrict__ keep) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  const bool k = j < M || keys[j - M] != keys[j];
+  keep[vals ? vals[j] : (unsigned)j] = k ? 1 : 0;
 }
 
 }  // namespace vgicp

@@ -324,11 +324,19 @@ class FastVGICPCuda(LsqRegistration):
         self.vgicp_cuda_.crop_target(center, radius, max_points)
         self.target_ = _DeviceMap()
 
+    def thinTarget(self, leaf_size, max_points_per_voxel):
+        """Keep at most max_points_per_voxel target points per cell of a leaf_size grid, the oldest (call after an append)."""
+        self.vgicp_cuda_.thin_target(leaf_size, max_points_per_voxel)
+        self.target_ = _DeviceMap()
+
     def append_source_to_target(self, T):
         self.appendSourceToTarget(T)
 
     def crop_target(self, center, radius, max_points=0):
         self.cropTarget(center, radius, max_points)
+
+    def thin_target(self, leaf_size, max_points_per_voxel):
+        self.thinTarget(leaf_size, max_points_per_voxel)
 
     # -- motion compensation (an extension).  Afterwards the source on the device is no longer the cloud given to setInputSource:
     # input_ becomes a copy of it (its points stay for align's output), so setInputSource(that cloud) reloads the raw cloud.

@@ -139,6 +139,21 @@ def voxel_downsample_values(pts, values, leaf):
     return (sums / counts[:, None]).astype(np.float32), (vsums / counts).astype(np.float32)
 
 
+def thin_indices(pts, leaf, M):
+    """Rows vgicp_thin_target keeps, ascending: row i is kept iff fewer than M earlier rows share its cell, with the header's
+    cells c = floor(p * (1 / (float)leaf)) in float32 (one multiplication per axis)."""
+    p = np.asarray(pts, dtype=np.float32).reshape(-1, 3)
+    inv = np.float32(1.0) / np.float32(leaf)
+    cells = np.floor(p * inv).astype(np.int64)
+    _, group = np.unique(cells, axis=0, return_inverse=True)
+    group = group.reshape(-1)
+    order = np.argsort(group, kind="stable")  # rows of one cell contiguous, in array order
+    g = group[order]
+    starts = np.flatnonzero(np.r_[True, g[1:] != g[:-1]])
+    rank = np.arange(len(g)) - np.repeat(starts, np.diff(np.r_[starts, len(g)]))  # earlier rows of the same cell
+    return np.sort(order[rank < M])
+
+
 def kitti_like_pair(beams=64, az_steps=2083, seed=42, pose=(0.8, 0.05, 0.7), downsample=0.25, max_points=None):
     """(target, source, T_gt): target scanned at the origin, source from a sensor moved by pose=(tx, ty, yaw_deg).
     T_gt maps source-frame points into the target frame (what registration should recover)."""

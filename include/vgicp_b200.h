@@ -217,14 +217,15 @@ VGICP_API int vgicp_register(vgicp_handle h, const float* target_xyz, size_t n_t
 enum { VGICP_ROBUST_NONE = 0, VGICP_ROBUST_HUBER = 1, VGICP_ROBUST_CAUCHY = 2, VGICP_ROBUST_GEMAN_MCCLURE = 3 };
 VGICP_API int vgicp_set_robust_kernel(vgicp_handle h, int kind, double scale);
 /* ---- local map for scan-to-map odometry (not in the reference) -------------------------------------------------------------
- * Each frame: register the new scan against the map (vgicp_align), append it at the pose found, crop what is too far or too old.
- * Both calls work on the device arrays in place (no PCIe traffic for the map) and leave the state that set_target_cloud +
- * set_target_covariances + create_target_voxelmap with the resulting arrays would leave: the target has covariances, no
- * neighbour rows (vgicp_get_target_neighbors returns VGICP_ERR_BAD_STATE; find_target_neighbors + calculate_target_covariances
- * recompute k-NN covariances of the merged map if wanted), and the voxel map is rebuilt over the whole target at the resolution it
- * was first created with.  Handle settings (robust kernel, neighbour search, ...) are kept.  Neither is available with an NDT
- * problem selected or with stage-1 sharding (VGICP_ERR_UNSUPPORTED); source sharding is unaffected (every rank makes the same
- * deterministic change).  Every error below is returned before anything is modified, and all but the empty crop before any launch.
+ * Each frame: register the new scan against the map (vgicp_align), append it at the pose found, thin the cells that hold too
+ * many points, crop what is too far or too old.  These calls work on the device arrays in place (no PCIe traffic for the map) and
+ * leave the state that set_target_cloud + set_target_covariances + create_target_voxelmap with the resulting arrays would leave:
+ * the target has covariances, no neighbour rows (vgicp_get_target_neighbors returns VGICP_ERR_BAD_STATE; find_target_neighbors +
+ * calculate_target_covariances recompute k-NN covariances of the merged map if wanted), and the voxel map is rebuilt over the
+ * whole target at the resolution it was first created with.  Handle settings (robust kernel, neighbour search, ...) are kept.
+ * None is available with an NDT problem selected or with stage-1 sharding (VGICP_ERR_UNSUPPORTED); source sharding is unaffected
+ * (every rank makes the same deterministic change).  Every error below is returned before anything is modified, and all but the
+ * empty crop and the thinning's checks of the points before any launch.
  *
  * vgicp_append_source_to_target: the target grows from n_t to n_t + n_s points; rows n_t .. n_t + n_s - 1 hold the current source
  * transformed by T (column-major 4x4, cast to float like every pose):
@@ -246,6 +247,20 @@ VGICP_API int vgicp_append_source_to_target(vgicp_handle h, const double T[16]);
  * Errors: VGICP_ERR_INVALID_ARGUMENT (null center, NaN or negative radius, a crop that would leave no points: target and map are
  * then left exactly as they were), VGICP_ERR_BAD_STATE (target without points or covariances). */
 VGICP_API int vgicp_crop_target(vgicp_handle h, const double center[3], double radius, size_t max_points);
+/* vgicp_thin_target: keep at most M = max_points_per_voxel points per cell of a grid of leaf_size, the oldest; rebuild the map.
+ *   cells   l = (float)leaf_size, inv = 1.0f / l; per axis c_a = floorf(p_a * inv) (one IEEE single multiplication).
+ *   rule    target row i is kept iff fewer than M earlier rows (in array order) share its cell.  Appends go to the end, so a new
+ *           scan only fills the cells that still have room, and a vehicle that stands still adds nothing to full cells.
+ * Kept points and their covariances are unchanged and stay in their original order (a stable subsequence of the rows).  The state
+ * afterwards is the one described above, also when nothing is dropped.  Two host synchronisations (the cells' box, the new size).
+ * Per frame: vgicp_align, vgicp_append_source_to_target, vgicp_thin_target, then vgicp_crop_target (radius, optional cap).
+ * Errors, all returned before anything is modified (target and map stay exactly as they were):
+ *   VGICP_ERR_INVALID_ARGUMENT  leaf_size not finite and > 0, l or inv not finite and > 0, M < 1; found by the first pass over
+ *                               the points: a non-finite target coordinate, a cell outside [-2^31, 2^31), or a cell box too wide
+ *                               for a 64-bit key (sum over the axes of bits(max c_a - min c_a) > 64);
+ *   VGICP_ERR_BAD_STATE         target without points or covariances;
+ *   VGICP_ERR_UNSUPPORTED       an NDT problem selected, or stage-1 sharding. */
+VGICP_API int vgicp_thin_target(vgicp_handle h, double leaf_size, int max_points_per_voxel);
 /* ---- motion compensation (not in the reference) ---------------------------------------------------------------------------
  * A spinning or solid-state LiDAR fires the points of one sweep over its period while the vehicle moves; each point is in the
  * sensor frame of its own firing time.  vgicp_deskew_source re-expresses every source point in the sensor frame at t_ref under a
