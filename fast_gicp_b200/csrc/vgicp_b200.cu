@@ -380,16 +380,116 @@ Pose to_pose(const double* T) {  // Eigen::Isometry3d (column-major) -> float im
   return p;
 }
 
-int set_cloud(vgicp_handle h, Cloud& c, const float* xyz, size_t n, size_t stride, bool on_device = false) {
-  // NDT: set_{source,target}_cloud resets that cloud's voxel map only (ndt_cuda.cu:104,114); it is rebuilt by the next create_voxelmaps.
-  // (The multi-source pool's cloud belongs to neither.)
-  if (&c == &h->source || &c == &h->target) {
-    h->ndt_ready = false;
-    VoxelMap& nm = (&c == &h->target) ? h->ndt_t : h->ndt_s;
-    nm.built = false;
-    nm.pending = false;
+// ---- handle state: what a change to an input invalidates ----------------------------------------------------------------------
+// These flags are written here and by the functions that produce what they describe (find_neighbors, calc_covariances*,
+// set_covariances, voxelmap_begin / voxelmap_finish, ndt_prepare), nowhere else; nothing here calls the CUDA API.  "Order" is the
+// k-NN order: knn_sorted with its query range.  Two asymmetries are deliberate: computed target covariances keep the VGICP map
+// while uploaded ones drop it (vgicp_set_target_covariances), and a deskew keeps the timestamps (the same points, moved).
+
+void drop_map(VoxelMap& m) { m.built = m.pending = false; }
+
+// drops the cloud's rows, order and NDT map and ndt_ready, and by kind of change:
+enum class Change {
+  replaced,  // set_*_cloud(_device), vgicp_register, the multi-source pool: also the covariances, the source's timestamps, the VGICP map
+  moved,     // deskew: also the covariances
+  edited,    // append / crop / thin: rows added or removed with their covariances; the caller begins the VGICP map build
+};
+void points_changed(vgicp_handle h, Cloud& c, Change what) {
+  c.k = 0;
+  c.knn_sorted = nullptr;
+  c.knn_q_begin = c.knn_q_end = 0;
+  if (what != Change::edited) c.has_cov = false;
+  if (&c != &h->source && &c != &h->target) return;  // the multi-source pool's cloud belongs to no map
+  h->ndt_ready = false;
+  drop_map(&c == &h->target ? h->ndt_t : h->ndt_s);  // NDT: that cloud's map only (ndt_cuda.cu:104,114)
+  if (what == Change::replaced && &c == &h->source) h->ct_has_times = false;  // the timestamps belong to the points they came with
+  if (what == Change::replaced && &c == &h->target) drop_map(h->map);
+}
+
+// find_neighbors, the stage-1 replay; set_neighbors without an order: host rows follow none, so calc_covariances runs unsharded
+void neighbors_set(Cloud& c, int k, const float4* order = nullptr, int q_begin = 0, int q_end = 0) {
+  c.k = k;
+  c.knn_sorted = order;
+  c.knn_q_begin = q_begin;
+  c.knn_q_end = q_end;
+}
+void covariances_set(Cloud& c) { c.has_cov = true; }
+void map_begun(VoxelMap& m) { m.built = false; m.pending = true; }
+
+void covariances_dropped(vgicp_handle h) {
+  h->target.has_cov = h->source.has_cov = false;
+  drop_map(h->map);
+}
+
+// with both streams idle: the reference swaps its NDT maps (ndt_cuda.cu:90-93); a pending build was enqueued on the other stream
+void clouds_swapped(vgicp_handle h) {
+  std::swap(h->source, h->target);
+  h->ct_has_times = false;
+  drop_map(h->map);
+  for (VoxelMap* vm : {&h->ndt_t, &h->ndt_s})
+    if (vm->pending) drop_map(*vm);
+  std::swap(h->ndt_t, h->ndt_s);
+  h->ndt_ready = false;
+}
+
+void problem_set(vgicp_handle h, int problem) {
+  if (problem != h->problem) h->ndt_ready = h->has_lin = false;
+  h->problem = problem;
+}
+void lin_set(vgicp_handle h, const Pose& T) {
+  h->lin = T;
+  h->has_lin = true;
+}
+
+// Both timestamp setters: refused unless every t_i - tau is finite as the kernels form it (a float subtraction is monotonic in t_i, so
+// S = max |t_i - tau| is reached at lo or hi); then install() puts the values in ct_times
+template <class F>
+int timestamps_commit(vgicp_handle h, const char* who, float lo, float hi, double t_ref, F&& install) {
+  const float tau = (float)t_ref;
+  const double span = fmax(fabs((double)(lo - tau)), fabs((double)(hi - tau)));
+  if (!std::isfinite(span)) return fail(h, VGICP_ERR_INVALID_ARGUMENT, std::string(who) + ": t_i - t_ref overflows a float");
+  if (int rc = install()) return rc;
+  h->ct_has_times = true;
+  h->ct_tau = tau;
+  h->ct_span = span;
+  h->ct_lo = lo;
+  h->ct_hi = hi;
+  h->ct_t_ref = t_ref;
+  return VGICP_OK;
+}
+
+// What an entry point needs before it launches anything.  The conditions are tested in this order, and the first one that does
+// not hold is the error: a robust kind with NDT (kNeedEval) or continuous time with NDT (kNeedCt); a multi-GPU communicator
+// (kNeedOneGpu) or any sharding (kNeedCt); the clouds (VGICP: source points, their covariances with kNeedEval, the voxel map; NDT:
+// source and target points); the linearisation point (kNeedLin); the source's timestamps (kNeedCt).
+enum : unsigned {
+  kNeedEval = 1,    // evaluates residuals: a robust kind must fit the problem (NDT has its own Cauchy weight), covariances (VGICP)
+  kNeedLin = 2,     // the correspondences of vgicp_update_correspondences
+  kNeedOneGpu = 4,  // not in a multi-GPU communicator
+  kNeedCt = 8,      // continuous time: VGICP on one GPU without sharding, with the source's timestamps
+};
+int check_ready(vgicp_handle h, const char* who, unsigned need) {
+  const std::string w(who);
+  if ((need & kNeedCt) && h->problem != 0) return fail(h, VGICP_ERR_UNSUPPORTED, w + ": continuous-time registration is defined for the VGICP problem only");
+  if ((need & kNeedEval) && h->problem != 0 && h->robust_kind != VGICP_ROBUST_NONE)
+    return fail(h, VGICP_ERR_UNSUPPORTED, w + ": a robust kernel is set (vgicp_set_robust_kernel) and an NDT problem is selected; NDT has its own weight");
+  if ((need & kNeedOneGpu) && h->comm_ranks > 1) return fail(h, VGICP_ERR_UNSUPPORTED, w + ": not available on a handle in a multi-GPU communicator");
+  if ((need & kNeedCt) && (h->comm_ranks > 1 || h->stage1_sharding || h->shard_end >= 0))
+    return fail(h, VGICP_ERR_UNSUPPORTED, w + ": not available with source or stage-1 sharding or in a multi-GPU communicator");
+  if (h->problem != 0) {
+    if (!h->source.has_pts || !h->target.has_pts) return fail(h, VGICP_ERR_BAD_STATE, w + ": NDT needs source and target clouds");
+  } else {
+    if (!h->source.has_pts) return fail(h, VGICP_ERR_BAD_STATE, w + ": source cloud not set");
+    if ((need & kNeedEval) && !h->source.has_cov) return fail(h, VGICP_ERR_BAD_STATE, w + ": source covariances required");
+    if (!h->map.built && !h->map.pending) return fail(h, VGICP_ERR_BAD_STATE, w + ": target voxel map not built");
   }
-  if (&c == &h->source) h->ct_has_times = false;  // the timestamps belong to the points they came with
+  if ((need & kNeedLin) && !h->has_lin) return fail(h, VGICP_ERR_BAD_STATE, w + ": update_correspondences has not been called");
+  if ((need & kNeedCt) && !h->ct_has_times) return fail(h, VGICP_ERR_BAD_STATE, w + ": the source has no timestamps (vgicp_set_source_timestamps)");
+  return VGICP_OK;
+}
+
+int set_cloud(vgicp_handle h, Cloud& c, const float* xyz, size_t n, size_t stride, bool on_device = false) {
+  points_changed(h, c, Change::replaced);
   if (n > 0 && !xyz) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "set_cloud: null points");
   if (stride < 12 || (stride % 4) != 0) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "set_cloud: stride_bytes must be a multiple of 4 and >= 12");
   if (n > (size_t)0x7fffffff / 64) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "set_cloud: too many points");
@@ -428,11 +528,8 @@ int set_neighbors(vgicp_handle h, Cloud& c, int k, const int* idx, size_t nk) {
   CU_TRY(h, cudaGetLastError());
   CU_TRY(h, cudaMemcpyAsync(h->map.h_counters + 8, bad, sizeof(int), cudaMemcpyDeviceToHost, c.st));
   CU_TRY(h, cudaStreamSynchronize(c.st));
-  if (h->map.h_counters[8] != 0) {
-    c.k = 0;
-    return fail(h, VGICP_ERR_INVALID_ARGUMENT, "set_neighbors: neighbour index outside [0, num_points)");
-  }
-  c.k = k;
+  neighbors_set(c, h->map.h_counters[8] != 0 ? 0 : k);
+  if (c.k == 0) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "set_neighbors: neighbour index outside [0, num_points)");
   return VGICP_OK;
 }
 
@@ -441,20 +538,20 @@ int find_neighbors(vgicp_handle h, Cloud& c, int k) {
   if (k <= 0 || k > kMaxK || k > c.n) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "find_neighbors: need 1 <= k <= min(num_points, 64)");
   CU_TRY(h, c.nbr.reserve((size_t)c.n * k));
   CU_TRY(h, c.knn_scratch.reserve(knn_grid_scratch_bytes(c.n, nullptr, nullptr)));
-  c.knn_q_begin = 0;
-  c.knn_q_end = c.n;
+  int q_begin = 0, q_end = c.n;
   if (h->stage1_sharding && h->comm_ranks > 1 && h->arena_peers[h->comm_rank]) {  // this rank's slice of the queries (sorted positions)
     const long long base = c.n / h->comm_ranks, rem = c.n % h->comm_ranks, r = h->comm_rank;
-    c.knn_q_begin = (int)(r * base + (r < rem ? r : rem));
-    c.knn_q_end = c.knn_q_begin + (int)base + (r < rem ? 1 : 0);
+    q_begin = (int)(r * base + (r < rem ? r : rem));
+    q_end = q_begin + (int)base + (r < rem ? 1 : 0);
   }
   cudaError_t ke = cudaSuccess;
   int nl = 0;
-  KLAUNCH_ST(h, c.st, VGICP_PROF_KNN, ke = launch_knn_grid(c.pts.p, c.n, k, c.nbr.p, c.knn_scratch.p, c.knn_scratch.cap, c.knn_q_begin, c.knn_q_end, &nl, &c.knn_sorted, c.st));
+  const float4* sorted = nullptr;
+  KLAUNCH_ST(h, c.st, VGICP_PROF_KNN, ke = launch_knn_grid(c.pts.p, c.n, k, c.nbr.p, c.knn_scratch.p, c.knn_scratch.cap, q_begin, q_end, &nl, &sorted, c.st));
   h->launches += nl > 0 ? nl - 1 : 0;
   CU_TRY(h, ke);
   CU_TRY(h, cudaEventRecord(c.ready, c.st));
-  c.k = k;
+  neighbors_set(c, k, sorted, q_begin, q_end);
   return VGICP_OK;
 }
 
@@ -488,7 +585,7 @@ int calc_covariances(vgicp_handle h, Cloud& c, int method) {
     KLAUNCH_ST(h, c.st, VGICP_PROF_COVARIANCE, ke = launch_covariance_knn(c.pts.p, c.nbr.p, c.n, c.k, method, c.covA.p, c.covB.p, c.st));
     CU_TRY(h, ke);
   }
-  c.has_cov = true;
+  covariances_set(c);
   CU_TRY(h, cudaEventRecord(c.ready, c.st));
   if (method == VGICP_REG_NORMALIZED_MIN_EIG)
     return fail(h, VGICP_ERR_UNSUPPORTED, "unimplemented covariance regularization method was selected (NORMALIZED_MIN_EIG has no GPU path in the reference either); raw covariances kept");
@@ -509,7 +606,7 @@ int calc_covariances_rbf(vgicp_handle h, Cloud& c, int method) {
     h->launches++;
     CU_TRY(h, ke);
   }
-  c.has_cov = true;
+  covariances_set(c);
   CU_TRY(h, cudaEventRecord(c.ready, c.st));
   if (method == VGICP_REG_NORMALIZED_MIN_EIG) return fail(h, VGICP_ERR_UNSUPPORTED, "unimplemented covariance regularization method was selected; raw covariances kept");
   return VGICP_OK;
@@ -551,7 +648,7 @@ int set_covariances(vgicp_handle h, Cloud& c, const float* in9, size_t n) {
     CU_TRY(h, cudaMemcpyAsync(c.covB.p, b.data(), sizeof(float2) * c.n, cudaMemcpyHostToDevice, c.st));
     CU_TRY(h, cudaStreamSynchronize(c.st));
   }
-  c.has_cov = true;
+  covariances_set(c);
   CU_TRY(h, cudaEventRecord(c.ready, c.st));
   return VGICP_OK;
 }
@@ -606,8 +703,7 @@ int voxelmap_begin(vgicp_handle h, Cloud& t, VoxelMap& m) {
     m.created = true;
     m.res = (float)h->resolution;
   }
-  m.built = false;
-  m.pending = false;
+  drop_map(m);
   const int n = t.n;
   CU_TRY(h, m.coords.reserve(n));
   CU_TRY(h, m.slot_of_point.reserve(n));
@@ -618,7 +714,7 @@ int voxelmap_begin(vgicp_handle h, Cloud& t, VoxelMap& m) {
   // small clouds pass with the initial 8192 buckets (1082 voxels at 17 k points); large ones are given three sizes to try at once
   int rc = voxelmap_attempt(h, t, m, m.init_num_buckets, n > 200000 ? 3 : 1);
   if (rc) return rc;
-  m.pending = true;
+  map_begun(m);
   return VGICP_OK;
 }
 
@@ -856,36 +952,6 @@ int launch_linearize(vgicp_handle h, const Pose& Teval, int kind) {
       k_linearize<decltype(mode)::value, WHAT, decltype(g)::value, RB><<<L.grid, kLinThreads, 0, h->stream>>>(a);
     });
   });
-}
-
-// What an entry point needs before it launches anything.  The conditions are tested in this order, and the first one that does
-// not hold is the error: a robust kind with NDT (kNeedEval) or continuous time with NDT (kNeedCt); a multi-GPU communicator
-// (kNeedOneGpu) or any sharding (kNeedCt); the clouds (VGICP: source points, their covariances with kNeedEval, the voxel map; NDT:
-// source and target points); the linearisation point (kNeedLin); the source's timestamps (kNeedCt).
-enum : unsigned {
-  kNeedEval = 1,    // evaluates residuals: a robust kind must fit the problem (NDT has its own Cauchy weight), covariances (VGICP)
-  kNeedLin = 2,     // the correspondences of vgicp_update_correspondences
-  kNeedOneGpu = 4,  // not in a multi-GPU communicator
-  kNeedCt = 8,      // continuous time: VGICP on one GPU without sharding, with the source's timestamps
-};
-int check_ready(vgicp_handle h, const char* who, unsigned need) {
-  const std::string w(who);
-  if ((need & kNeedCt) && h->problem != 0) return fail(h, VGICP_ERR_UNSUPPORTED, w + ": continuous-time registration is defined for the VGICP problem only");
-  if ((need & kNeedEval) && h->problem != 0 && h->robust_kind != VGICP_ROBUST_NONE)
-    return fail(h, VGICP_ERR_UNSUPPORTED, w + ": a robust kernel is set (vgicp_set_robust_kernel) and an NDT problem is selected; NDT has its own weight");
-  if ((need & kNeedOneGpu) && h->comm_ranks > 1) return fail(h, VGICP_ERR_UNSUPPORTED, w + ": not available on a handle in a multi-GPU communicator");
-  if ((need & kNeedCt) && (h->comm_ranks > 1 || h->stage1_sharding || h->shard_end >= 0))
-    return fail(h, VGICP_ERR_UNSUPPORTED, w + ": not available with source or stage-1 sharding or in a multi-GPU communicator");
-  if (h->problem != 0) {
-    if (!h->source.has_pts || !h->target.has_pts) return fail(h, VGICP_ERR_BAD_STATE, w + ": NDT needs source and target clouds");
-  } else {
-    if (!h->source.has_pts) return fail(h, VGICP_ERR_BAD_STATE, w + ": source cloud not set");
-    if ((need & kNeedEval) && !h->source.has_cov) return fail(h, VGICP_ERR_BAD_STATE, w + ": source covariances required");
-    if (!h->map.built && !h->map.pending) return fail(h, VGICP_ERR_BAD_STATE, w + ": target voxel map not built");
-  }
-  if ((need & kNeedLin) && !h->has_lin) return fail(h, VGICP_ERR_BAD_STATE, w + ": update_correspondences has not been called");
-  if ((need & kNeedCt) && !h->ct_has_times) return fail(h, VGICP_ERR_BAD_STATE, w + ": the source has no timestamps (vgicp_set_source_timestamps)");
-  return VGICP_OK;
 }
 
 // builds what an NDT evaluation needs (idempotent): target map, and for D2D the source map + its Gaussians as a cloud
@@ -1473,18 +1539,12 @@ int vgicp_set_neighbor_search_method(vgicp_handle h, int method, double radius) 
 int vgicp_set_source_cloud(vgicp_handle h, const float* xyz, size_t n, size_t stride_bytes) {
   CHECK_HANDLE(h);
   DeviceGuard g(h->device);
-  h->source.k = 0;  // the reference keeps stale neighbours/covariances; every caller recomputes them right after
-  h->source.has_cov = false;
   return set_cloud(h, h->source, xyz, n, stride_bytes);
 }
 
 int vgicp_set_target_cloud(vgicp_handle h, const float* xyz, size_t n, size_t stride_bytes) {
   CHECK_HANDLE(h);
   DeviceGuard g(h->device);
-  h->target.k = 0;
-  h->target.has_cov = false;
-  h->map.built = false;
-  h->map.pending = false;
   return set_cloud(h, h->target, xyz, n, stride_bytes);
 }
 
@@ -1497,16 +1557,7 @@ int vgicp_swap_source_and_target(vgicp_handle h) {  // fast_vgicp_cuda.cu:97-107
   if (h->map.pending) { int rc0 = voxelmap_finish(h, h->target, h->map); if (rc0) return rc0; }
   CU_TRY(h, cudaStreamSynchronize(h->stream));
   CU_TRY(h, cudaStreamSynchronize(h->stream_b));
-  std::swap(h->source, h->target);
-  h->ct_has_times = false;
-  h->map.built = false;
-  h->map.pending = false;
-  // NDT: the reference swaps its two maps (ndt_cuda.cu:90-93); a map that does not exist (P2D never builds the source's) is built by
-  // the next create_voxelmaps.  Pending builds were enqueued on the old streams: both streams are idle here.
-  for (VoxelMap* vm : {&h->ndt_t, &h->ndt_s})
-    if (vm->pending) { vm->pending = false; vm->built = false; }
-  std::swap(h->ndt_t, h->ndt_s);
-  h->ndt_ready = false;
+  clouds_swapped(h);
   if (h->problem != 0) return VGICP_OK;
   if (!h->target.has_pts || !h->target.has_cov) return VGICP_OK;
   return build_voxelmap(h);
@@ -1560,8 +1611,7 @@ int vgicp_set_source_covariances(vgicp_handle h, const float* in9, size_t n) {
 int vgicp_set_target_covariances(vgicp_handle h, const float* in9, size_t n) {
   CHECK_HANDLE(h);
   DeviceGuard g(h->device);
-  h->map.built = false;  // the voxel Gaussians average the target covariances: the map must be rebuilt (create_target_voxelmap)
-  h->map.pending = false;
+  drop_map(h->map);  // the voxel Gaussians average the target covariances: the map must be rebuilt (create_target_voxelmap)
   return set_covariances(h, h->target, in9, n);
 }
 int vgicp_get_source_covariances(vgicp_handle h, float* out9, size_t cap) {
@@ -1692,8 +1742,7 @@ int vgicp_update_correspondences(vgicp_handle h, const double T[16]) {  // fast_
   CHECK_HANDLE(h);
   if (!T) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "update_correspondences: null pose");
   if (int rc = check_ready(h, "update_correspondences", 0)) return rc;
-  h->lin = to_pose(T);  // linearized_x = trans.cast<float>()
-  h->has_lin = true;
+  lin_set(h, to_pose(T));  // linearized_x = trans.cast<float>()
   // the lookup itself is fused into the evaluation kernel; the explicit list is only built by the getter
   return VGICP_OK;
 }
@@ -1771,8 +1820,7 @@ int vgicp_align(vgicp_handle h, const double guess[16], const vgicp_lsq_params* 
     const bool lin = st.phase == kLmLinearize;
     const Pose Teval = to_pose(lin ? st.x0.m : st.xi.m);
     if (lin) {  // linearized_x: the correspondences of this evaluation and of the trials from it
-      h->lin = Teval;
-      h->has_lin = true;
+      lin_set(h, Teval);
     }
     const double* rec = nullptr;
     int rc = evaluate(h, Teval, lin ? kEvalLinearize : (speculate ? kEvalSpec : kEvalError), &rec);
@@ -1922,8 +1970,6 @@ int vgicp_align_sources(vgicp_handle h, const float* const* xyz, const size_t* n
     c.pts.attach(h->src_pts.p + off[i], cap);
     c.covA.attach(h->src_covA.p + off[i], cap);
     c.covB.attach(h->src_covB.p + off[i], cap);
-    c.k = 0;
-    c.has_cov = false;
     if ((rc = set_cloud(h, c, xyz[i], n[i], stride_bytes, on_device != 0))) return rc;
     if ((rc = find_neighbors(h, c, k))) return rc;
     rc = calc_covariances(h, c, regularization_method);
@@ -2050,14 +2096,10 @@ static int stage1_resident(vgicp_handle h, int k, int reg) {
     // the host state the enqueue code leaves behind, as it left it when the graph was captured
     Cloud* cl[2] = {&h->target, &h->source};
     for (int j = 0; j < 2; j++) {
-      cl[j]->knn_sorted = G.sorted[j];
-      cl[j]->knn_q_begin = 0;
-      cl[j]->knn_q_end = cl[j]->n;
-      cl[j]->k = k;
-      cl[j]->has_cov = true;
+      neighbors_set(*cl[j], k, G.sorted[j], 0, cl[j]->n);
+      covariances_set(*cl[j]);
     }
-    h->map.built = false;
-    h->map.pending = true;
+    map_begun(h->map);
     h->map.pending_B = G.pending_B;
     h->launches += G.launches;
     for (int i = 0; i < VGICP_PROF_NUM_CATEGORIES; i++) h->prof_launches[i] += G.prof_launches[i];
@@ -2113,9 +2155,7 @@ int vgicp_register(vgicp_handle h, const float* target_xyz, size_t n_target, con
   CHECK_HANDLE(h);
   DeviceGuard g(h->device);
   int rc;
-  h->target.k = 0; h->target.has_cov = false; h->map.built = false; h->map.pending = false;
   if ((rc = set_cloud(h, h->target, target_xyz, n_target, stride_bytes, on_device != 0))) return rc;
-  h->source.k = 0; h->source.has_cov = false;
   if ((rc = set_cloud(h, h->source, source_xyz, n_source, stride_bytes, on_device != 0))) return rc;
   // resident clouds on the plain path: stage 1 through the graph (one launch once it is captured)
   const bool graph = on_device && n_target > 0 && n_source > 0 && stage1_graph_eligible(h, regularization_method);
@@ -2146,18 +2186,12 @@ int vgicp_transform_source(vgicp_handle h, const double T[16], float* out_xyz, s
 int vgicp_set_source_cloud_device(vgicp_handle h, const float* d_xyz, size_t n, size_t stride_bytes) {
   CHECK_HANDLE(h);
   DeviceGuard g(h->device);
-  h->source.k = 0;
-  h->source.has_cov = false;
   return set_cloud(h, h->source, d_xyz, n, stride_bytes, true);
 }
 
 int vgicp_set_target_cloud_device(vgicp_handle h, const float* d_xyz, size_t n, size_t stride_bytes) {
   CHECK_HANDLE(h);
   DeviceGuard g(h->device);
-  h->target.k = 0;
-  h->target.has_cov = false;
-  h->map.built = false;
-  h->map.pending = false;
   return set_cloud(h, h->target, d_xyz, n, stride_bytes, true);
 }
 
@@ -2174,13 +2208,7 @@ static int local_map_check(vgicp_handle h, const char* who) {
 // create_target_voxelmap would leave (covariances, no neighbour rows, the map build enqueued at the map's first resolution)
 static int local_map_rebuild(vgicp_handle h) {
   Cloud& t = h->target;
-  t.k = 0;
-  t.knn_sorted = nullptr;
-  t.knn_q_begin = t.knn_q_end = 0;
-  t.has_cov = true;
-  h->ndt_ready = false;
-  h->ndt_t.built = false;
-  h->ndt_t.pending = false;
+  points_changed(h, t, Change::edited);
   int rc = voxelmap_begin(h, t, h->map);
   if (rc) return rc;
   CU_TRY(h, cudaEventRecord(t.ready, t.st));
@@ -2382,48 +2410,55 @@ static int timestamps_pack(vgicp_handle h, const char* who, const float* t, size
   return VGICP_OK;
 }
 
-int vgicp_deskew_source(vgicp_handle h, const float* t, size_t n, size_t stride_bytes, const double twist[6], double t_ref) {
-  CHECK_HANDLE(h);
-  DeviceGuard g(h->device);
-  if (n > 0 && (!t || !twist)) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "deskew_source: null timestamps or twist");
-  int rc = timestamps_check(h, "deskew_source", n, stride_bytes, t_ref);
-  if (rc) return rc;
+// the twist as the kernel takes it (float) must be finite; checked before the timestamps are read
+static int deskew_twist_check(vgicp_handle h, const char* who, const double twist[6]) {
+  for (int j = 0; j < 6; j++)
+    if (!std::isfinite((float)twist[j])) return fail(h, VGICP_ERR_INVALID_ARGUMENT, std::string(who) + ": non-finite twist");
+  return VGICP_OK;
+}
+
+// Both deskews: the series bound in double against t_ref, then k_deskew_points over the source on its stream with the timestamps
+// d_t (device memory, one float per point), ordered after the main stream's reads of the source points and after an append
+static int deskew_enqueue(vgicp_handle h, const char* who, const float* d_t, const double twist[6], float lo, float hi, double t_ref) {
   Cloud& s = h->source;
-  const float tau = (float)t_ref;
   float xi[6];
   for (int j = 0; j < 6; j++) xi[j] = (float)twist[j];
-  for (int j = 0; j < 6; j++)
-    if (!std::isfinite(xi[j])) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "deskew_source: non-finite twist");
-  std::vector<float>& packed = h->deskew_times;
-  float lo = 0.0f, hi = 0.0f;
-  if ((rc = timestamps_pack(h, "deskew_source", t, n, stride_bytes, packed, &lo, &hi))) return rc;
   const double span = fmax(fabs((double)lo - t_ref), fabs((double)hi - t_ref));
   const double omega = sqrt(twist[0] * twist[0] + twist[1] * twist[1] + twist[2] * twist[2]);
   if (omega * span > 1.5707963267948966)
-    return fail(h, VGICP_ERR_INVALID_ARGUMENT, "deskew_source: the rotation over the sweep exceeds pi/2 (|omega| * max |t_i - t_ref|), beyond the series");
-  // the kernel overwrites the source points: it must not overtake the evaluations on the main stream, nor an append that reads them
+    return fail(h, VGICP_ERR_INVALID_ARGUMENT, std::string(who) + ": the rotation over the sweep exceeds pi/2 (|omega| * max |t_i - t_ref|), beyond the series");
   if (s.st != h->stream) {
     if (!h->ev_deskew) CU_TRY(h, cudaEventCreateWithFlags(&h->ev_deskew, cudaEventDisableTiming));
     CU_TRY(h, cudaEventRecord(h->ev_deskew, h->stream));
     CU_TRY(h, cudaStreamWaitEvent(s.st, h->ev_deskew, 0));
   }
   if (s.st != h->target.st) CU_TRY(h, cudaStreamWaitEvent(s.st, h->ev_append, 0));
+  KLAUNCH_ST(h, s.st, VGICP_PROF_OTHER,
+             k_deskew_points<<<blocks_for(s.n, 256), 256, 0, s.st>>>(s.pts.p, d_t, s.n, (float)t_ref, xi[0], xi[1], xi[2], xi[3], xi[4], xi[5]));
+  CU_TRY(h, cudaGetLastError());
+  CU_TRY(h, cudaEventRecord(s.ready, s.st));
+  points_changed(h, s, Change::moved);
+  return VGICP_OK;
+}
+
+int vgicp_deskew_source(vgicp_handle h, const float* t, size_t n, size_t stride_bytes, const double twist[6], double t_ref) {
+  CHECK_HANDLE(h);
+  DeviceGuard g(h->device);
+  if (n > 0 && (!t || !twist)) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "deskew_source: null timestamps or twist");
+  int rc = timestamps_check(h, "deskew_source", n, stride_bytes, t_ref);
+  if (rc) return rc;
+  if ((rc = deskew_twist_check(h, "deskew_source", twist))) return rc;
+  std::vector<float>& packed = h->deskew_times;
+  float lo = 0.0f, hi = 0.0f;
+  if ((rc = timestamps_pack(h, "deskew_source", t, n, stride_bytes, packed, &lo, &hi))) return rc;
+  Cloud& s = h->source;
   CU_TRY(h, s.staging.reserve(n * sizeof(float)));
   CU_TRY(h, cudaMemcpyAsync(s.staging.p, packed.data(), n * sizeof(float), cudaMemcpyHostToDevice, s.st));
   CU_TRY(h, cudaEventRecord(h->ev_copy, s.st));
-  KLAUNCH_ST(h, s.st, VGICP_PROF_OTHER,
-             k_deskew_points<<<blocks_for(n, 256), 256, 0, s.st>>>(s.pts.p, reinterpret_cast<const float*>(s.staging.p), (int)n, tau, xi[0], xi[1], xi[2], xi[3], xi[4], xi[5]));
-  CU_TRY(h, cudaGetLastError());
-  CU_TRY(h, cudaEventRecord(s.ready, s.st));
-  // the state set_source_cloud leaves: no neighbour rows, no covariances, the NDT source map reset
-  s.k = 0;
-  s.has_cov = false;
-  h->ndt_ready = false;
-  h->ndt_s.built = false;
-  h->ndt_s.pending = false;
+  rc = deskew_enqueue(h, "deskew_source", reinterpret_cast<const float*>(s.staging.p), twist, lo, hi, t_ref);
   // the packed timestamps are reused by the next call: the copy out of them must have landed
   CU_TRY(h, cudaEventSynchronize(h->ev_copy));
-  return VGICP_OK;
+  return rc;
 }
 
 // ---- continuous-time registration: the sweep's body twist estimated with the pose from per-point timestamps ----
@@ -2436,20 +2471,12 @@ int vgicp_set_source_timestamps(vgicp_handle h, const float* t, size_t n, size_t
   std::vector<float> packed;
   float lo = 0.0f, hi = 0.0f;
   if ((rc = timestamps_pack(h, "set_source_timestamps", t, n, stride_bytes, packed, &lo, &hi))) return rc;
-  const float tau = (float)t_ref;
-  // S = max |t_i - tau| over the float differences the kernels form (a float subtraction is monotonic in t_i)
-  const double span = fmax(fabs((double)(lo - tau)), fabs((double)(hi - tau)));
-  if (!std::isfinite(span)) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "set_source_timestamps: t_i - t_ref overflows a float");
-  CU_TRY(h, h->ct_times.reserve(n));
-  CU_TRY(h, cudaMemcpyAsync(h->ct_times.p, packed.data(), n * sizeof(float), cudaMemcpyHostToDevice, h->stream));
-  CU_TRY(h, cudaStreamSynchronize(h->stream));  // (`packed` goes out of scope)
-  h->ct_has_times = true;
-  h->ct_tau = tau;
-  h->ct_span = span;
-  h->ct_lo = lo;
-  h->ct_hi = hi;
-  h->ct_t_ref = t_ref;
-  return VGICP_OK;
+  return timestamps_commit(h, "set_source_timestamps", lo, hi, t_ref, [&]() -> int {
+    CU_TRY(h, h->ct_times.reserve(n));
+    CU_TRY(h, cudaMemcpyAsync(h->ct_times.p, packed.data(), n * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+    CU_TRY(h, cudaStreamSynchronize(h->stream));  // (`packed` goes out of scope)
+    return VGICP_OK;
+  });
 }
 
 // The same state from timestamps already in this GPU's memory: one kernel packs them into the spare buffer, counting the
@@ -2481,18 +2508,10 @@ int vgicp_set_source_timestamps_device(vgicp_handle h, const float* d_t, size_t 
     return v;
   };
   // min and max are exact in any order (only the sign of a zero can differ from the host pass, which leaves every |t - tau| alike)
-  const float lo = from_key(~st[1]), hi = from_key(st[2]);
-  const float tau = (float)t_ref;
-  const double span = fmax(fabs((double)(lo - tau)), fabs((double)(hi - tau)));
-  if (!std::isfinite(span)) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "set_source_timestamps_device: t_i - t_ref overflows a float");
-  std::swap(h->ct_times, h->ct_spare);
-  h->ct_has_times = true;
-  h->ct_tau = tau;
-  h->ct_span = span;
-  h->ct_lo = lo;
-  h->ct_hi = hi;
-  h->ct_t_ref = t_ref;
-  return VGICP_OK;
+  return timestamps_commit(h, "set_source_timestamps_device", from_key(~st[1]), from_key(st[2]), t_ref, [&]() -> int {
+    std::swap(h->ct_times, h->ct_spare);
+    return VGICP_OK;
+  });
 }
 
 // vgicp_deskew_source with the stored timestamps and t_ref: k_deskew_points reads ct_times, nothing is uploaded
@@ -2501,37 +2520,11 @@ int vgicp_deskew_source_stored(vgicp_handle h, const double twist[6]) {
   DeviceGuard g(h->device);
   if (!twist) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "deskew_source_stored: null twist");
   if (!h->ct_has_times) return fail(h, VGICP_ERR_BAD_STATE, "deskew_source_stored: the source has no timestamps (vgicp_set_source_timestamps(_device))");
-  Cloud& s = h->source;
-  const size_t n = (size_t)s.n;
-  const double t_ref = h->ct_t_ref;
-  const float tau = (float)t_ref;
-  float xi[6];
-  for (int j = 0; j < 6; j++) xi[j] = (float)twist[j];
-  for (int j = 0; j < 6; j++)
-    if (!std::isfinite(xi[j])) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "deskew_source_stored: non-finite twist");
-  const double span = fmax(fabs((double)h->ct_lo - t_ref), fabs((double)h->ct_hi - t_ref));
-  const double omega = sqrt(twist[0] * twist[0] + twist[1] * twist[1] + twist[2] * twist[2]);
-  if (omega * span > 1.5707963267948966)
-    return fail(h, VGICP_ERR_INVALID_ARGUMENT, "deskew_source_stored: the rotation over the sweep exceeds pi/2 (|omega| * max |t_i - t_ref|), beyond the series");
-  // ordering as vgicp_deskew_source's: after the main stream's reads of the source points and after an append
-  if (s.st != h->stream) {
-    if (!h->ev_deskew) CU_TRY(h, cudaEventCreateWithFlags(&h->ev_deskew, cudaEventDisableTiming));
-    CU_TRY(h, cudaEventRecord(h->ev_deskew, h->stream));
-    CU_TRY(h, cudaStreamWaitEvent(s.st, h->ev_deskew, 0));
-  }
-  if (s.st != h->target.st) CU_TRY(h, cudaStreamWaitEvent(s.st, h->ev_append, 0));
-  KLAUNCH_ST(h, s.st, VGICP_PROF_OTHER,
-             k_deskew_points<<<blocks_for(n, 256), 256, 0, s.st>>>(s.pts.p, h->ct_times.p, (int)n, tau, xi[0], xi[1], xi[2], xi[3], xi[4], xi[5]));
-  CU_TRY(h, cudaGetLastError());
-  CU_TRY(h, cudaEventRecord(s.ready, s.st));
+  int rc = deskew_twist_check(h, "deskew_source_stored", twist);
+  if (!rc) rc = deskew_enqueue(h, "deskew_source_stored", h->ct_times.p, twist, h->ct_lo, h->ct_hi, h->ct_t_ref);
+  if (rc) return rc;
   // the next write of the timestamp buffers (on the main stream) must not overtake this read of ct_times
-  if (s.st != h->stream) CU_TRY(h, cudaStreamWaitEvent(h->stream, s.ready, 0));
-  // the state vgicp_deskew_source leaves: no neighbour rows, no covariances, the NDT source map reset, the timestamps kept
-  s.k = 0;
-  s.has_cov = false;
-  h->ndt_ready = false;
-  h->ndt_s.built = false;
-  h->ndt_s.pending = false;
+  if (h->source.st != h->stream) CU_TRY(h, cudaStreamWaitEvent(h->stream, h->source.ready, 0));
   return VGICP_OK;
 }
 
@@ -2673,10 +2666,8 @@ int vgicp_comm_export_arena(vgicp_handle h, size_t max_points, unsigned char* ha
       cl[j]->covB.attach(reinterpret_cast<float2*>(base + max_points * 16), max_points);
       cl[j]->arena_slot = j;
       cl[j]->arena_seq = 0;
-      cl[j]->has_cov = false;
     }
-    h->map.built = false;
-    h->map.pending = false;
+    covariances_dropped(h);
   }
   cudaIpcMemHandle_t ipc;
   CU_TRY(h, cudaIpcGetMemHandle(&ipc, h->arena));
@@ -2760,8 +2751,7 @@ int vgicp_clear_source_shard(vgicp_handle h) {
 int vgicp_set_problem(vgicp_handle h, int problem) {
   CHECK_HANDLE(h);
   if (problem < 0 || problem > 2) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "set_problem: 0 VGICP, 1 NDT P2D, 2 NDT D2D");
-  if (problem != h->problem) { h->ndt_ready = false; h->has_lin = false; }
-  h->problem = problem;
+  problem_set(h, problem);
   return VGICP_OK;
 }
 

@@ -83,6 +83,20 @@ def main():
     full_sharded = c2.align()
     ms_full_sharded = 1e3 * (time.perf_counter() - t1)
     cov_equal = bool(np.array_equal(c2.get_source_covariances(), c.get_source_covariances()) and np.array_equal(c2.get_target_covariances(), c.get_target_covariances()))
+    # host-supplied neighbour rows after a k-NN search of a smaller cloud: the covariances must not follow that search's order.
+    # B is the target scaled, so that covariances left over from the run above differ from B's
+    tgt_b = (tgt * np.float32(1.01)).astype(np.float32)
+    c3 = Core(local)
+    c3.set_target_cloud(tgt_b)
+    c3.find_target_neighbors(20)
+    c3.calculate_target_covariances(REG_PLANE)
+    c2.set_target_cloud(tgt_b[: len(tgt_b) // 2])
+    c2.find_target_neighbors(20)
+    c2.set_target_cloud(tgt_b)
+    c2.set_target_neighbors(20, c3.get_target_neighbors())
+    c2.calculate_target_covariances(REG_PLANE)
+    given_rows_cov_equal = bool(np.array_equal(c2.get_target_covariances(), c3.get_target_covariances()))
+    c3.close()
     err2 = c2.comm_error()
     dist.barrier()
     c2.comm_shutdown()
@@ -97,6 +111,7 @@ def main():
         "iters": [int(sharded.nr_iterations), int(full.nr_iterations)], "converged": bool(sharded.converged), "ms_per_evaluation": ms_eval,
         "stage1_sharded_covariances_equal": cov_equal, "stage1_sharded_T": [float(x) for x in pose_from_c(full_sharded.T).reshape(-1)],
         "stage1_sharded_iters": int(full_sharded.nr_iterations), "stage1_sharded_comm_error": err2, "ms_registration_stage1_sharded": ms_full_sharded,
+        "given_rows_covariances_equal": given_rows_cov_equal,
     }
     print(json.dumps(out), flush=True)
     dist.barrier()

@@ -50,6 +50,8 @@ def test_sharded_evaluation_matches_single_gpu():
         # stage 1 sharded too: the exchanged covariances are the unsharded ones bit for bit, so the registration walks the same iterates
         assert r["stage1_sharded_comm_error"] == 0 and r["stage1_sharded_covariances_equal"]
         assert r["stage1_sharded_T"] == r["T"] and r["stage1_sharded_iters"] == r["iters"][0]
+        # neighbour rows given by the host after a k-NN search of a smaller cloud: unsharded covariances, bit for bit
+        assert r["given_rows_covariances_equal"]
     # every rank holds bit-identical sums (same doubles added in rank order)
     for r in res[1:]:
         assert r["H_sum"] == res[0]["H_sum"] and r["b"] == res[0]["b"] and r["err"] == res[0]["err"] and r["T"] == res[0]["T"]
