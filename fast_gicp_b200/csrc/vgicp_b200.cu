@@ -1049,18 +1049,31 @@ int multi_reserve(vgicp_handle h, int rows, int grid) {
 
 // Staged input of one round, in h->h_multi_in: Pose[n_hyp][2] (Tlin, Teval per hypothesis), then the row list (hypothesis per
 // row, the rows of all launches of the round back to back).  One copy to the device per round.
-Pose* multi_poses(vgicp_handle h) { return reinterpret_cast<Pose*>(h->h_multi_in); }
 size_t multi_rows_offset(int n_hyp) { return ((size_t)n_hyp * 2 * sizeof(Pose) + 15) & ~(size_t)15; }
-int* multi_rows(vgicp_handle h, int n_hyp) { return reinterpret_cast<int*>(h->h_multi_in + multi_rows_offset(n_hyp)); }
-int multi_upload(vgicp_handle h, int n_hyp, int n_rows) {
-  CU_TRY(h, cudaMemcpyAsync(h->d_multi_in, h->h_multi_in, multi_rows_offset(n_hyp) + (size_t)n_rows * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-  return VGICP_OK;
-}
+struct MultiRound {
+  vgicp_handle h;
+  int n_hyp;
+  int n = 0;  // rows staged
+  Pose* poses = reinterpret_cast<Pose*>(h->h_multi_in);
+  int* rows = reinterpret_cast<int*>(h->h_multi_in + multi_rows_offset(n_hyp));
+  // the next row: hypothesis i, evaluated at Te over the correspondences of Tl
+  void add(int i, const double* Tl, const double* Te) {
+    rows[n++] = i;
+    poses[2 * i] = to_pose(Tl);
+    poses[2 * i + 1] = to_pose(Te);
+  }
+  // a new sequence number for the round's records, and the copy
+  int upload() {
+    h->multi.seq++;
+    CU_TRY(h, cudaMemcpyAsync(h->d_multi_in, h->h_multi_in, multi_rows_offset(n_hyp) + (size_t)n * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    return VGICP_OK;
+  }
+};
 
 // one launch over rows [row0, row0 + n) of the staged row list, all computing `kind`; the records land in rows [row0, row0 + n)
 // of the multi-pose output.  count: also count the hits (kEvalLinearize / kEvalError only).  src: the multi-source kernels, each
 // row on its own source and grid from this descriptor table (L: the launch class's kernel, grid = the largest of its rows)
-int launch_multi(vgicp_handle h, const LinLaunch& L, int n_hyp, int kind, bool count, int row0, int n, const SourceRow* src = nullptr) {
+int launch_multi(vgicp_handle h, const LinLaunch& L, int n_hyp, int kind, bool count, int row0, int n, const SourceRow* src) {
   const LinArgs& a = L.a;
   const EvalChannel::Dest d = h->multi.dest(h->exec_hint == 0, row0);
   MultiArgs m;
@@ -1069,23 +1082,24 @@ int launch_multi(vgicp_handle h, const LinLaunch& L, int n_hyp, int kind, bool c
   m.partials = h->multi.partials.p;  // (the launches of a round run one after the other on the stream: slices and tickets are reused)
   m.tickets = h->multi.tickets;
   m.out = d.out; m.done = d.done; m.done_seq = d.seq;
+  m.src = src;
   const dim3 grid(L.grid, n);
   return launch_eval(h, kind, a.robust, [&](auto what, auto rb) {
     constexpr int WHAT = decltype(what)::value;
     constexpr bool RB = decltype(rb)::value;
-    auto with_count = [&](auto cnt) {
+    auto with_rows = [&](auto cnt, auto per_source) {
       constexpr bool COUNT = decltype(cnt)::value && WHAT != kEvalSpec;  // (the speculative evaluation counts no hits)
+      constexpr bool SRC = decltype(per_source)::value;
       if (L.stream) {
-        if (src) k_linearize_stream_multi_src<WHAT, RB><<<grid, kLinThreads, sizeof(LinStreamSmem), h->stream>>>(a, m, src);
-        else k_linearize_stream_multi<WHAT, COUNT, RB><<<grid, kLinThreads, sizeof(LinStreamSmem), h->stream>>>(a, m);
+        k_linearize_stream_multi<WHAT, COUNT, RB, SRC><<<grid, kLinThreads, sizeof(LinStreamSmem), h->stream>>>(a, m);
         return true;
       }
       return with_lin_shape(h->offset_mode, L.G, [&](auto mode, auto g) {
-        if (src) k_linearize_multi_src<decltype(mode)::value, WHAT, decltype(g)::value, RB><<<grid, kLinThreads, 0, h->stream>>>(a, m, src);
-        else k_linearize_multi<decltype(mode)::value, WHAT, decltype(g)::value, COUNT, RB><<<grid, kLinThreads, 0, h->stream>>>(a, m);
+        k_linearize_multi<decltype(mode)::value, WHAT, decltype(g)::value, COUNT, RB, SRC><<<grid, kLinThreads, 0, h->stream>>>(a, m);
       });
     };
-    return count ? with_count(std::true_type{}) : with_count(std::false_type{});
+    if (m.src) return with_rows(std::false_type{}, std::true_type{});  // (the multi-source rows count no hits)
+    return count ? with_rows(std::true_type{}, std::false_type{}) : with_rows(std::false_type{}, std::false_type{});
   });
 }
 
@@ -1107,6 +1121,13 @@ struct LmState {
   int it, lm_j, converged, lm_failed, n_linearize, n_error, nr_iterations;
 };
 enum { kLmLinearize = 0, kLmError = 1, kLmDone = 2 };
+
+// the caller's parameters, or the defaults when it passes none
+vgicp_lsq_params lsq_params(const vgicp_lsq_params* params) {
+  vgicp_lsq_params P;
+  if (params) P = *params; else vgicp_lsq_default_params(&P);
+  return P;
+}
 
 template <int N>
 LmState<N> lm_init(const double* guess, const vgicp_lsq_params& P) {
@@ -1254,7 +1275,10 @@ bool lm_consume(LmState<6>* st, const double* rec, bool spec) {
   return true;
 }
 
-void lm_result(const LmState<6>& st, vgicp_align_result* res) {
+// a finished run's estimate, final system matrix and counters: the whole vgicp_align_result, all of vgicp_align_ct_result but the twist
+template <int N, class R>
+void lm_result(const LmState<N>& st, R* res) {
+  static_assert(sizeof(res->H) == sizeof(st.final_H), "the result's H is the state's N x N final_H");
   memset(res, 0, sizeof(*res));
   memcpy(res->T, st.x0.m, sizeof(res->T));
   memcpy(res->H, st.final_H, sizeof(res->H));
@@ -1812,8 +1836,7 @@ int vgicp_align(vgicp_handle h, const double guess[16], const vgicp_lsq_params* 
   DeviceGuard g(h->device);
   if (!guess || !res) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "align: null argument");
   { int rc = check_ready(h, "align", kNeedEval); if (!rc) rc = sync_inputs(h); if (rc) return rc; }
-  vgicp_lsq_params P;
-  if (params) P = *params; else vgicp_lsq_default_params(&P);
+  const vgicp_lsq_params P = lsq_params(params);
   const bool speculate = h->speculate != 0 && !P.use_gauss_newton;
   LmState<6> st = lm_init<6>(guess, P);
   while (st.phase != kLmDone) {
@@ -1831,6 +1854,50 @@ int vgicp_align(vgicp_handle h, const double guess[16], const vgicp_lsq_params* 
   return VGICP_OK;
 }
 
+// The optimiser rounds of B LM states over shared multi-row launches (vgicp_align_multi, vgicp_align_sources).  Each round stages
+// the running rows -- the linearisations first, then the trials, class by class within each -- and issues one launch per class and
+// evaluation kind, with the largest grid of its rows; then every record goes to its state.  classes: the kernel and arguments of
+// each launch class; cls[i], grid[i]: state i's class and its single-pose grid; src: the multi-source descriptor table (state i on
+// source i), or nullptr (every state on the handle's source).
+int lm_rounds(vgicp_handle h, std::vector<LmState<6>>& st, const std::vector<LinLaunch>& classes, const std::vector<int>& cls,
+              const std::vector<int>& grid, const SourceRow* src, bool speculate) {
+  const int B = (int)st.size();
+  int grid_max = 0;
+  for (int i = 0; i < B; i++) grid_max = grid[i] > grid_max ? grid[i] : grid_max;
+  int rc = multi_reserve(h, B, grid_max);
+  if (rc) return rc;
+  struct Group { int row0, n, cls, grid; bool lin; };
+  std::vector<Group> groups;
+  for (;;) {
+    MultiRound round{h, B};
+    int n_lin = 0;
+    groups.clear();
+    for (int lin = 1; lin >= 0; lin--) {
+      for (int q = 0; q < (int)classes.size(); q++) {
+        Group gr{round.n, 0, q, 0, lin != 0};
+        for (int i = 0; i < B; i++) {
+          if (cls[i] != q || st[i].phase != (lin ? kLmLinearize : kLmError)) continue;
+          round.add(i, st[i].x0.m, lin ? st[i].x0.m : st[i].xi.m);
+          gr.grid = grid[i] > gr.grid ? grid[i] : gr.grid;
+        }
+        gr.n = round.n - gr.row0;
+        if (gr.n) groups.push_back(gr);
+      }
+      if (lin) n_lin = round.n;
+    }
+    if (round.n == 0) return VGICP_OK;
+    if ((rc = round.upload())) return rc;
+    for (const Group& gr : groups) {
+      LinLaunch L = classes[gr.cls];
+      L.grid = gr.grid;
+      if ((rc = launch_multi(h, L, B, gr.lin ? kEvalLinearize : (speculate ? kEvalSpec : kEvalError), false, gr.row0, gr.n, src))) return rc;
+    }
+    if ((rc = h->multi.wait(h, round.n, (size_t)round.n * kMultiOut))) return rc;
+    const double* rec = h->multi.h_out;
+    for (int r = 0; r < round.n; r++) lm_consume(&st[round.rows[r]], rec + (size_t)r * kMultiOut, r >= n_lin && speculate);
+  }
+}
+
 // B registrations from B initial guesses.  Each hypothesis runs vgicp_align's state machine; every round stages the poses of the
 // running hypotheses and evaluates all of them in one launch per evaluation kind.  With LM and speculation every round after the
 // first is one k_linearize_multi<kEvalSpec> launch, whose accepted trials feed their linearisation straight back, as in vgicp_align.
@@ -1840,39 +1907,13 @@ int vgicp_align_multi(vgicp_handle h, const double* guesses, int n_guesses, cons
   if (!guesses || !results || n_guesses < 1 || n_guesses > kMultiMaxHyp) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "align_multi: null argument or n_guesses outside [1, 4096]");
   int rc = check_ready(h, "align_multi", kNeedEval | kNeedOneGpu);
   if (rc || (rc = sync_inputs(h))) return rc;
-  vgicp_lsq_params P;
-  if (params) P = *params; else vgicp_lsq_default_params(&P);
+  const vgicp_lsq_params P = lsq_params(params);
   const int B = n_guesses;
   const LinLaunch L = make_lin_launch(h);
-  if ((rc = multi_reserve(h, B, L.grid))) return rc;
   std::vector<LmState<6>> st(B);
   for (int i = 0; i < B; i++) st[i] = lm_init<6>(guesses + 16 * i, P);
   const bool speculate = h->speculate != 0 && !P.use_gauss_newton;
-  for (;;) {
-    Pose* poses = multi_poses(h);
-    int* rows = multi_rows(h, B);
-    int n = 0;
-    for (int i = 0; i < B; i++)
-      if (st[i].phase == kLmLinearize) {
-        rows[n++] = i;
-        poses[2 * i] = poses[2 * i + 1] = to_pose(st[i].x0.m);
-      }
-    const int n_lin = n;
-    for (int i = 0; i < B; i++)
-      if (st[i].phase == kLmError) {
-        rows[n++] = i;
-        poses[2 * i] = to_pose(st[i].x0.m);
-        poses[2 * i + 1] = to_pose(st[i].xi.m);
-      }
-    if (n == 0) break;
-    h->multi.seq++;
-    if ((rc = multi_upload(h, B, n))) return rc;
-    if (n_lin && (rc = launch_multi(h, L, B, kEvalLinearize, false, 0, n_lin))) return rc;
-    if (n > n_lin && (rc = launch_multi(h, L, B, speculate ? kEvalSpec : kEvalError, false, n_lin, n - n_lin))) return rc;
-    if ((rc = h->multi.wait(h, n, (size_t)n * kMultiOut))) return rc;
-    const double* rec = h->multi.h_out;
-    for (int r = 0; r < n; r++) lm_consume(&st[rows[r]], rec + (size_t)r * kMultiOut, r >= n_lin && speculate);
-  }
+  if ((rc = lm_rounds(h, st, {L}, std::vector<int>(B, 0), std::vector<int>(B, L.grid), nullptr, speculate))) return rc;
   for (int i = 0; i < B; i++) lm_result(st[i], &results[i]);
   return VGICP_OK;
 }
@@ -1889,15 +1930,10 @@ int vgicp_evaluate_poses(vgicp_handle h, const double* T, int n_poses, double* e
   const bool want_H = H36 != nullptr;
   const LinLaunch L = make_lin_launch(h);
   if ((rc = multi_reserve(h, B, L.grid))) return rc;
-  Pose* poses = multi_poses(h);
-  int* rows = multi_rows(h, B);
-  for (int i = 0; i < B; i++) {
-    poses[2 * i] = poses[2 * i + 1] = to_pose(T + 16 * i);  // linearized_x = trans.cast<float>(), evaluated at the same pose
-    rows[i] = i;
-  }
-  h->multi.seq++;
-  if ((rc = multi_upload(h, B, B))) return rc;
-  if ((rc = launch_multi(h, L, B, want_H ? kEvalLinearize : kEvalError, true, 0, B))) return rc;
+  MultiRound round{h, B};
+  for (int i = 0; i < B; i++) round.add(i, T + 16 * i, T + 16 * i);  // linearized_x = trans.cast<float>(), evaluated at the same pose
+  if ((rc = round.upload())) return rc;
+  if ((rc = launch_multi(h, L, B, want_H ? kEvalLinearize : kEvalError, true, 0, B, nullptr))) return rc;
   if ((rc = h->multi.wait(h, B, (size_t)B * kMultiOut))) return rc;
   const double* rec = h->multi.h_out;
   for (int i = 0; i < B; i++) {
@@ -1936,8 +1972,7 @@ int vgicp_align_sources(vgicp_handle h, const float* const* xyz, const size_t* n
   if (!h->map.built && !h->map.pending) return fail(h, VGICP_ERR_BAD_STATE, "align_sources: target voxel map not built");
   int rc = sync_inputs(h);
   if (rc) return rc;
-  vgicp_lsq_params P;
-  if (params) P = *params; else vgicp_lsq_default_params(&P);
+  const vgicp_lsq_params P = lsq_params(params);
 
   // pool slots: at least one spare element per source (the streaming kernel reads covB in whole 16-byte units) and an even start,
   // so that every source's covB is 16-byte aligned like a cloud of its own
@@ -1962,9 +1997,10 @@ int vgicp_align_sources(vgicp_handle h, const float* const* xyz, const size_t* n
   CU_TRY(h, cudaEventRecord(c.ready, h->stream));
   CU_TRY(h, cudaStreamWaitEvent(c.st, c.ready, 0));
 
-  // stage 1, source by source, and each source's launch shape
+  // stage 1, source by source, and each source's launch shape and class: sources that share a kernel share the launches
   std::vector<SourceRow> desc(B);
-  std::vector<LinLaunch> shape(B);
+  std::vector<LinLaunch> classes;  // per class, the kernel and arguments of its first source
+  std::vector<int> cls(B), grid(B);
   for (int i = 0; i < B; i++) {
     const size_t cap = off[i + 1] - off[i];
     c.pts.attach(h->src_pts.p + off[i], cap);
@@ -1974,61 +2010,21 @@ int vgicp_align_sources(vgicp_handle h, const float* const* xyz, const size_t* n
     if ((rc = find_neighbors(h, c, k))) return rc;
     rc = calc_covariances(h, c, regularization_method);
     if (rc && !(rc == VGICP_ERR_UNSUPPORTED && regularization_method == VGICP_REG_NORMALIZED_MIN_EIG)) return rc;  // (raw covariances, as vgicp_register)
-    shape[i] = make_lin_launch(h, c.pts.p, c.covA.p, c.covB.p, c.n);
-    desc[i] = SourceRow{c.pts.p, c.covA.p, c.covB.p, c.n, shape[i].grid};
+    const LinLaunch L = make_lin_launch(h, c.pts.p, c.covA.p, c.covB.p, c.n);
+    desc[i] = SourceRow{c.pts.p, c.covA.p, c.covB.p, c.n, L.grid};
+    grid[i] = L.grid;
+    cls[i] = 0;
+    while (cls[i] < (int)classes.size() && !(classes[cls[i]].stream == L.stream && classes[cls[i]].G == L.G)) cls[i]++;
+    if (cls[i] == (int)classes.size()) classes.push_back(L);
   }
   CU_TRY(h, cudaMemcpyAsync(h->src_rows.p, desc.data(), sizeof(SourceRow) * B, cudaMemcpyHostToDevice, h->stream));
   CU_TRY(h, cudaStreamWaitEvent(h->stream, c.ready, 0));
 
-  // launch classes: sources that share a kernel share the launches
-  std::vector<int> cls(B), rep;  // class of each source; rep[c]: a source of class c (its kernel and arguments)
-  int grid_max = 0;
-  for (int i = 0; i < B; i++) {
-    int q = 0;
-    while (q < (int)rep.size() && !(shape[rep[q]].stream == shape[i].stream && shape[rep[q]].G == shape[i].G)) q++;
-    if (q == (int)rep.size()) rep.push_back(i);
-    cls[i] = q;
-    grid_max = shape[i].grid > grid_max ? shape[i].grid : grid_max;
-  }
-  if ((rc = multi_reserve(h, B, grid_max))) return rc;
   std::vector<LmState<6>> st(B);
   const double I[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
   for (int i = 0; i < B; i++) st[i] = lm_init<6>(guesses ? guesses + 16 * i : I, P);
   const bool speculate = h->speculate != 0 && !P.use_gauss_newton;
-  struct Group { int row0, n, cls, grid; bool lin; };
-  std::vector<Group> groups;
-  for (;;) {
-    Pose* poses = multi_poses(h);
-    int* rows = multi_rows(h, B);
-    int nr = 0, n_lin = 0;
-    groups.clear();
-    for (int lin = 1; lin >= 0; lin--) {  // the linearisations first, then the trials; class by class within each
-      for (int q = 0; q < (int)rep.size(); q++) {
-        const int row0 = nr;
-        int grid = 0;
-        for (int i = 0; i < B; i++) {
-          if (cls[i] != q || st[i].phase != (lin ? kLmLinearize : kLmError)) continue;
-          rows[nr++] = i;
-          poses[2 * i] = to_pose(st[i].x0.m);
-          poses[2 * i + 1] = to_pose(lin ? st[i].x0.m : st[i].xi.m);
-          grid = desc[i].grid > grid ? desc[i].grid : grid;
-        }
-        if (nr > row0) groups.push_back(Group{row0, nr - row0, q, grid, lin != 0});
-      }
-      if (lin) n_lin = nr;
-    }
-    if (nr == 0) break;
-    h->multi.seq++;
-    if ((rc = multi_upload(h, B, nr))) return rc;
-    for (const Group& gr : groups) {
-      LinLaunch L = shape[rep[gr.cls]];
-      L.grid = gr.grid;
-      if ((rc = launch_multi(h, L, B, gr.lin ? kEvalLinearize : (speculate ? kEvalSpec : kEvalError), false, gr.row0, gr.n, h->src_rows.p))) return rc;
-    }
-    if ((rc = h->multi.wait(h, nr, (size_t)nr * kMultiOut))) return rc;
-    const double* rec = h->multi.h_out;
-    for (int r = 0; r < nr; r++) lm_consume(&st[rows[r]], rec + (size_t)r * kMultiOut, r >= n_lin && speculate);
-  }
+  if ((rc = lm_rounds(h, st, classes, cls, grid, h->src_rows.p, speculate))) return rc;
   for (int i = 0; i < B; i++) lm_result(st[i], &results[i]);
   return VGICP_OK;
 }
@@ -2565,8 +2561,7 @@ int vgicp_align_ct(vgicp_handle h, const double guess[16], const double twist_gu
   if (rc) return rc;
   if (!twist_in_series(twist_guess, h->ct_span) || !twist_in_series(twist_prior, h->ct_span))
     return fail(h, VGICP_ERR_INVALID_ARGUMENT, "align_ct: the twist guess or prior rotates more than pi/2 over the sweep (|omega| * max |s_i|), beyond the series");
-  vgicp_lsq_params P;
-  if (params) P = *params; else vgicp_lsq_default_params(&P);
+  const vgicp_lsq_params P = lsq_params(params);
   if ((rc = sync_inputs(h))) return rc;
   CU_TRY(h, h->ct.open(1, kCtStride, (size_t)kLinMaxBlocks * kCtStride, h->stream));
   LmState<12> st = lm_init<12>(guess, P);
@@ -2591,15 +2586,8 @@ int vgicp_align_ct(vgicp_handle h, const double guess[16], const double twist_gu
     }
     lm_advance(&st, rec);
   }
-  memset(res, 0, sizeof(*res));
-  memcpy(res->T, st.x0.m, sizeof(res->T));
+  lm_result(st, res);
   memcpy(res->twist, st.tw0, sizeof(res->twist));
-  memcpy(res->H, st.final_H, sizeof(res->H));
-  res->nr_iterations = st.nr_iterations;
-  res->converged = st.converged;
-  res->n_linearize = st.n_linearize;
-  res->n_compute_error = st.n_error;
-  res->lm_failed = st.lm_failed;
   return VGICP_OK;
 }
 

@@ -1229,6 +1229,19 @@ constexpr int kMultiMaxHyp = 4096;
 constexpr int kMultiOut = 48;        // per-row record: [0..42] err, H, b;  [43] speculative: err over the old correspondences;
 constexpr int kMultiOutCount = 44;   //                 [44] hit count (the length of the reference's correspondence list)
 
+// Multi-source rows (vgicp_align_sources; the kernels' SRC): many source clouds against the same map.  m.hyp[y] names row y's
+// source, which is both its pose pair in m.poses and its entry in the descriptor table m.src: the source's arrays, its size and the
+// grid of its single-pose launch.  The launch has the largest grid of its rows; a row's blocks past its own grid leave at once, and
+// the others split the tasks and fold the partials over the row's grid, not gridDim.x, so each row's sums are its single-pose sums
+// bit for bit.
+struct SourceRow {
+  const float4* pts;
+  const float4* covA;
+  const float2* covB;
+  int n;
+  int grid;
+};
+
 struct MultiArgs {
   const int* hyp;            // [gridDim.y]: hypothesis evaluated by each row
   const Pose* poses;         // [hypothesis][2] = Tlin, Teval
@@ -1237,7 +1250,21 @@ struct MultiArgs {
   double* out;               // [gridDim.y][kMultiOut]; may be mapped pinned host memory
   volatile unsigned long long* done;  // optional [gridDim.y] (mapped host memory): set to done_seq once the row's record is complete
   unsigned long long done_seq;
+  const SourceRow* src;      // multi-source: [source] descriptor table (the SRC kernels); nullptr for multi-pose
 };
+
+// the row's source and grid, or false in the blocks past the row's grid (before any barrier, shared store or partial)
+__device__ __forceinline__ bool source_row(const MultiArgs& m, SourceRow& s) {
+  const SourceRow* __restrict__ src = m.src;  // read-only in the kernel: no store aliases it
+  s = src[__ldg(&m.hyp[blockIdx.y])];
+  return blockIdx.x < (unsigned)s.grid;
+}
+// the single-pose arguments with the row's source in place of the handle's
+__device__ __forceinline__ LinArgs source_args(const LinArgs& a, const SourceRow& s) {
+  LinArgs r = a;
+  r.pts = s.pts; r.covA = s.covA; r.covB = s.covB; r.n = s.n;
+  return r;
+}
 
 // the row's Tlin, Teval staged in shared memory (sp[0], sp[1]): read like the single-pose kernels' parameter-space poses, without
 // holding 24 more registers (which made ptxas spill in the error-only kernels)
@@ -1249,8 +1276,8 @@ __device__ __forceinline__ int multi_row(const MultiArgs& m, Pose* sp) {
   return y;
 }
 template <int NV>
-__device__ __forceinline__ bool multi_reduce(const LinArgs& a, const MultiArgs& m, int y, const float* sum, double (*fin)[kLinStride]) {
-  return lin_reduce<NV>(a, sum, fin, m.partials + (size_t)y * gridDim.x * kLinStride, m.tickets + y, 0);
+__device__ __forceinline__ bool multi_reduce(const LinArgs& a, const MultiArgs& m, int y, const float* sum, double (*fin)[kLinStride], unsigned nblk) {
+  return lin_reduce<NV>(a, sum, fin, m.partials + (size_t)y * gridDim.x * kLinStride, m.tickets + y, nblk);
 }
 // thread 0 of a row's last block: the row's record, its hit count (COUNT), then the row's ticket and completion word
 template <int WHAT, bool COUNT>
@@ -1261,81 +1288,46 @@ __device__ __forceinline__ void multi_finish(const MultiArgs& m, int y, const do
   lin_publish(m.tickets, m.done, m.done_seq, y);
 }
 
-template <int MODE, int WHAT, int G, bool COUNT, bool RB>
+// SRC: every row evaluates its own source from m.src over its own grid (multi-source); otherwise the launch's source over gridDim.x
+template <int MODE, int WHAT, int G, bool COUNT, bool RB, bool SRC>
 __global__ void __launch_bounds__(kLinThreads, 1) k_linearize_multi(const LinArgs a, const MultiArgs m) {
   static_assert(!(WHAT == kEvalSpec && COUNT), "the speculative evaluation does not count hits");
+  static_assert(!(SRC && COUNT), "the multi-source rows count no hits");
   constexpr int NV = eval_values(WHAT) + (COUNT ? 1 : 0);
   __shared__ double fin[4][kLinStride];
   __shared__ Pose sp[2];
+  SourceRow s;
+  unsigned nblk = 0;  // gridDim.x
+  if constexpr (SRC) {
+    if (!source_row(m, s)) return;
+    nblk = (unsigned)s.grid;
+  }
   const int y = multi_row(m, sp);
   float sum[NV];
-  lin_eval_accumulate<MODE, WHAT, G, COUNT, RB>(a, sp[0], sp[1], sum, 0);
-  if (!multi_reduce<NV>(a, m, y, sum, fin)) return;
+  if constexpr (SRC) lin_eval_accumulate<MODE, WHAT, G, COUNT, RB>(source_args(a, s), sp[0], sp[1], sum, nblk);
+  else lin_eval_accumulate<MODE, WHAT, G, COUNT, RB>(a, sp[0], sp[1], sum, nblk);
+  if (!multi_reduce<NV>(a, m, y, sum, fin, nblk)) return;
   if (threadIdx.x == 0) multi_finish<WHAT, COUNT>(m, y, fin[0]);
 }
 
-template <int WHAT, bool COUNT, bool RB>
+template <int WHAT, bool COUNT, bool RB, bool SRC>
 __global__ void __launch_bounds__(kLinThreads, 1) k_linearize_stream_multi(const LinArgs a, const MultiArgs m) {
+  static_assert(!(SRC && COUNT), "the multi-source rows count no hits");
   constexpr int NV = eval_values(WHAT) + (COUNT ? 1 : 0);
   __shared__ double fin[4][kLinStride];
   __shared__ Pose sp[2];
+  SourceRow s;
+  unsigned nblk = 0;  // gridDim.x
+  if constexpr (SRC) {
+    if (!source_row(m, s)) return;
+    nblk = (unsigned)s.grid;
+  }
   const int y = multi_row(m, sp);
   float sum[NV];
-  lin_stream_accumulate<WHAT, COUNT, RB>(a, sp[0], sp[1], sum, 0);
-  if (!multi_reduce<NV>(a, m, y, sum, fin)) return;
+  if constexpr (SRC) lin_stream_accumulate<WHAT, COUNT, RB>(source_args(a, s), sp[0], sp[1], sum, nblk);
+  else lin_stream_accumulate<WHAT, COUNT, RB>(a, sp[0], sp[1], sum, nblk);
+  if (!multi_reduce<NV>(a, m, y, sum, fin, nblk)) return;
   if (threadIdx.x == 0) multi_finish<WHAT, COUNT>(m, y, fin[0]);
-}
-
-// Multi-source evaluation (vgicp_align_sources): many source clouds against the same map.  m.hyp[y] names row y's source, which is
-// both its pose pair in m.poses and its entry in the descriptor table: the source's arrays, its size and the grid of its
-// single-pose launch.  The launch has the largest grid of its rows; a row's blocks past its own grid leave at once, and the others
-// split the tasks and fold the partials over the row's grid, not gridDim.x, so each row's sums are its single-pose sums bit for bit.
-struct SourceRow {
-  const float4* pts;
-  const float4* covA;
-  const float2* covB;
-  int n;
-  int grid;
-};
-
-// the row's source and grid, or false in the blocks past the row's grid (before any barrier, shared store or partial)
-__device__ __forceinline__ bool source_row(const MultiArgs& m, const SourceRow* src, SourceRow& s) {
-  s = src[__ldg(&m.hyp[blockIdx.y])];
-  return blockIdx.x < (unsigned)s.grid;
-}
-// the single-pose arguments with the row's source in place of the handle's
-__device__ __forceinline__ LinArgs source_args(const LinArgs& a, const SourceRow& s) {
-  LinArgs r = a;
-  r.pts = s.pts; r.covA = s.covA; r.covB = s.covB; r.n = s.n;
-  return r;
-}
-
-template <int MODE, int WHAT, int G, bool RB>
-__global__ void __launch_bounds__(kLinThreads, 1) k_linearize_multi_src(const LinArgs a, const MultiArgs m, const SourceRow* __restrict__ src) {
-  constexpr int NV = eval_values(WHAT);
-  __shared__ double fin[4][kLinStride];
-  __shared__ Pose sp[2];
-  SourceRow s;
-  if (!source_row(m, src, s)) return;
-  const int y = multi_row(m, sp);
-  float sum[NV];
-  lin_eval_accumulate<MODE, WHAT, G, false, RB>(source_args(a, s), sp[0], sp[1], sum, (unsigned)s.grid);
-  if (!lin_reduce<NV>(a, sum, fin, m.partials + (size_t)y * gridDim.x * kLinStride, m.tickets + y, (unsigned)s.grid)) return;
-  if (threadIdx.x == 0) multi_finish<WHAT, false>(m, y, fin[0]);
-}
-
-template <int WHAT, bool RB>
-__global__ void __launch_bounds__(kLinThreads, 1) k_linearize_stream_multi_src(const LinArgs a, const MultiArgs m, const SourceRow* __restrict__ src) {
-  constexpr int NV = eval_values(WHAT);
-  __shared__ double fin[4][kLinStride];
-  __shared__ Pose sp[2];
-  SourceRow s;
-  if (!source_row(m, src, s)) return;
-  const int y = multi_row(m, sp);
-  float sum[NV];
-  lin_stream_accumulate<WHAT, false, RB>(source_args(a, s), sp[0], sp[1], sum, (unsigned)s.grid);
-  if (!lin_reduce<NV>(a, sum, fin, m.partials + (size_t)y * gridDim.x * kLinStride, m.tickets + y, (unsigned)s.grid)) return;
-  if (threadIdx.x == 0) multi_finish<WHAT, false>(m, y, fin[0]);
 }
 
 // Materialise the reference's correspondence list for the getter (fast_vgicp_cuda.cu:221-225): dense [n_off][n] voxel ids,

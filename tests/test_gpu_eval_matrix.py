@@ -294,7 +294,8 @@ def test_ndt(pair02, relative_pose, big, size, problem, method):
 
 @pytest.mark.parametrize("size", ALIGN_SIZES)
 def test_speculation_and_multi_hypothesis_are_bit_identical(pair02, relative_pose, big, size):
-    """DIRECT1 where it streams (k_linearize_stream<2> / k_linearize_stream_multi) and, over the hash table, where it does not."""
+    """DIRECT1 where it streams (k_linearize_stream<kEvalSpec> / k_linearize_stream_multi<kEvalSpec, ..., SRC = false>) and, over the
+    hash table, where it does not."""
     h = vgicp_handle(size, "plane", pair02, relative_pose, big)
     c = h["core"]
     c.set_neighbor_search_method(O.DIRECT1)
