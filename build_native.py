@@ -74,7 +74,8 @@ PREP_LIB_PATH = os.path.join(LIB_DIR, "libvgicp_prep_b200.so")
 def build_prep(force=False):
     """Input-preparation library (include/vgicp_prep_b200.h): lib/libvgicp_prep_b200.so, independent of libvgicp_b200.so."""
     hdr = os.path.join(ROOT, "include", "vgicp_prep_b200.h")
-    deps = (PREP_SRC, hdr, os.path.join(CSRC, "vgicp_sort.cuh"))  # the exact grid uses the library's radix sort
+    # the exact grid uses the library's radix sort; both grids its block rank, cell box and device arrays
+    deps = (PREP_SRC, hdr) + tuple(os.path.join(CSRC, f) for f in ("vgicp_sort.cuh", "vgicp_scan.cuh", "vgicp_devbuf.hpp"))
     if not force and os.path.exists(PREP_LIB_PATH) and all(os.path.getmtime(d) <= os.path.getmtime(PREP_LIB_PATH) for d in deps):
         return PREP_LIB_PATH
     os.makedirs(LIB_DIR, exist_ok=True)

@@ -18,8 +18,11 @@
 #include <new>
 #include <string>
 
+#include "../vgicp_scan.cuh"
 #include "../vgicp_sort.cuh"
 #include "vgicp_prep_b200.h"
+
+using namespace vgicp;
 
 namespace {
 
@@ -151,57 +154,18 @@ __global__ void __launch_bounds__(kHist) k_prep_walk(const float4* __restrict__ 
   }
 }
 
-// rank of every flushed centroid = number of flushes at smaller point indices; one block per 1024 points, decoupled look-back over
-// epoch-tagged block totals (a block only waits for blocks with a smaller index, which were scheduled before it)
+// rank of every flushed centroid = number of flushes at smaller point indices (block_rank, one block per kRankThreads points);
 // output records of 3 + F floats: x y z, then the F fields
 template <int F>
-__global__ void __launch_bounds__(1024) k_prep_scatter(const float4* __restrict__ flushed, int n, float* __restrict__ out, size_t cap, unsigned long long* chunk_state,
-                                                       unsigned epoch, int* __restrict__ total, const float* __restrict__ fflushed) {
-  __shared__ int warp_sums[32];
-  __shared__ int s_base;
-  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  const int i = blockIdx.x * 1024 + tid;
+__global__ void __launch_bounds__(kRankThreads) k_prep_scatter(const float4* __restrict__ flushed, int n, float* __restrict__ out, size_t cap, unsigned long long* chunk_state,
+                                                               unsigned epoch, int* __restrict__ total, const float* __restrict__ fflushed) {
+  const int i = blockIdx.x * kRankThreads + threadIdx.x;
   float4 f = make_float4(0.f, 0.f, 0.f, 0.f);
   if (i < n) f = flushed[i];
   const int flag = f.w != 0.f ? 1 : 0;
-  int v = flag;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    int t = __shfl_up_sync(0xffffffffu, v, o);
-    if (lane >= o) v += t;
-  }
-  if (lane == 31) warp_sums[wid] = v;
-  __syncthreads();
-  if (wid == 0) {
-    int w = warp_sums[lane];
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      int t = __shfl_up_sync(0xffffffffu, w, o);
-      if (lane >= o) w += t;
-    }
-    warp_sums[lane] = w;
-    const int block_total = __shfl_sync(0xffffffffu, w, 31);
-    volatile unsigned long long* state = chunk_state;
-    if (lane == 0) {
-      state[blockIdx.x] = ((unsigned long long)epoch << 32) | (unsigned)block_total;
-      __threadfence();
-    }
-    int base = 0;
-    for (int p = (int)blockIdx.x - 1 - lane; p >= 0; p -= 32) {
-      unsigned long long sv;
-      while ((unsigned)((sv = state[p]) >> 32) != epoch) {}
-      base += (int)(unsigned)(sv & 0xffffffffULL);
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) base += __shfl_xor_sync(0xffffffffu, base, o);
-    if (lane == 0) {
-      s_base = base;
-      if (blockIdx.x == gridDim.x - 1) *total = base + block_total;
-    }
-  }
-  __syncthreads();
+  const int r = block_rank(flag, chunk_state, epoch, total);
   if (flag) {
-    const size_t pos = (size_t)(s_base + (wid > 0 ? warp_sums[wid - 1] : 0) + v - 1);
+    const size_t pos = (size_t)r;
     if (pos < cap) {
       float* o = out + (3 + F) * pos;
       o[0] = f.x; o[1] = f.y; o[2] = f.z;
@@ -254,72 +218,31 @@ constexpr int kGridBoxThreads = 256;
 constexpr int kGridWarps = 4;                  // warps per centroid block
 constexpr int kGridItems = 4;                  // points per lane per round of a centroid warp
 constexpr int kGridChunk = 32 * kGridItems;    // points staged per round
-// box state words: [0..2] ~enc(min g), [3..5] enc(max g) (all reduced with unsigned max, zero = empty), [6] kept count,
-// [7] a kept cell outside the int range, [8] surviving voxels m
+// state words: [0..7] the box of the kept points' cells (kBoxWords) with the kept count in [6] and a kept cell outside the int
+// range in [7], [8] surviving voxels m
 constexpr int kGridState = 9;
-
-__host__ __device__ inline unsigned grid_enc(int g) { return (unsigned)g ^ 0x80000000u; }  // order-preserving int -> unsigned
-__host__ __device__ inline int grid_dec(unsigned u) { return (int)(u ^ 0x80000000u); }
-
-// 0: dropped (non-finite, or near the origin when filtering), 1: kept with cells g, 2: kept but a cell outside the int range
-__device__ __forceinline__ int grid_cell(float x, float y, float z, float inv, int filter, int g[3]) {
-  if (!(isfinite(x) && isfinite(y) && isfinite(z))) return 0;
-  if (filter && __fadd_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)), __fmul_rn(z, z)) < 1e-3f) return 0;
-  const float c[3] = {floorf(__fmul_rn(x, inv)), floorf(__fmul_rn(y, inv)), floorf(__fmul_rn(z, inv))};
-#pragma unroll
-  for (int a = 0; a < 3; a++) {
-    if (!(c[a] >= -2147483648.0f && c[a] < 2147483648.0f)) return 2;
-    g[a] = (int)c[a];
-  }
-  return 1;
-}
 
 __global__ void __launch_bounds__(kGridBoxThreads) k_grid_box(const float* __restrict__ in, size_t stride_f, int n, float inv, int filter, float4* __restrict__ pts4,
                                                               unsigned* __restrict__ st) {
-  __shared__ unsigned sh[8];
-  if (threadIdx.x < 8) sh[threadIdx.x] = 0;
-  __syncthreads();
   unsigned mx[6] = {0, 0, 0, 0, 0, 0}, kept = 0, bad = 0;
   for (int i = blockIdx.x * kGridBoxThreads + threadIdx.x; i < n; i += gridDim.x * kGridBoxThreads) {
     const float* p = in + (size_t)i * stride_f;
     const float x = p[0], y = p[1], z = p[2];
     pts4[i] = make_float4(x, y, z, 0.f);
     int g[3];
-    const int s = grid_cell(x, y, z, inv, filter, g);
+    const int s = cell_of(x, y, z, inv, filter, g);
     kept += s != 0;
     bad |= s == 2;
-    if (s == 1) {
-#pragma unroll
-      for (int a = 0; a < 3; a++) {
-        mx[a] = max(mx[a], ~grid_enc(g[a]));
-        mx[3 + a] = max(mx[3 + a], grid_enc(g[a]));
-      }
-    }
+    if (s == 1) box_add(mx, g);
   }
-  const unsigned full = 0xffffffffu;
-#pragma unroll
-  for (int a = 0; a < 6; a++) mx[a] = __reduce_max_sync(full, mx[a]);
-  kept = __reduce_add_sync(full, kept);
-  bad = __reduce_or_sync(full, bad);
-  if ((threadIdx.x & 31) == 0) {
-#pragma unroll
-    for (int a = 0; a < 6; a++) atomicMax(&sh[a], mx[a]);
-    atomicAdd(&sh[6], kept);
-    atomicOr(&sh[7], bad);
-  }
-  __syncthreads();
-  if (threadIdx.x < 6) atomicMax(&st[threadIdx.x], sh[threadIdx.x]);
-  else if (threadIdx.x == 6) atomicAdd(&st[6], sh[6]);
-  else if (threadIdx.x == 7) atomicOr(&st[7], sh[7]);
+  box_flush(mx, kept, bad, st);
 }
 
 // key of every point (voxel index, or V for a dropped one) and the digit counts of all sort passes
 __global__ void __launch_bounds__(vgicp::kSortThreads) k_grid_keys(const float4* __restrict__ pts4, int n, float inv, int filter, int3 min_b, unsigned div_x, unsigned div_xy,
                                                                    unsigned dropped_key, int passes, unsigned* __restrict__ keys, unsigned* __restrict__ hist) {
-  using namespace vgicp;
   __shared__ unsigned sh[kSortMaxPasses * kSortBins];
-  for (int i = threadIdx.x; i < passes * kSortBins; i += kSortThreads) sh[i] = 0;
-  __syncthreads();
+  sort_hist_zero(sh, passes);
   const int n_round = (n + 31) & ~31;
   for (int i = blockIdx.x * kSortThreads + threadIdx.x; i < n_round; i += gridDim.x * kSortThreads) {  // warp-uniform trip count
     const bool valid = i < n;
@@ -327,26 +250,21 @@ __global__ void __launch_bounds__(vgicp::kSortThreads) k_grid_keys(const float4*
     if (valid) {
       const float4 p = pts4[i];
       int g[3];
-      if (grid_cell(p.x, p.y, p.z, inv, filter, g) == 1)
+      if (cell_of(p.x, p.y, p.z, inv, filter, g) == 1)
         key = ((unsigned)g[0] - (unsigned)min_b.x) + ((unsigned)g[1] - (unsigned)min_b.y) * div_x + ((unsigned)g[2] - (unsigned)min_b.z) * div_xy;
       keys[i] = key;
     }
     sort_hist_add(sh, passes, valid, key);
   }
-  __syncthreads();
-  for (int i = threadIdx.x; i < passes * kSortBins; i += kSortThreads)
-    if (sh[i]) atomicAdd(&hist[i], sh[i]);
+  sort_hist_flush(sh, passes, hist);
 }
 
 // the sorted positions that start a voxel reaching the minimum (the run of equal keys starting at p is at least min_points long iff
-// key[p + min_points - 1] is still p's key), ranked in key order: vstart[rank] = p, st[8] = their number.  One block per 1024 of the
-// kept points' positions, decoupled look-back over epoch-tagged block totals as in k_prep_scatter.
-__global__ void __launch_bounds__(1024) k_grid_heads(const unsigned* __restrict__ keys, int kept, unsigned min_points, unsigned long long* chunk_state, unsigned epoch,
-                                                     int* __restrict__ vstart, unsigned* __restrict__ st) {
-  __shared__ int warp_sums[32];
-  __shared__ int s_base;
-  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  const int p = blockIdx.x * 1024 + tid;
+// key[p + min_points - 1] is still p's key), ranked in key order by block_rank: vstart[rank] = p, st[8] = their number.  One block
+// per kRankThreads of the kept points' positions.
+__global__ void __launch_bounds__(kRankThreads) k_grid_heads(const unsigned* __restrict__ keys, int kept, unsigned min_points, unsigned long long* chunk_state, unsigned epoch,
+                                                             int* __restrict__ vstart, unsigned* __restrict__ st) {
+  const int p = blockIdx.x * kRankThreads + threadIdx.x;
   int flag = 0;
   if (p < kept) {
     const unsigned k = keys[p];
@@ -356,43 +274,8 @@ __global__ void __launch_bounds__(1024) k_grid_heads(const unsigned* __restrict_
       flag = q < kept && keys[q] == k;
     }
   }
-  int v = flag;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    int t = __shfl_up_sync(0xffffffffu, v, o);
-    if (lane >= o) v += t;
-  }
-  if (lane == 31) warp_sums[wid] = v;
-  __syncthreads();
-  if (wid == 0) {
-    int w = warp_sums[lane];
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      int t = __shfl_up_sync(0xffffffffu, w, o);
-      if (lane >= o) w += t;
-    }
-    warp_sums[lane] = w;
-    const int block_total = __shfl_sync(0xffffffffu, w, 31);
-    volatile unsigned long long* state = chunk_state;
-    if (lane == 0) {
-      state[blockIdx.x] = ((unsigned long long)epoch << 32) | (unsigned)block_total;
-      __threadfence();
-    }
-    int base = 0;
-    for (int b = (int)blockIdx.x - 1 - lane; b >= 0; b -= 32) {
-      unsigned long long sv;
-      while ((unsigned)((sv = state[b]) >> 32) != epoch) {}
-      base += (int)(unsigned)(sv & 0xffffffffULL);
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) base += __shfl_xor_sync(0xffffffffu, base, o);
-    if (lane == 0) {
-      s_base = base;
-      if (blockIdx.x == gridDim.x - 1) st[8] = (unsigned)(base + block_total);
-    }
-  }
-  __syncthreads();
-  if (flag) vstart[s_base + (wid > 0 ? warp_sums[wid - 1] : 0) + v - 1] = p;
+  const int r = block_rank(flag, chunk_state, epoch, reinterpret_cast<int*>(st + 8));
+  if (flag) vstart[r] = p;
 }
 
 // One round of a centroid warp: the run's points among sorted positions base ... base + kGridChunk - 1, x y z and the F fields of
@@ -465,27 +348,6 @@ __global__ void __launch_bounds__(kGridWarps * 32, 1) k_grid_centroids(const uns
     if (lane < R) out[(size_t)r * R + lane] = __fdiv_rn(s, (float)count);
   }
 }
-
-template <typename T>
-struct DevBuf {  // grow-only device array
-  T* p = nullptr;
-  size_t cap = 0;
-  cudaError_t reserve(size_t n) {
-    if (n <= cap) return cudaSuccess;
-    if (p) cudaFree(p);
-    p = nullptr;
-    cap = 0;
-    const size_t want = n + n / 4 + 16;
-    cudaError_t e = cudaMalloc(&p, want * sizeof(T));
-    if (e == cudaSuccess) cap = want;
-    return e;
-  }
-  void release() {
-    if (p) cudaFree(p);
-    p = nullptr;
-    cap = 0;
-  }
-};
 
 }  // namespace
 
@@ -589,7 +451,7 @@ cudaError_t launch_filter(vgicp_prep_handle h, const float* d_in, size_t stride_
   const cudaError_t e = cudaMemsetAsync(h->flushed.p, 0, (size_t)ni * sizeof(float4), h->stream);
   if (e != cudaSuccess) return e;
   k_prep_walk<F><<<1, kHist, 0, h->stream>>>(h->pts4.p, h->entry.p, ni, inv_leaf, h->flushed.p, h->tail, fa);
-  k_prep_scatter<F><<<chunks, 1024, 0, h->stream>>>(h->flushed.p, ni, d_out, out_cap, h->chunk_state.p, h->chunk_epoch, h->d_counts, h->fflushed.p);
+  k_prep_scatter<F><<<chunks, kRankThreads, 0, h->stream>>>(h->flushed.p, ni, d_out, out_cap, h->chunk_state.p, h->chunk_epoch, h->d_counts, h->fflushed.p);
   k_prep_tail<F><<<1, kHist, 0, h->stream>>>(h->tail, h->d_counts, d_out, out_cap, h->d_counts + 1, h->ftail.p);
   return cudaGetLastError();
 }
@@ -603,22 +465,6 @@ cudaError_t stage_input(vgicp_prep_handle h, const float* points, size_t n, size
   cudaError_t e = h->staging.reserve(n * stride_bytes);
   if (e == cudaSuccess) e = cudaMemcpyAsync(h->staging.p, points, (n - 1) * stride_bytes + span, cudaMemcpyHostToDevice, h->stream);
   *d_in = reinterpret_cast<const float*>(h->staging.p);
-  return e;
-}
-
-// a fresh epoch for the look-back state of `chunks` blocks (cleared when newly allocated or when the epoch wraps)
-cudaError_t next_chunk_epoch(vgicp_prep_handle h, int chunks) {
-  const unsigned long long* before = h->chunk_state.p;
-  cudaError_t e = h->chunk_state.reserve((size_t)chunks);
-  if (e != cudaSuccess) return e;
-  if (h->chunk_state.p != before) {  // fresh allocation: no stale epoch may match
-    e = cudaMemsetAsync(h->chunk_state.p, 0, h->chunk_state.cap * sizeof(unsigned long long), h->stream);
-    h->chunk_epoch = 0;
-  }
-  if (e == cudaSuccess && ++h->chunk_epoch == 0) {
-    e = cudaMemsetAsync(h->chunk_state.p, 0, h->chunk_state.cap * sizeof(unsigned long long), h->stream);
-    h->chunk_epoch = 1;
-  }
   return e;
 }
 
@@ -644,8 +490,8 @@ int run_filter(vgicp_prep_handle h, const char* who, const float* points, size_t
     PREP_TRY(h, h->out.reserve(rec * n));
     d_out = h->out.p;
   }
-  const int chunks = (ni + 1023) / 1024;
-  PREP_TRY(h, next_chunk_epoch(h, chunks));
+  const int chunks = (ni + kRankThreads - 1) / kRankThreads;
+  PREP_TRY(h, lookback_next(h->chunk_state, h->chunk_epoch, chunks, h->stream));
   const float inv_leaf = 1.0f / leaf;
   const size_t sf = stride_bytes / 4;
   const int flt = remove_near_origin ? 1 : 0;
@@ -685,7 +531,6 @@ cudaError_t launch_centroids(vgicp_prep_handle h, const float* d_in, size_t stri
 
 int run_voxel_grid(vgicp_prep_handle h, const float* points, size_t n, size_t stride_bytes, int on_device, float leaf, int remove_near_origin, const int* off, int F,
                    unsigned min_points, float* out, size_t cap, int out_on_device, size_t* n_out) {
-  using namespace vgicp;
   const size_t rec = 3 + (size_t)F;
   PREP_TRY(h, cudaSetDevice(h->device));
   const int ni = (int)n;
@@ -713,8 +558,8 @@ int run_voxel_grid(vgicp_prep_handle h, const float* points, size_t n, size_t st
   int lo[3];
   long long div[3];
   for (int a = 0; a < 3; a++) {
-    lo[a] = grid_dec(~h->h_grid[a]);
-    div[a] = (long long)grid_dec(h->h_grid[3 + a]) - lo[a] + 1;
+    lo[a] = cell_dec(~h->h_grid[a]);
+    div[a] = (long long)cell_dec(h->h_grid[3 + a]) - lo[a] + 1;
   }
   const long long lim = 0x7fffffff;
   if (div[0] > lim || div[1] > lim / div[0] || div[2] > lim / (div[0] * div[1]))
@@ -735,10 +580,10 @@ int run_voxel_grid(vgicp_prep_handle h, const float* points, size_t n, size_t st
                                           h->stream));
   const unsigned* keys = h->gkeys[passes & 1].p;
   // 3. the voxels that reach the minimum, ranked; 4. their centroids
-  const int chunks = (kept + 1023) / 1024;
-  PREP_TRY(h, next_chunk_epoch(h, chunks));
+  const int chunks = (kept + kRankThreads - 1) / kRankThreads;
+  PREP_TRY(h, lookback_next(h->chunk_state, h->chunk_epoch, chunks, h->stream));
   PREP_TRY(h, h->gvstart.reserve((size_t)kept));
-  k_grid_heads<<<chunks, 1024, 0, h->stream>>>(keys, kept, min_points, h->chunk_state.p, h->chunk_epoch, h->gvstart.p, h->d_grid);
+  k_grid_heads<<<chunks, kRankThreads, 0, h->stream>>>(keys, kept, min_points, h->chunk_state.p, h->chunk_epoch, h->gvstart.p, h->d_grid);
   PREP_TRY(h, cudaGetLastError());
   float* d_out = out;
   size_t out_cap = cap;

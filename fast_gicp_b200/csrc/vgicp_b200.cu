@@ -27,56 +27,6 @@ using namespace vgicp;
 
 namespace {
 
-template <typename T>
-struct DevBuf {  // grow-only device array
-  T* p = nullptr;
-  size_t cap = 0;
-  bool external = false;  // points into memory owned elsewhere (the multi-GPU exchange arena): fixed capacity, never freed here
-  cudaError_t reserve(size_t n) {
-    if (n <= cap) return cudaSuccess;
-    if (external) return cudaErrorMemoryAllocation;
-    if (p) cudaFree(p);
-    p = nullptr;
-    cap = 0;
-    size_t want = n + n / 4 + 16;
-    cudaError_t e = cudaMalloc(&p, want * sizeof(T));
-    if (e == cudaSuccess) cap = want;
-    return e;
-  }
-  // reserve that keeps the first `keep` elements: copied in stream order on `st`; the old array is freed once `st` has drained,
-  // since work enqueued there may still read it
-  cudaError_t grow(size_t n, size_t keep, cudaStream_t st) {
-    if (n <= cap) return cudaSuccess;
-    if (external) return cudaErrorMemoryAllocation;
-    const size_t want = n + n / 4 + 16;
-    T* q = nullptr;
-    cudaError_t e = cudaMalloc(&q, want * sizeof(T));
-    if (e != cudaSuccess) return e;
-    if (keep) e = cudaMemcpyAsync(q, p, keep * sizeof(T), cudaMemcpyDeviceToDevice, st);
-    if (e == cudaSuccess && p) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) {
-      cudaFree(q);
-      return e;
-    }
-    if (p) cudaFree(p);
-    p = q;
-    cap = want;
-    return cudaSuccess;
-  }
-  void release() {
-    if (p && !external) cudaFree(p);
-    p = nullptr;
-    cap = 0;
-    external = false;
-  }
-  void attach(T* q, size_t capacity) {  // switch to external storage
-    release();
-    p = q;
-    cap = capacity;
-    external = true;
-  }
-};
-
 struct Cloud {
   DevBuf<float4> pts;
   DevBuf<int> nbr;
@@ -750,19 +700,10 @@ int voxelmap_finish(vgicp_handle h, Cloud& t, VoxelMap& m) {
     }
   }
   {
-    const int chunks = (B + 1023) / 1024;
-    const unsigned long long* before = m.chunk_state.p;
-    CU_TRY(h, m.chunk_state.reserve(chunks));
-    if (m.chunk_state.p != before) {  // fresh allocation: no stale epoch may match
-      CU_TRY(h, cudaMemsetAsync(m.chunk_state.p, 0, m.chunk_state.cap * sizeof(unsigned long long), t.st));
-      m.chunk_epoch = 0;
-    }
-    if (++m.chunk_epoch == 0) {  // wrapped: clear once and restart
-      CU_TRY(h, cudaMemsetAsync(m.chunk_state.p, 0, m.chunk_state.cap * sizeof(unsigned long long), t.st));
-      m.chunk_epoch = 1;
-    }
+    const int chunks = blocks_for(B, kRankThreads);
+    CU_TRY(h, lookback_next(m.chunk_state, m.chunk_epoch, chunks, t.st));
     KLAUNCH_ST(h, t.st, VGICP_PROF_VOXELMAP,
-               k_table_assign_ids<<<chunks, 1024, 0, t.st>>>(m.coords.p, m.slots.p, B, m.buckets.p, m.d_counters + 1, m.dense, m.chunk_state.p, m.chunk_epoch));
+               k_table_assign_ids<<<chunks, kRankThreads, 0, t.st>>>(m.coords.p, m.slots.p, B, m.buckets.p, m.d_counters + 1, m.dense, m.chunk_state.p, m.chunk_epoch));
   }
   // voxel Gaussians: stable sort of the points by voxel id, then one warp per voxel adds its points in index order
   {
@@ -2245,26 +2186,15 @@ int vgicp_append_source_to_target(vgicp_handle h, const double T[16]) {
 static int local_map_rank(vgicp_handle h, const unsigned char* keep, float cx, float cy, float cz, float r2, size_t* passed) {
   Cloud& t = h->target;
   const int n = t.n;
-  const int blocks = blocks_for(n, kCropThreads);
+  const int blocks = blocks_for(n, kRankThreads);
   CU_TRY(h, h->crop_rank.reserve(n));
-  {
-    const unsigned long long* before = h->crop_state.p;
-    CU_TRY(h, h->crop_state.reserve(blocks));
-    if (h->crop_state.p != before) {  // fresh allocation: no stale epoch may match
-      CU_TRY(h, cudaMemsetAsync(h->crop_state.p, 0, h->crop_state.cap * sizeof(unsigned long long), t.st));
-      h->crop_epoch = 0;
-    }
-    if (++h->crop_epoch == 0) {  // wrapped: clear once and restart
-      CU_TRY(h, cudaMemsetAsync(h->crop_state.p, 0, h->crop_state.cap * sizeof(unsigned long long), t.st));
-      h->crop_epoch = 1;
-    }
-  }
+  CU_TRY(h, lookback_next(h->crop_state, h->crop_epoch, blocks, t.st));
   CU_TRY(h, h->spare_pts.reserve(n));
   CU_TRY(h, h->spare_covA.reserve(n));
   CU_TRY(h, h->spare_covB.reserve(n));
   int* d_count = h->map.d_counters + 10;
   KLAUNCH_ST(h, t.st, VGICP_PROF_OTHER,
-             k_crop_rank<<<blocks, kCropThreads, 0, t.st>>>(t.pts.p, keep, n, cx, cy, cz, r2, h->crop_rank.p, d_count, h->crop_state.p, h->crop_epoch));
+             k_crop_rank<<<blocks, kRankThreads, 0, t.st>>>(t.pts.p, keep, n, cx, cy, cz, r2, h->crop_rank.p, d_count, h->crop_state.p, h->crop_epoch));
   CU_TRY(h, cudaGetLastError());
   // the host needs the new size (and must refuse an empty result before anything is modified)
   CU_TRY(h, cudaMemcpyAsync(h->map.h_counters + 10, d_count, sizeof(int), cudaMemcpyDeviceToHost, t.st));
@@ -2320,19 +2250,19 @@ int vgicp_thin_target(vgicp_handle h, double leaf_size, int max_points_per_voxel
   const int n = t.n;
   if (n == 0) return fail(h, VGICP_ERR_BAD_STATE, "thin_target: the target has no points");
   // 1. the box of the cells, read back: the refusals and the key width are decided before anything is modified
-  CU_TRY(h, h->thin_box.reserve(kThinBoxWords));
-  CU_TRY(h, cudaMemsetAsync(h->thin_box.p, 0, kThinBoxWords * sizeof(unsigned), t.st));
+  CU_TRY(h, h->thin_box.reserve(kBoxWords));
+  CU_TRY(h, cudaMemsetAsync(h->thin_box.p, 0, kBoxWords * sizeof(unsigned), t.st));
   const int bb = blocks_for(n, kThinBoxThreads);
   KLAUNCH_ST(h, t.st, VGICP_PROF_OTHER, k_thin_box<<<bb < 4 * kNumSMs ? bb : 4 * kNumSMs, kThinBoxThreads, 0, t.st>>>(t.pts.p, n, inv, h->thin_box.p));
   CU_TRY(h, cudaGetLastError());
-  unsigned box[kThinBoxWords];
+  unsigned box[kBoxWords];
   CU_TRY(h, cudaMemcpyAsync(box, h->thin_box.p, sizeof(box), cudaMemcpyDeviceToHost, t.st));
   CU_TRY(h, cudaStreamSynchronize(t.st));
   if (box[6]) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "thin_target: a target point has a non-finite coordinate");
   if (box[7]) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "thin_target: a cell floor(p * (1 / leaf)) lies outside [-2^31, 2^31)");
   int lo[3], bits[3];
   for (int a = 0; a < 3; a++) {
-    lo[a] = thin_dec(~box[a]);
+    lo[a] = cell_dec(~box[a]);
     const unsigned span = box[3 + a] - ~box[a];  // max - min
     bits[a] = span ? 32 - __builtin_clz(span) : 0;
   }

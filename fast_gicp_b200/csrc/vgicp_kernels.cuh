@@ -23,6 +23,7 @@
 #include <type_traits>
 
 #include "vgicp_deskew.cuh"
+#include "vgicp_scan.cuh"
 #include "vgicp_sort.cuh"
 #include "vgicp_stage1.cuh"
 
@@ -241,55 +242,14 @@ __global__ void k_table_lookup_points(const int4* __restrict__ coords, int n, co
   if (found < 0) atomicAdd(fail_counter, 1);
 }
 
-// voxel id = rank of the slot among occupied slots; buckets = {coord, id} or {0,0,0,-1} (voxel_coord_select_kernel :61-73).
-// One block per 1024 buckets: block scan, then a decoupled look-back over the totals the preceding blocks publish in
-// chunk_state (epoch << 32 | total; the epoch changes every launch, so the array never needs clearing).  A block only ever
-// waits for blocks with a smaller index, which the hardware scheduled before it.
-__global__ void __launch_bounds__(1024) k_table_assign_ids(const int4* __restrict__ coords, const int* __restrict__ slots, int num_buckets, int4* __restrict__ buckets,
-                                                          int* __restrict__ num_voxels, const DenseIndex dense, unsigned long long* chunk_state, unsigned epoch) {
-  __shared__ int warp_sums[32];
-  __shared__ int s_base;
-  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  const int b = blockIdx.x * 1024 + tid;
+// voxel id = rank of the slot among occupied slots (block_rank); buckets = {coord, id} or {0,0,0,-1} (voxel_coord_select_kernel
+// :61-73).  One block per kRankThreads buckets.
+__global__ void __launch_bounds__(kRankThreads) k_table_assign_ids(const int4* __restrict__ coords, const int* __restrict__ slots, int num_buckets, int4* __restrict__ buckets,
+                                                                   int* __restrict__ num_voxels, const DenseIndex dense, unsigned long long* chunk_state, unsigned epoch) {
+  const int b = blockIdx.x * kRankThreads + threadIdx.x;
   const int r = b < num_buckets ? slots[b] : -1;
   const int flag = r >= 0 ? 1 : 0;
-  int v = flag;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    int t = __shfl_up_sync(0xffffffffu, v, o);
-    if (lane >= o) v += t;
-  }
-  if (lane == 31) warp_sums[wid] = v;
-  __syncthreads();
-  if (wid == 0) {
-    int w = warp_sums[lane];
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      int t = __shfl_up_sync(0xffffffffu, w, o);
-      if (lane >= o) w += t;
-    }
-    warp_sums[lane] = w;
-    const int total = __shfl_sync(0xffffffffu, w, 31);
-    volatile unsigned long long* state = chunk_state;
-    if (lane == 0) {
-      state[blockIdx.x] = ((unsigned long long)epoch << 32) | (unsigned)total;
-      __threadfence();
-    }
-    int base = 0;  // lanes split the predecessors
-    for (int p = (int)blockIdx.x - 1 - lane; p >= 0; p -= 32) {
-      unsigned long long sv;
-      while ((unsigned)((sv = state[p]) >> 32) != epoch) {}
-      base += (int)(unsigned)(sv & 0xffffffffULL);
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) base += __shfl_xor_sync(0xffffffffu, base, o);
-    if (lane == 0) {
-      s_base = base;
-      if (blockIdx.x == gridDim.x - 1) *num_voxels = base + total;
-    }
-  }
-  __syncthreads();
-  const int prefix = s_base + (wid > 0 ? warp_sums[wid - 1] : 0) + v - flag;  // exclusive
+  const int prefix = block_rank(flag, chunk_state, epoch, num_voxels);
   if (b < num_buckets) {
     if (flag) {
       int4 c = coords[r];
@@ -311,8 +271,7 @@ __global__ void __launch_bounds__(1024) k_table_assign_ids(const int4* __restric
 __global__ void __launch_bounds__(kSortThreads) k_voxel_sort_keys(const int* __restrict__ slot_of_point, const int4* __restrict__ buckets, int n, unsigned invalid, int passes,
                                                                   unsigned* __restrict__ keys, unsigned* __restrict__ hist) {
   __shared__ unsigned sh[kSortMaxPasses * kSortBins];
-  for (int i = threadIdx.x; i < passes * kSortBins; i += kSortThreads) sh[i] = 0;
-  __syncthreads();
+  sort_hist_zero(sh, passes);
   const int n_round = (n + 31) & ~31;
   for (int i = blockIdx.x * kSortThreads + threadIdx.x; i < n_round; i += gridDim.x * kSortThreads) {
     const bool valid = i < n;
@@ -324,9 +283,7 @@ __global__ void __launch_bounds__(kSortThreads) k_voxel_sort_keys(const int* __r
     }
     sort_hist_add(sh, passes, valid, (unsigned long long)key);
   }
-  __syncthreads();
-  for (int i = threadIdx.x; i < passes * kSortBins; i += kSortThreads)
-    if (sh[i]) atomicAdd(&hist[i], sh[i]);
+  sort_hist_flush(sh, passes, hist);
 }
 
 // [start, end) of every voxel in the sorted list

@@ -1,14 +1,12 @@
 // vgicp_local_map.cuh -- kernels of the local-map operations (vgicp_append_source_to_target, vgicp_thin_target,
 // vgicp_crop_target): the target cloud grows by the registered source and is compacted by a voxel cap and a crop, all in place on
 // the device, so that scan-to-map odometry never moves the map over PCIe.  Included after vgicp_kernels.cuh (Pose,
-// transform_point, vgicp_sort.cuh).  The arithmetic the header documents is spelled as IEEE single operations (__f*_rn): this
+// transform_point, vgicp_scan.cuh, vgicp_sort.cuh).  The arithmetic the header documents is spelled as IEEE single operations (__f*_rn): this
 // unit is compiled with contraction on.
 #pragma once
 #include <cuda_runtime.h>
 
 namespace vgicp {
-
-constexpr int kCropThreads = 1024;  // points per block of the crop's scan (one look-back state word per block)
 
 // Appended row i: point = transform_point(T, a_i), the bytes vgicp_transform_source returns; covariance = R C_i R^T with
 //   M_ik = (R_i0 C_0k + R_i1 C_1k) + R_i2 C_2k,   N_ij = (M_i0 R_j0 + M_i1 R_j1) + M_i2 R_j2,
@@ -38,16 +36,10 @@ __global__ void k_append_transformed(const float4* __restrict__ src_pts, const f
 }
 
 // Crop, pass 1: point i passes when d^2 = (dx dx + dy dy) + dz dz <= r2 (dx = p.x - c.x, ...) and, when `keep` is given,
-// keep[i] != 0; rank[i] = number of passing points before i, or -1.  The total lands in *count.  Block scan, then the decoupled
-// look-back of k_table_assign_ids over the totals the preceding blocks publish in `state` (epoch << 32 | total; the epoch changes
-// every launch, so the array never needs clearing).  A block only ever waits for blocks with a smaller index, which the hardware
-// scheduled before it.
-__global__ void __launch_bounds__(kCropThreads) k_crop_rank(const float4* __restrict__ pts, const unsigned char* __restrict__ keep, int n, float cx, float cy, float cz,
+// keep[i] != 0; rank[i] = number of passing points before i (block_rank), or -1.  The total lands in *count.
+__global__ void __launch_bounds__(kRankThreads) k_crop_rank(const float4* __restrict__ pts, const unsigned char* __restrict__ keep, int n, float cx, float cy, float cz,
                                                             float r2, int* __restrict__ rank, int* __restrict__ count, unsigned long long* state_words, unsigned epoch) {
-  __shared__ int warp_sums[32];
-  __shared__ int s_base;
-  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  const int i = blockIdx.x * kCropThreads + tid;
+  const int i = blockIdx.x * kRankThreads + threadIdx.x;
   int flag = 0;
   if (i < n) {
     const float4 p = pts[i];
@@ -55,43 +47,8 @@ __global__ void __launch_bounds__(kCropThreads) k_crop_rank(const float4* __rest
     const float d2 = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
     flag = d2 <= r2 && (!keep || keep[i]) ? 1 : 0;
   }
-  int v = flag;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int t = __shfl_up_sync(0xffffffffu, v, o);
-    if (lane >= o) v += t;
-  }
-  if (lane == 31) warp_sums[wid] = v;
-  __syncthreads();
-  if (wid == 0) {
-    int w = warp_sums[lane];
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int t = __shfl_up_sync(0xffffffffu, w, o);
-      if (lane >= o) w += t;
-    }
-    warp_sums[lane] = w;
-    const int total = __shfl_sync(0xffffffffu, w, 31);
-    volatile unsigned long long* state = state_words;
-    if (lane == 0) {
-      state[blockIdx.x] = ((unsigned long long)epoch << 32) | (unsigned)total;
-      __threadfence();
-    }
-    int base = 0;  // lanes split the predecessors
-    for (int p = (int)blockIdx.x - 1 - lane; p >= 0; p -= 32) {
-      unsigned long long sv;
-      while ((unsigned)((sv = state[p]) >> 32) != epoch) {}
-      base += (int)(unsigned)(sv & 0xffffffffULL);
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) base += __shfl_xor_sync(0xffffffffu, base, o);
-    if (lane == 0) {
-      s_base = base;
-      if (blockIdx.x == gridDim.x - 1) *count = base + total;
-    }
-  }
-  __syncthreads();
-  if (i < n) rank[i] = flag ? s_base + (wid > 0 ? warp_sums[wid - 1] : 0) + v - 1 : -1;
+  const int r = block_rank(flag, state_words, epoch, count);
+  if (i < n) rank[i] = flag ? r : -1;
 }
 
 // Crop, pass 2: passing point i with rank r >= first goes to row r - first of the output arrays (stable compaction of the newest
@@ -111,58 +68,20 @@ __global__ void k_crop_scatter(const float4* __restrict__ pts, const float4* __r
 // sorted stably by a u64 cell key, so the rows of one cell are contiguous and in array order; sorted position j is then kept iff
 // j < M or key[j - M] != key[j].  k_crop_rank with the resulting mask (and r2 = +inf) and k_crop_scatter compact the target.
 constexpr int kThinBoxThreads = 256;
-// box words: [0..2] ~enc(min c), [3..5] enc(max c) (unsigned max reductions, zero = empty), [6] a non-finite coordinate,
-// [7] a cell outside [-2^31, 2^31)
-constexpr int kThinBoxWords = 8;
 
-__host__ __device__ inline unsigned thin_enc(int c) { return (unsigned)c ^ 0x80000000u; }  // order-preserving int -> unsigned
-__host__ __device__ inline int thin_dec(unsigned u) { return (int)(u ^ 0x80000000u); }
-
-// 0: a coordinate is not finite, 1: cells in c, 2: a cell outside the int range
-__device__ __forceinline__ int thin_cell(float4 p, float inv, int c[3]) {
-  if (!(isfinite(p.x) && isfinite(p.y) && isfinite(p.z))) return 0;
-  const float f[3] = {floorf(__fmul_rn(p.x, inv)), floorf(__fmul_rn(p.y, inv)), floorf(__fmul_rn(p.z, inv))};
-#pragma unroll
-  for (int a = 0; a < 3; a++) {
-    if (!(f[a] >= -2147483648.0f && f[a] < 2147483648.0f)) return 2;
-    c[a] = (int)f[a];
-  }
-  return 1;
-}
-
-// one pass over the target: the cells' bounding box and the two refusal flags (st zeroed by the caller)
+// one pass over the target: the cells' box (kBoxWords), the number of non-finite points in word 6 and a cell outside
+// [-2^31, 2^31) in word 7 (st zeroed by the caller)
 __global__ void __launch_bounds__(kThinBoxThreads) k_thin_box(const float4* __restrict__ pts, int n, float inv, unsigned* __restrict__ st) {
-  __shared__ unsigned sh[kThinBoxWords];
-  if (threadIdx.x < kThinBoxWords) sh[threadIdx.x] = 0;
-  __syncthreads();
   unsigned mx[6] = {0, 0, 0, 0, 0, 0}, nonfinite = 0, range = 0;
   for (int i = blockIdx.x * kThinBoxThreads + threadIdx.x; i < n; i += gridDim.x * kThinBoxThreads) {
+    const float4 p = pts[i];
     int c[3];
-    const int s = thin_cell(pts[i], inv, c);
-    nonfinite |= s == 0;
+    const int s = cell_of(p.x, p.y, p.z, inv, 0, c);
+    nonfinite += s == 0;
     range |= s == 2;
-    if (s == 1) {
-#pragma unroll
-      for (int a = 0; a < 3; a++) {
-        mx[a] = max(mx[a], ~thin_enc(c[a]));
-        mx[3 + a] = max(mx[3 + a], thin_enc(c[a]));
-      }
-    }
+    if (s == 1) box_add(mx, c);
   }
-  const unsigned full = 0xffffffffu;
-#pragma unroll
-  for (int a = 0; a < 6; a++) mx[a] = __reduce_max_sync(full, mx[a]);
-  nonfinite = __reduce_or_sync(full, nonfinite);
-  range = __reduce_or_sync(full, range);
-  if ((threadIdx.x & 31) == 0) {
-#pragma unroll
-    for (int a = 0; a < 6; a++) atomicMax(&sh[a], mx[a]);
-    atomicOr(&sh[6], nonfinite);
-    atomicOr(&sh[7], range);
-  }
-  __syncthreads();
-  if (threadIdx.x < 6) atomicMax(&st[threadIdx.x], sh[threadIdx.x]);
-  else if (threadIdx.x < kThinBoxWords) atomicOr(&st[threadIdx.x], sh[threadIdx.x]);
+  box_flush(mx, nonfinite, range, st);
 }
 
 // key of every point, (c_x - min_x) | (c_y - min_y) << b_x | (c_z - min_z) << (b_x + b_y), and the digit counts of all sort passes
@@ -171,24 +90,22 @@ __global__ void __launch_bounds__(kThinBoxThreads) k_thin_box(const float4* __re
 __global__ void __launch_bounds__(kSortThreads) k_thin_keys(const float4* __restrict__ pts, int n, float inv, int3 lo, int sh_y, int sh_z, int passes,
                                                             unsigned long long* __restrict__ keys, unsigned* __restrict__ hist) {
   __shared__ unsigned sh[kSortMaxPasses * kSortBins];
-  for (int i = threadIdx.x; i < passes * kSortBins; i += kSortThreads) sh[i] = 0;
-  __syncthreads();
+  sort_hist_zero(sh, passes);
   const int n_round = (n + 31) & ~31;
   for (int i = blockIdx.x * kSortThreads + threadIdx.x; i < n_round; i += gridDim.x * kSortThreads) {  // warp-uniform trip count
     const bool valid = i < n;
     unsigned long long key = 0;
     if (valid) {
+      const float4 p = pts[i];
       int c[3];
-      thin_cell(pts[i], inv, c);
+      cell_of(p.x, p.y, p.z, inv, 0, c);
       const unsigned long long dy = (unsigned)c[1] - (unsigned)lo.y, dz = (unsigned)c[2] - (unsigned)lo.z;
       key = (unsigned long long)((unsigned)c[0] - (unsigned)lo.x) | (dy ? dy << sh_y : 0ull) | (dz ? dz << sh_z : 0ull);
       keys[i] = key;
     }
     sort_hist_add(sh, passes, valid, key);
   }
-  __syncthreads();
-  for (int i = threadIdx.x; i < passes * kSortBins; i += kSortThreads)
-    if (sh[i]) atomicAdd(&hist[i], sh[i]);
+  sort_hist_flush(sh, passes, hist);
 }
 
 // sorted position j is kept iff j < M or key[j - M] != key[j]; the flag goes to the point's original index (vals == nullptr: the

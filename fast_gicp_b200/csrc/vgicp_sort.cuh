@@ -32,13 +32,35 @@ inline size_t sort_scratch_bytes(int n, int passes) {
   return sizeof(unsigned) * ((size_t)kSortMaxPasses * kSortBins + 64 + (size_t)passes * sort_num_tiles(n) * kSortBins);
 }
 
+// The digit counts of a kSortThreads block in shared memory, sh[passes * kSortBins]: zeroed by the whole block before the first
+// count, and added to the global histograms `hist` by the whole block after the last one
+__device__ __forceinline__ void sort_hist_zero(unsigned* sh, int passes) {
+  for (int i = threadIdx.x; i < passes * kSortBins; i += kSortThreads) sh[i] = 0;
+  __syncthreads();
+}
+__device__ __forceinline__ void sort_hist_flush(const unsigned* sh, int passes, unsigned* __restrict__ hist) {
+  __syncthreads();
+  for (int i = threadIdx.x; i < passes * kSortBins; i += kSortThreads)
+    if (sh[i]) atomicAdd(&hist[i], sh[i]);
+}
+
+// histogram accumulation for kernels that produce the keys themselves (stage 1 computes the Morton codes and their digit counts
+// in one pass): call with all 32 lanes between sort_hist_zero and sort_hist_flush
+__device__ __forceinline__ void sort_hist_add(unsigned* sh, int passes, bool valid, unsigned long long key) {
+  const int lane = threadIdx.x & 31;
+  for (int p = 0; p < passes; p++) {
+    const unsigned d = valid ? (unsigned)((key >> (p * kSortRadixBits)) & (unsigned long long)(kSortBins - 1)) : (unsigned)kSortBins + lane;
+    const unsigned peers = __match_any_sync(0xffffffffu, d);
+    if (valid && lane == __ffs(peers) - 1) atomicAdd(&sh[p * kSortBins + d], (unsigned)__popc(peers));
+  }
+}
+
 // digit counts of every pass in one sweep over the keys; lanes with equal digits elect one to add for all (the inputs are
 // spatially coherent: most lanes of a warp share their high digits)
 template <typename KeyT>
 __global__ void __launch_bounds__(kSortThreads) k_sort_hist(const KeyT* __restrict__ keys, int n, int passes, unsigned* __restrict__ hist) {
   __shared__ unsigned sh[kSortMaxPasses * kSortBins];
-  for (int i = threadIdx.x; i < passes * kSortBins; i += kSortThreads) sh[i] = 0;
-  __syncthreads();
+  sort_hist_zero(sh, passes);
   const int lane = threadIdx.x & 31;
   const int n_round = (n + 31) & ~31;
   for (int i = blockIdx.x * kSortThreads + threadIdx.x; i < n_round; i += gridDim.x * kSortThreads) {  // warp-uniform trip count
@@ -50,20 +72,7 @@ __global__ void __launch_bounds__(kSortThreads) k_sort_hist(const KeyT* __restri
       if (valid && lane == __ffs(peers) - 1) atomicAdd(&sh[p * kSortBins + d], (unsigned)__popc(peers));
     }
   }
-  __syncthreads();
-  for (int i = threadIdx.x; i < passes * kSortBins; i += kSortThreads)
-    if (sh[i]) atomicAdd(&hist[i], sh[i]);
-}
-
-// histogram accumulation for kernels that produce the keys themselves (stage 1 computes the Morton codes and their digit counts
-// in one pass): call with all 32 lanes, then flush after a __syncthreads
-__device__ __forceinline__ void sort_hist_add(unsigned* sh, int passes, bool valid, unsigned long long key) {
-  const int lane = threadIdx.x & 31;
-  for (int p = 0; p < passes; p++) {
-    const unsigned d = valid ? (unsigned)((key >> (p * kSortRadixBits)) & (unsigned long long)(kSortBins - 1)) : (unsigned)kSortBins + lane;
-    const unsigned peers = __match_any_sync(0xffffffffu, d);
-    if (valid && lane == __ffs(peers) - 1) atomicAdd(&sh[p * kSortBins + d], (unsigned)__popc(peers));
-  }
+  sort_hist_flush(sh, passes, hist);
 }
 
 // shared memory of one scatter tile

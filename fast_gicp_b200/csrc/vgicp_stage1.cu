@@ -500,8 +500,7 @@ __device__ __forceinline__ int shared_level(unsigned long long a, unsigned long 
 // Morton codes of the finest cells + the digit histograms of the sort
 __global__ void __launch_bounds__(kSortThreads) k_grid_codes(GridArgs a, int passes, unsigned* __restrict__ hist) {
   __shared__ unsigned sh[kSortMaxPasses * kSortBins];
-  for (int i = threadIdx.x; i < passes * kSortBins; i += kSortThreads) sh[i] = 0;
-  __syncthreads();
+  sort_hist_zero(sh, passes);
   const GridGeom g = grid_geom(a.bbox_min, a.bbox_max, a.L);
   const int n_round = (a.n + 31) & ~31;
   for (int i = blockIdx.x * kSortThreads + threadIdx.x; i < n_round; i += gridDim.x * kSortThreads) {
@@ -515,9 +514,7 @@ __global__ void __launch_bounds__(kSortThreads) k_grid_codes(GridArgs a, int pas
     }
     sort_hist_add(sh, passes, valid, code);
   }
-  __syncthreads();
-  for (int i = threadIdx.x; i < passes * kSortBins; i += kSortThreads)
-    if (sh[i]) atomicAdd(&hist[i], sh[i]);
+  sort_hist_flush(sh, passes, hist);
 }
 
 // cells per level (from the sorted codes) -> the finest level whose cells, together with all coarser ones, fit half the table

@@ -1,6 +1,7 @@
 #!/bin/bash
 # compute-sanitizer passes over the hot path: memcheck + racecheck + synccheck on one full registration per neighbour mode,
-# and on both k-NN search paths.  One log per tool, written by the loop at the end.
+# on both k-NN search paths, and on all four users of the shared block rank (voxel ids, crop and thinning, both voxel grids).
+# One log per tool, written by the loop at the end.
 set -u
 cat > /tmp/san_driver.py <<'PY'
 import sys, numpy as np
@@ -39,12 +40,14 @@ c.set_resolution(0.5); c.set_neighbor_search_method("DIRECT1")
 r = c.register(bt, bs)
 print("stream", len(bs), "converged", bool(r.converged))
 c.close()
-# local map: append the registered source (the target's arrays grow with a device copy), crop it (scan + look-back, compaction)
+# local map: append the registered source (the target's arrays grow with a device copy), thin it (cell box, u64 keys and sort,
+# keep mask), crop it (block rank, compaction)
 c = Core(0)
 c.set_neighbor_search_method("DIRECT7")
 r = c.register(tgt, src)
 from fast_gicp_b200.core import pose_from_c
 c.append_source_to_target(pose_from_c(r.T))
+c.thin_target(0.5, 2)
 c.crop_target((0.0, 0.0, 0.0), 30.0, len(tgt))
 r = c.align(pose_from_c(r.T))
 print("local map", c.num_target_points(), "converged", bool(r.converged))
@@ -85,6 +88,9 @@ c.deskew_source_stored([0.0, 0.0, 0.35, 8.0, 0.0, 0.0])
 c.find_source_neighbors(20); c.calculate_source_covariances(3)
 r = c.align_ct(np.eye(4), np.zeros(6), np.zeros(6), np.full(6, 1e-3))
 print("raw scan", m, "points, ct converged", bool(r.converged))
+# the exact voxel grid with fields and a minimum count (k_grid_box, k_grid_keys and the sort, k_grid_heads, k_grid_centroids)
+g = p.voxel_grid(torch.from_numpy(rec).cuda(), 0.25, [4, 3], 2)
+print("voxel grid", g.shape[0], "voxels of >= 2 points")
 c.close(); p.close()
 # NDT D2D through the same evaluation kernels
 c = Core(0)
