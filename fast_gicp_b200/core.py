@@ -48,6 +48,7 @@ EXPORTED_SYMBOLS = [
     "vgicp_append_source_to_target", "vgicp_crop_target", "vgicp_thin_target", "vgicp_deskew_source",
     "vgicp_set_source_timestamps", "vgicp_compute_error_ct", "vgicp_align_ct",
     "vgicp_set_source_timestamps_device", "vgicp_deskew_source_stored", "vgicp_align_sources",
+    "vgicp_carve_default_params", "vgicp_carve_target",
 ]
 PROF_NUM_CATEGORIES = 7
 
@@ -66,6 +67,18 @@ class LsqParams(C.Structure):
         ("use_gauss_newton", C.c_int),
         ("lm_max_iterations", C.c_int),
         ("lm_init_lambda_factor", C.c_double),
+    ]
+
+
+class CarveParams(C.Structure):
+    _fields_ = [
+        ("width", C.c_int),
+        ("height", C.c_int),
+        ("elevation_min", C.c_double),
+        ("elevation_max", C.c_double),
+        ("window", C.c_int),
+        ("margin", C.c_double),
+        ("margin_rel", C.c_double),
     ]
 
 
@@ -173,6 +186,8 @@ def load_library():
         "vgicp_append_source_to_target": [hp, dp],
         "vgicp_crop_target": [hp, dp, C.c_double, C.c_size_t],
         "vgicp_thin_target": [hp, C.c_double, C.c_int],
+        "vgicp_carve_default_params": [C.POINTER(CarveParams)],
+        "vgicp_carve_target": [hp, dp, C.POINTER(CarveParams), C.POINTER(C.c_size_t)],
         "vgicp_deskew_source": [hp, C.c_void_p, C.c_size_t, C.c_size_t, dp, C.c_double],
         "vgicp_set_source_timestamps": [hp, C.c_void_p, C.c_size_t, C.c_size_t, C.c_double],
         "vgicp_compute_error_ct": [hp, dp, dp, dp, dp, dp, dp, dp],
@@ -187,6 +202,7 @@ def load_library():
         fn.argtypes = argtypes
         fn.restype = C.c_int
     L.vgicp_lsq_default_params.restype = None
+    L.vgicp_carve_default_params.restype = None
     L.vgicp_last_error.argtypes = [hp]
     L.vgicp_last_error.restype = C.c_char_p
     L.vgicp_profile_category_name.argtypes = [C.c_int]
@@ -203,6 +219,20 @@ def default_params(**kw):
     for k, v in kw.items():
         setattr(p, k, v)
     return p
+
+
+def carve_params(**kw):
+    """vgicp_carve_target's parameters as a dict: the library's defaults (vgicp_carve_default_params), overridden by kw.  Keys:
+    width, height, elevation_min, elevation_max (rad), window, margin (m), margin_rel; synthetic.carve_indices takes the same dict."""
+    p = CarveParams()
+    load_library().vgicp_carve_default_params(C.byref(p))
+    out = {name: getattr(p, name) for name, _ in CarveParams._fields_}
+    for k, v in kw.items():
+        if k not in out:
+            raise TypeError(f"unknown carve parameter {k!r}")
+        if v is not None:
+            out[k] = v
+    return out
 
 
 def pose_to_c(T):
@@ -602,6 +632,17 @@ class Core:
         """Keep at most max_points_per_voxel target points per cell floor(p * (1 / leaf_size)) (float32), the oldest in array
         order; rebuild the voxel map.  Kept rows are unchanged and stay in order.  Errors raise and change nothing."""
         self._check(self._lib.vgicp_thin_target(self._h, float(leaf_size), int(max_points_per_voxel)))
+
+    def carve_target(self, T, width=None, height=None, elevation_min=None, elevation_max=None, window=None, margin=None, margin_rel=None):
+        """Remove the target points the current source (the scan in its sensor frame, placed by the 4x4 T) sees through: every map
+        point clearly in front of the least range measured in its range-image window (include/vgicp_b200.h gives the float32
+        rule).  None takes the library's default.  Returns the number of points removed; errors raise and change nothing."""
+        p = CarveParams(**carve_params(width=width, height=height, elevation_min=elevation_min, elevation_max=elevation_max, window=window, margin=margin,
+                                       margin_rel=margin_rel))
+        t = pose_to_c(T)
+        removed = C.c_size_t(0)
+        self._check(self._lib.vgicp_carve_target(self._h, _dp(t), C.byref(p), C.byref(removed)))
+        return removed.value
 
     # ---- motion compensation
     def deskew_source(self, times, twist, t_ref=0.0):

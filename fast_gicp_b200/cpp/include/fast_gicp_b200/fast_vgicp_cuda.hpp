@@ -76,6 +76,18 @@ public:
     checkStrict(vgicp_thin_target(vgicp_cuda_, leaf_size, max_points_per_voxel));
     target_ = pcl::make_shared<PointCloudTarget>();
   }
+  // remove the target points the current source, placed by T, sees through (call after align, before appendSourceToTarget);
+  // params: NULL = vgicp_carve_default_params; returns the number of points removed
+  size_t carveTarget(const Matrix4& T, const vgicp_carve_params* params = nullptr) {
+    double Td[16];
+    for (int i = 0; i < 16; i++) Td[i] = static_cast<double>(T.v[i]);
+    vgicp_carve_params P;
+    if (params) P = *params; else vgicp_carve_default_params(&P);
+    size_t removed = 0;
+    checkStrict(vgicp_carve_target(vgicp_cuda_, Td, &P, &removed));
+    target_ = pcl::make_shared<PointCloudTarget>();
+    return removed;
+  }
 
   // Motion compensation (an extension): every source point becomes Exp((t_i - t_ref) twist) p_i, the point in the sensor frame at
   // t_ref (include/vgicp_b200.h), then the source covariances are recomputed as setInputSource computes them.  t: n float

@@ -135,6 +135,11 @@ static Eigen::Matrix4f to_mat4f(const ArrF& m) {
   for (int r = 0; r < 4; r++) for (int c = 0; c < 4; c++) T(r, c) = a(r, c);
   return T;
 }
+static vgicp_carve_params carve_defaults() {
+  vgicp_carve_params P;
+  vgicp_carve_default_params(&P);
+  return P;
+}
 template <typename S, int N>
 static py::array_t<S> to_numpy(const Eigen::Matrix<S, N, N>& M) {
   py::array_t<S> out({N, N});
@@ -295,6 +300,14 @@ PYBIND11_MODULE(pygicp, m) {
          },
          py::arg("center"), py::arg("radius"), py::arg("max_points") = 0)
     .def("thin_target", &VgicpCuda::thinTarget, py::arg("leaf_size"), py::arg("max_points_per_voxel"))
+    .def("carve_target",
+         [](VgicpCuda& v, const ArrF& T, int width, int height, double elevation_min, double elevation_max, int window, double margin, double margin_rel) {
+           const vgicp_carve_params P{width, height, elevation_min, elevation_max, window, margin, margin_rel};
+           return v.carveTarget(to_mat4f(T), &P);
+         },
+         py::arg("T"), py::arg("width") = carve_defaults().width, py::arg("height") = carve_defaults().height,
+         py::arg("elevation_min") = carve_defaults().elevation_min, py::arg("elevation_max") = carve_defaults().elevation_max,
+         py::arg("window") = carve_defaults().window, py::arg("margin") = carve_defaults().margin, py::arg("margin_rel") = carve_defaults().margin_rel)
     // motion compensation (not in the reference binding): one relative timestamp per source point, twist = [omega, v]
     .def("deskew_source",
          [](VgicpCuda& v, const ArrF& times, const ArrD& twist, double t_ref) {

@@ -258,6 +258,10 @@ struct vgicp_context {
   DevBuf<unsigned char> thin_scratch;
   DevBuf<unsigned char> thin_keep;
   DevBuf<unsigned> thin_box;
+
+  // carving of the local map (vgicp_carve_target): the scan's range image, float bits of the least range per pixel (the keep
+  // mask is thin_keep)
+  DevBuf<unsigned> carve_img;
 };
 
 namespace {
@@ -1406,6 +1410,7 @@ int vgicp_destroy(vgicp_handle h) {
   h->spare_pts.release(); h->spare_covA.release(); h->spare_covB.release();
   for (int j = 0; j < 2; j++) { h->thin_keys[j].release(); h->thin_vals[j].release(); }
   h->thin_scratch.release(); h->thin_keep.release(); h->thin_box.release();
+  h->carve_img.release();
   h->eval.release();
   h->multi.release();
   if (h->d_multi_in) cudaFree(h->d_multi_in);
@@ -2181,7 +2186,7 @@ int vgicp_append_source_to_target(vgicp_handle h, const double T[16]) {
   return local_map_rebuild(h);
 }
 
-// k_crop_rank over the target (keep: the optional per-point mask) and the read-back of the number of passing points, the one
+// k_crop_rank over the target (keep: the optional per-point mask, which replaces the radius test) and the read-back of the number of passing points, the one
 // synchronisation of a crop and the second of a thinning; also sizes the spare arrays k_crop_scatter compacts into
 static int local_map_rank(vgicp_handle h, const unsigned char* keep, float cx, float cy, float cz, float r2, size_t* passed) {
   Cloud& t = h->target;
@@ -2299,11 +2304,82 @@ int vgicp_thin_target(vgicp_handle h, double leaf_size, int max_points_per_voxel
     skeys = h->thin_keys[passes & 1].p;
     svals = h->thin_vals[passes & 1].p;
   }
-  // 4. the keep mask; 5. the crop's compaction with it (every point passes r^2 = +inf: the coordinates are finite)
+  // 4. the keep mask; 5. the crop's compaction with it (the mask alone decides)
   KLAUNCH_ST(h, t.st, VGICP_PROF_OTHER, k_thin_keep<<<blocks_for(n, 256), 256, 0, t.st>>>(skeys, svals, n, max_points_per_voxel, h->thin_keep.p));
   CU_TRY(h, cudaGetLastError());
   size_t kept = 0;
   if ((rc = local_map_rank(h, h->thin_keep.p, 0.0f, 0.0f, 0.0f, std::numeric_limits<float>::infinity(), &kept))) return rc;
+  return local_map_compact(h, 0, (int)kept);
+}
+
+void vgicp_carve_default_params(vgicp_carve_params* p) {
+  if (!p) return;
+  p->width = 1024;
+  p->height = 64;
+  p->elevation_min = -25.0 * M_PI / 180.0;
+  p->elevation_max = 3.0 * M_PI / 180.0;
+  p->window = 1;
+  p->margin = 0.3;
+  p->margin_rel = 0.02;
+}
+
+// Carving: the scan's range image (memset, k_carve_image on the target's stream after the source is ready), the keep mask
+// (k_carve_keep), then thinning's compaction with it (the one synchronisation: the new size)
+int vgicp_carve_target(vgicp_handle h, const double T[16], const vgicp_carve_params* params, size_t* removed) {
+  CHECK_HANDLE(h);
+  DeviceGuard g(h->device);
+  if (!T || !params) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "carve_target: null pose or params");
+  for (int i = 0; i < 16; i++)
+    if (!std::isfinite(T[i])) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "carve_target: non-finite pose");
+  const vgicp_carve_params& P = *params;
+  if (P.width < 1 || P.height < 1 || (long long)P.width * P.height > (1ll << 24))
+    return fail(h, VGICP_ERR_INVALID_ARGUMENT, "carve_target: width and height must be >= 1 with width * height <= 2^24");
+  const double half_pi = 0.5 * M_PI;
+  if (!(P.elevation_min > -half_pi && P.elevation_max < half_pi && P.elevation_min < P.elevation_max))
+    return fail(h, VGICP_ERR_INVALID_ARGUMENT, "carve_target: the elevation limits must lie in (-pi/2, pi/2) with elevation_min < elevation_max");
+  const double t_lo = tan(P.elevation_min), t_hi = tan(P.elevation_max);
+  CarveImage im;
+  im.W = P.width;
+  im.H = P.height;
+  im.wq = (float)P.width * 0.25f;
+  im.e_lo = (float)t_lo;
+  im.inv_de = (float)(P.height / (t_hi - t_lo));
+  if (!std::isfinite(im.e_lo) || !(std::isfinite(im.inv_de) && im.inv_de > 0.0f))
+    return fail(h, VGICP_ERR_INVALID_ARGUMENT, "carve_target: (float)tan(elevation_min) must be finite and the float row scale finite and > 0");
+  if (P.window < 0 || P.window > 8) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "carve_target: window must lie in [0, 8]");
+  if (!(P.margin >= 0.0) || !std::isfinite((float)P.margin)) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "carve_target: margin must be finite and >= 0");
+  if (!(P.margin_rel >= 0.0 && P.margin_rel < 1.0)) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "carve_target: margin_rel must lie in [0, 1)");
+  int rc = local_map_check(h, "carve_target");
+  if (rc) return rc;
+  Cloud& s = h->source;
+  Cloud& t = h->target;
+  if (!s.has_pts || s.n == 0) return fail(h, VGICP_ERR_BAD_STATE, "carve_target: the source has no points");
+  const int n = t.n;
+  if (n == 0) return fail(h, VGICP_ERR_BAD_STATE, "carve_target: the target has no points");
+  // Ti = [R^T | -R^T t] in double, cast once
+  Pose Ti;
+  for (int j = 0; j < 3; j++) {
+    for (int k = 0; k < 3; k++) Ti.r[j * 3 + k] = (float)T[j * 4 + k];  // R_kj
+    Ti.t[j] = (float)(-((T[j * 4 + 0] * T[12] + T[j * 4 + 1] * T[13]) + T[j * 4 + 2] * T[14]));
+  }
+  const size_t pixels = (size_t)P.width * (size_t)P.height;
+  CU_TRY(h, h->carve_img.reserve(pixels));
+  CU_TRY(h, h->thin_keep.reserve(n));
+  // 1. the range image, from the source on the target's stream; the next upload into the source must not overtake this read
+  CU_TRY(h, cudaMemsetAsync(h->carve_img.p, 0xFF, pixels * sizeof(unsigned), t.st));
+  if (s.st != t.st) CU_TRY(h, cudaStreamWaitEvent(t.st, s.ready, 0));
+  KLAUNCH_ST(h, t.st, VGICP_PROF_OTHER, k_carve_image<<<blocks_for(s.n, 256), 256, 0, t.st>>>(s.pts.p, s.n, im, h->carve_img.p));
+  CU_TRY(h, cudaGetLastError());
+  CU_TRY(h, cudaEventRecord(h->ev_append, t.st));
+  if (s.st != t.st) CU_TRY(h, cudaStreamWaitEvent(s.st, h->ev_append, 0));
+  // 2. the keep mask; 3. thinning's compaction with it (the mask alone decides: a non-finite point it keeps stays)
+  KLAUNCH_ST(h, t.st, VGICP_PROF_OTHER,
+             k_carve_keep<<<blocks_for(n, 256), 256, 0, t.st>>>(t.pts.p, n, Ti, im, h->carve_img.p, P.window, (float)P.margin, (float)P.margin_rel, h->thin_keep.p));
+  CU_TRY(h, cudaGetLastError());
+  size_t kept = 0;
+  if ((rc = local_map_rank(h, h->thin_keep.p, 0.0f, 0.0f, 0.0f, std::numeric_limits<float>::infinity(), &kept))) return rc;
+  if (kept == 0) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "carve_target: the carve would leave no points");
+  if (removed) *removed = (size_t)n - kept;
   return local_map_compact(h, 0, (int)kept);
 }
 

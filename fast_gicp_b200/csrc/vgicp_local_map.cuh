@@ -35,17 +35,22 @@ __global__ void k_append_transformed(const float4* __restrict__ src_pts, const f
   dst_covB[i] = make_float2(__fmul_rn(0.5f, __fadd_rn(N[5], N[7])), N[8]);
 }
 
-// Crop, pass 1: point i passes when d^2 = (dx dx + dy dy) + dz dz <= r2 (dx = p.x - c.x, ...) and, when `keep` is given,
-// keep[i] != 0; rank[i] = number of passing points before i (block_rank), or -1.  The total lands in *count.
+// Crop, pass 1: point i passes when d^2 = (dx dx + dy dy) + dz dz <= r2 (dx = p.x - c.x, ...) or, when `keep` is given, when
+// keep[i] != 0 (the radius is then not tested: a carve keeps non-finite points); rank[i] = number of passing points before i
+// (block_rank), or -1.  The total lands in *count.
 __global__ void __launch_bounds__(kRankThreads) k_crop_rank(const float4* __restrict__ pts, const unsigned char* __restrict__ keep, int n, float cx, float cy, float cz,
                                                             float r2, int* __restrict__ rank, int* __restrict__ count, unsigned long long* state_words, unsigned epoch) {
   const int i = blockIdx.x * kRankThreads + threadIdx.x;
   int flag = 0;
   if (i < n) {
-    const float4 p = pts[i];
-    const float dx = __fsub_rn(p.x, cx), dy = __fsub_rn(p.y, cy), dz = __fsub_rn(p.z, cz);
-    const float d2 = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
-    flag = d2 <= r2 && (!keep || keep[i]) ? 1 : 0;
+    if (keep) {
+      flag = keep[i] ? 1 : 0;
+    } else {
+      const float4 p = pts[i];
+      const float dx = __fsub_rn(p.x, cx), dy = __fsub_rn(p.y, cy), dz = __fsub_rn(p.z, cz);
+      const float d2 = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
+      flag = d2 <= r2 ? 1 : 0;
+    }
   }
   const int r = block_rank(flag, state_words, epoch, count);
   if (i < n) rank[i] = flag ? r : -1;
@@ -115,6 +120,72 @@ __global__ void k_thin_keep(const unsigned long long* __restrict__ keys, const u
   if (j >= n) return;
   const bool k = j < M || keys[j - M] != keys[j];
   keep[vals ? vals[j] : (unsigned)j] = k ? 1 : 0;
+}
+
+// Carving (vgicp_carve_target): the scan's range image, then one test per map point against the least range in its window.  The
+// pixel and the range follow the header's recipe; a point has a pixel iff carve_pixel returns true.
+struct CarveImage {
+  int W, H;
+  float wq, e_lo, inv_de;  // W * 0.25f, (float)tan(elevation_min), (float)(H / (tan(elevation_max) - tan(elevation_min)))
+};
+
+__device__ __forceinline__ bool carve_pixel(const CarveImage& im, float x, float y, float z, int* row, int* col, float* r) {
+  if (!(isfinite(x) && isfinite(y) && isfinite(z))) return false;
+  const float s = __fadd_rn(fabsf(x), fabsf(y));
+  if (s == 0.0f) return false;
+  const float q = __fdiv_rn(fabsf(y), s);
+  const float a = y >= 0.0f ? (x >= 0.0f ? q : __fsub_rn(2.0f, q)) : (x < 0.0f ? __fadd_rn(2.0f, q) : __fsub_rn(4.0f, q));
+  const float xy = __fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y));
+  const float u = __fmul_rn(__fsub_rn(__fdiv_rn(z, __fsqrt_rn(xy)), im.e_lo), im.inv_de);
+  if (!(u >= 0.0f && u < (float)im.H)) return false;  // (also a NaN or infinite u when x x + y y underflows)
+  const int c = (int)floorf(__fmul_rn(a, im.wq));
+  *col = c == im.W ? 0 : c;
+  *row = (int)floorf(u);
+  *r = __fsqrt_rn(__fadd_rn(xy, __fmul_rn(z, z)));
+  return true;
+}
+
+// one thread per source point: the least range per pixel (img filled with 0xFFFFFFFF, "no return", by the caller)
+__global__ void k_carve_image(const float4* __restrict__ src, int n, const CarveImage im, unsigned* __restrict__ img) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float4 p = src[i];
+  int row, col;
+  float r;
+  if (carve_pixel(im, p.x, p.y, p.z, &row, &col, &r)) atomicMin(img + (size_t)row * im.W + col, __float_as_uint(r));
+}
+
+// one thread per target point: into the sensor frame by Ti (row-major 3x4), the pixel, the least range r_min in the window, and
+// keep[i] = 0 iff r < r_min - (margin + margin_rel r_min)
+__global__ void k_carve_keep(const float4* __restrict__ pts, int n, const Pose Ti, const CarveImage im, const unsigned* __restrict__ img, int window, float margin,
+                             float margin_rel, unsigned char* __restrict__ keep) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float4 m = pts[i];
+  float s[3];
+#pragma unroll
+  for (int j = 0; j < 3; j++)
+    s[j] = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(Ti.r[j * 3 + 0], m.x), __fmul_rn(Ti.r[j * 3 + 1], m.y)), __fmul_rn(Ti.r[j * 3 + 2], m.z)), Ti.t[j]);
+  int row, col;
+  float r;
+  bool removed = false;
+  if (carve_pixel(im, s[0], s[1], s[2], &row, &col, &r)) {
+    unsigned best = 0xFFFFFFFFu;
+    const int r0 = row - window < 0 ? 0 : row - window, r1 = row + window >= im.H ? im.H - 1 : row + window;
+    for (int rr = r0; rr <= r1; rr++) {
+      const unsigned* line = img + (size_t)rr * im.W;
+      for (int dc = -window; dc <= window; dc++) {
+        int cc = (col + dc) % im.W;
+        if (cc < 0) cc += im.W;
+        best = min(best, __ldg(line + cc));
+      }
+    }
+    if (best != 0xFFFFFFFFu) {
+      const float r_min = __uint_as_float(best);
+      removed = r < __fsub_rn(r_min, __fadd_rn(margin, __fmul_rn(margin_rel, r_min)));
+    }
+  }
+  keep[i] = removed ? 0 : 1;
 }
 
 }  // namespace vgicp

@@ -329,6 +329,13 @@ class FastVGICPCuda(LsqRegistration):
         self.vgicp_cuda_.thin_target(leaf_size, max_points_per_voxel)
         self.target_ = _DeviceMap()
 
+    def carveTarget(self, T, **params):
+        """Remove the target points the current source, placed by T, sees through (call after align, before
+        appendSourceToTarget); params: Core.carve_target's keywords.  Returns the number of points removed."""
+        removed = self.vgicp_cuda_.carve_target(np.asarray(T, dtype=np.float64), **params)
+        self.target_ = _DeviceMap()
+        return removed
+
     def append_source_to_target(self, T):
         self.appendSourceToTarget(T)
 
@@ -337,6 +344,9 @@ class FastVGICPCuda(LsqRegistration):
 
     def thin_target(self, leaf_size, max_points_per_voxel):
         self.thinTarget(leaf_size, max_points_per_voxel)
+
+    def carve_target(self, T, **params):
+        return self.carveTarget(T, **params)
 
     # -- motion compensation (an extension).  Afterwards the source on the device is no longer the cloud given to setInputSource:
     # input_ becomes a copy of it (its points stay for align's output), so setInputSource(that cloud) reloads the raw cloud.

@@ -154,6 +154,117 @@ def thin_indices(pts, leaf, M):
     return np.sort(order[rank < M])
 
 
+def _carve_pixels(p, W, H, wq, e_lo, inv_de):
+    """vgicp_carve_target's pixel and range of float32 sensor-frame points (n, 3) -> (has_pixel, row, col, r)."""
+    x, y, z = p[:, 0], p[:, 1], p[:, 2]
+    with np.errstate(all="ignore"):
+        s = np.abs(x) + np.abs(y)
+        q = np.abs(y) / s
+        a = np.where(y >= 0, np.where(x >= 0, q, np.float32(2) - q), np.where(x < 0, np.float32(2) + q, np.float32(4) - q))
+        xy = x * x + y * y
+        u = (z / np.sqrt(xy) - e_lo) * inv_de
+        ok = np.isfinite(x) & np.isfinite(y) & np.isfinite(z) & (s != 0) & (u >= 0) & (u < np.float32(H))
+        col = np.where(ok, np.floor(a * wq), 0).astype(np.int64)
+        row = np.where(ok, np.floor(u), 0).astype(np.int64)
+        r = np.sqrt(xy + z * z)
+    col[col == W] = 0
+    return ok, row, col, r
+
+
+def carve_indices(target, source, T, params):
+    """Rows vgicp_carve_target keeps, ascending, with the header's float32 rule: the source (the scan in its sensor frame) fills a
+    height x width image with its least range per pixel; target row i, taken into the sensor frame by Ti = [R^T | -R^T t] (formed
+    in double, cast once), is removed iff it has a pixel, a non-empty pixel lies within `window` rows and columns of it, and its
+    range r < r_min - (margin + margin_rel * r_min).  params: a dict with the keys of vgicp_carve_params (core.carve_params)."""
+    import math
+
+    W, H, w = int(params["width"]), int(params["height"]), int(params["window"])
+    wq = np.float32(W) * np.float32(0.25)
+    t_lo, t_hi = math.tan(params["elevation_min"]), math.tan(params["elevation_max"])
+    e_lo, inv_de = np.float32(t_lo), np.float32(H / (t_hi - t_lo))
+    margin, margin_rel = np.float32(params["margin"]), np.float32(params["margin_rel"])
+    empty = np.uint32(0xFFFFFFFF)
+    img = np.full(W * H, empty, dtype=np.uint32)
+    ok, row, col, r = _carve_pixels(np.asarray(source, dtype=np.float32).reshape(-1, 3), W, H, wq, e_lo, inv_de)
+    np.minimum.at(img, row[ok] * W + col[ok], r[ok].view(np.uint32))  # r >= 0: the bit order is the numeric order
+    Tm = np.asarray(T, dtype=np.float64)
+    Ti = np.empty((3, 4), dtype=np.float32)
+    for j in range(3):
+        for k in range(3):
+            Ti[j, k] = Tm[k, j]
+        Ti[j, 3] = -((float(Tm[0, j]) * float(Tm[0, 3]) + float(Tm[1, j]) * float(Tm[1, 3])) + float(Tm[2, j]) * float(Tm[2, 3]))
+    m = np.asarray(target, dtype=np.float32).reshape(-1, 3)
+    with np.errstate(all="ignore"):
+        s = np.stack([((Ti[j, 0] * m[:, 0] + Ti[j, 1] * m[:, 1]) + Ti[j, 2] * m[:, 2]) + Ti[j, 3] for j in range(3)], axis=1)
+    ok, row, col, r = _carve_pixels(s, W, H, wq, e_lo, inv_de)
+    best = np.full(len(m), empty, dtype=np.uint32)
+    for dr in range(-w, w + 1):
+        rr = row + dr
+        inside = (rr >= 0) & (rr < H)
+        for dc in range(-w, w + 1):
+            v = img[np.clip(rr, 0, H - 1) * W + (col + dc) % W]
+            best = np.minimum(best, np.where(inside, v, empty))
+    r_min = best.view(np.float32)
+    with np.errstate(all="ignore"):
+        removed = ok & (best != empty) & (r < r_min - (margin + margin_rel * r_min))
+    return np.flatnonzero(~removed)
+
+
+def in_boxes(pts, boxes, pad=(0.3, 0.3, 0.1)):
+    """Points (n, 3) inside any of the axis-aligned boxes [(lo, hi), ...] grown by pad per axis."""
+    p = np.asarray(pts, dtype=np.float64)
+    out = np.zeros(len(p), dtype=bool)
+    for lo, hi in boxes:
+        out |= np.all((p >= np.asarray(lo) - pad) & (p <= np.asarray(hi) + pad), axis=1)
+    return out
+
+
+def _path_point(s, step, turn_deg):
+    """Point and heading at arc length s along the path of 0.8 m-style steps whose heading turns turn_deg per step."""
+    k = int(s // step)
+    xy = np.zeros(2)
+    for i in range(k):
+        yaw = np.radians(turn_deg * i)
+        xy = xy + step * np.array([np.cos(yaw), np.sin(yaw)])
+    yaw = np.radians(turn_deg * k)
+    return xy + (s - k * step) * np.array([np.cos(yaw), np.sin(yaw)]), yaw
+
+
+DEFAULT_MOVERS = ((3.5, 8.0, 2.0),)  # (lane offset to the left in m, start ahead in m, speed over the sensor's)
+
+
+def moving_object_sequence(frames, seed, movers=DEFAULT_MOVERS, beams=64, az_steps=2083, downsample=0.25, step=0.8, turn_deg=2.0, size=(4.0, 2.0, 1.5)):
+    """A drive past moving vehicles -> (poses, scans, boxes): the sensor moves `step` m per frame along an arc turning turn_deg
+    per frame through _make_world(seed)'s world (scripts/bench_local_map.py's sequence: the same path and noise seeds); each mover
+    is a size[0] x size[1] x size[2] m axis-aligned box 0.2 m above the ground that follows the same path, offset to the left and
+    `ahead` m ahead at frame 0, at `speed` times the sensor's speed.  Static boxes that any mover's positions come within 1 m of
+    are removed from the world, so that no vehicle drives through a building.  boxes[k]: the movers' (lo, hi) at frame k, in the
+    world frame (in_boxes labels the points they produced).  scans[k] is in the sensor frame of poses[k]."""
+    world = _make_world(np.random.default_rng(seed))
+    boxes = []
+    for k in range(frames):
+        fb = []
+        for lane, ahead, speed in movers:
+            xy, yaw = _path_point(ahead + speed * step * k, step, turn_deg)
+            c = xy + lane * np.array([-np.sin(yaw), np.cos(yaw)])
+            lo = np.array([c[0] - size[0] / 2, c[1] - size[1] / 2, -1.53])
+            fb.append((lo, lo + np.array([size[0], size[1], size[2]])))
+        boxes.append(fb)
+    every = [b for fb in boxes for b in fb]
+    world = [(lo, hi) for lo, hi in world if not any(np.all(lo - 1.0 <= mhi) and np.all(mlo - 1.0 <= hi) for mlo, mhi in every)]
+    poses, scans = [], []
+    xy = np.zeros(2)
+    for k in range(frames):
+        yaw = np.radians(turn_deg * k)
+        T = np.eye(4)
+        T[:3, :3] = [[np.cos(yaw), -np.sin(yaw), 0], [np.sin(yaw), np.cos(yaw), 0], [0, 0, 1]]
+        T[:2, 3] = xy
+        xy = xy + step * np.array([np.cos(yaw), np.sin(yaw)])
+        poses.append(T)
+        scans.append(voxel_downsample(scan(world + boxes[k], beams, az_steps, T, np.random.default_rng(seed * 1000 + k)), downsample))
+    return poses, scans, boxes
+
+
 def kitti_like_pair(beams=64, az_steps=2083, seed=42, pose=(0.8, 0.05, 0.7), downsample=0.25, max_points=None):
     """(target, source, T_gt): target scanned at the origin, source from a sensor moved by pose=(tx, ty, yaw_deg).
     T_gt maps source-frame points into the target frame (what registration should recover)."""

@@ -253,7 +253,8 @@ VGICP_API int vgicp_crop_target(vgicp_handle h, const double center[3], double r
  *           scan only fills the cells that still have room, and a vehicle that stands still adds nothing to full cells.
  * Kept points and their covariances are unchanged and stay in their original order (a stable subsequence of the rows).  The state
  * afterwards is the one described above, also when nothing is dropped.  Two host synchronisations (the cells' box, the new size).
- * Per frame: vgicp_align, vgicp_append_source_to_target, vgicp_thin_target, then vgicp_crop_target (radius, optional cap).
+ * Per frame: vgicp_align, vgicp_carve_target, vgicp_append_source_to_target, vgicp_thin_target, then vgicp_crop_target (radius,
+ * optional cap).
  * Errors, all returned before anything is modified (target and map stay exactly as they were):
  *   VGICP_ERR_INVALID_ARGUMENT  leaf_size not finite and > 0, l or inv not finite and > 0, M < 1; found by the first pass over
  *                               the points: a non-finite target coordinate, a cell outside [-2^31, 2^31), or a cell box too wide
@@ -261,6 +262,48 @@ VGICP_API int vgicp_crop_target(vgicp_handle h, const double center[3], double r
  *   VGICP_ERR_BAD_STATE         target without points or covariances;
  *   VGICP_ERR_UNSUPPORTED       an NDT problem selected, or stage-1 sharding. */
 VGICP_API int vgicp_thin_target(vgicp_handle h, double leaf_size, int max_points_per_voxel);
+/* vgicp_carve_target: remove the moving objects' trails from the map.  The current source is the scan in its sensor frame (the
+ * sensor at the origin) and T (column-major 4x4) maps it into the target frame, e.g. the vgicp_align result.  Every target point
+ * that lies clearly in front of what the scan measured in its direction was seen through by the scan's rays: free space now, so
+ * it is removed.  All arithmetic below is IEEE single operations without contraction, in the order written.
+ *   pixel      of a sensor-frame point (x, y, z) in a height x width range image, without trigonometry:
+ *                q = |y| / (|x| + |y|);  a = q (x >= 0, y >= 0), 2 - q (x < 0, y >= 0), 2 + q (x < 0, y < 0), 4 - q (x >= 0, y < 0)
+ *                (the "diamond angle", monotone in the azimuth over [0, 4));  col = (int)floorf(a * wq), wq = width * 0.25f, and
+ *                col == width becomes 0.  A column spans 4 / width rad of azimuth on the axes and 8 / width on the diagonals.
+ *                rho = sqrtf(x x + y y), e = z / rho (the tangent of the elevation), u = (e - e_lo) * inv_de; the point has a
+ *                pixel iff 0 <= u < height, row = (int)floorf(u).  e_lo = (float)tan(elevation_min) and
+ *                inv_de = (float)(height / (tan(elevation_max) - tan(elevation_min))), in double with the C library's tan.
+ *                A point with |x| + |y| == 0 or a non-finite coordinate has no pixel.
+ *   range      r = sqrtf((x x + y y) + z z).
+ *   image      per pixel, the least r of the source points that land in it (atomicMin on the float bits: r >= 0, so the bit
+ *              order is the numeric order; independent of the order of the points); a pixel no point lands in is empty.
+ *   map point  into the sensor frame with Ti = [R^T | -R^T t], formed from T in double (Ti_jk = R_kj,
+ *              Ti_j3 = -((R_0j t_0 + R_1j t_1) + R_2j t_2)) and cast to float once:  s_j = ((Ti_j0 m_0 + Ti_j1 m_1) + Ti_j2 m_2) + Ti_j3.
+ *   test       r_min = the least r over the non-empty pixels within `window` rows and columns of the point's pixel (rows clipped at
+ *              the image's edges, columns modulo width); thr = r_min - (margin + margin_rel * r_min) with margin and margin_rel
+ *              cast to float.  The point is removed iff it has a pixel, its window holds a non-empty pixel, and r < thr.  A point
+ *              outside the vertical field of view, with an empty window, behind or on the measured surface, or with a non-finite
+ *              coordinate (in the map or after the transform) is kept.
+ * Kept points and their covariances are unchanged and stay in their original order; the state afterwards is the one described
+ * above, also when nothing is removed.  *removed (optional) receives the number of removed points.  One host synchronisation (the
+ * new size).  The source is not changed.  Call it after vgicp_align and before vgicp_append_source_to_target, so that the scan is
+ * not tested against its own points, and before vgicp_thin_target, so that the cells it frees can fill again.
+ * Errors, all returned before anything is modified (target and map stay exactly as they were):
+ *   VGICP_ERR_INVALID_ARGUMENT  null or non-finite T, null params, width or height < 1, width * height > 2^24, elevation limits
+ *                               not in (-pi/2, pi/2) with min < max, e_lo not finite or inv_de not finite and > 0, window not
+ *                               in [0, 8], margin negative or not finite as a float, margin_rel not in [0, 1), a carve that
+ *                               would leave no points;
+ *   VGICP_ERR_BAD_STATE         source without points, target without points or covariances;
+ *   VGICP_ERR_UNSUPPORTED       an NDT problem selected, or stage-1 sharding. */
+typedef struct {
+  int width, height;                   /* range image: columns (azimuth) x rows (elevation); 1024 x 64 */
+  double elevation_min, elevation_max; /* vertical field of view in rad, lower and upper edge: -25 and +3 degrees */
+  int window;                          /* pixels searched in each direction around the point's pixel, 0 .. 8; 1 */
+  double margin;                       /* m: a point must lie this far in front of the measured range; 0.3 */
+  double margin_rel;                   /* and this fraction of it in addition; 0.02 */
+} vgicp_carve_params;
+VGICP_API void vgicp_carve_default_params(vgicp_carve_params* p);
+VGICP_API int vgicp_carve_target(vgicp_handle h, const double T[16], const vgicp_carve_params* params, size_t* removed);
 /* ---- motion compensation (not in the reference) ---------------------------------------------------------------------------
  * A spinning or solid-state LiDAR fires the points of one sweep over its period while the vehicle moves; each point is in the
  * sensor frame of its own firing time.  vgicp_deskew_source re-expresses every source point in the sensor frame at t_ref under a

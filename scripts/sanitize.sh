@@ -40,12 +40,13 @@ c.set_resolution(0.5); c.set_neighbor_search_method("DIRECT1")
 r = c.register(bt, bs)
 print("stream", len(bs), "converged", bool(r.converged))
 c.close()
-# local map: append the registered source (the target's arrays grow with a device copy), thin it (cell box, u64 keys and sort,
-# keep mask), crop it (block rank, compaction)
+# local map: carve it with the registered source (range image, atomicMin, window test), append the source (the target's arrays
+# grow with a device copy), thin it (cell box, u64 keys and sort, keep mask), crop it (block rank, compaction)
 c = Core(0)
 c.set_neighbor_search_method("DIRECT7")
 r = c.register(tgt, src)
 from fast_gicp_b200.core import pose_from_c
+print("carved", c.carve_target(pose_from_c(r.T), window=2))
 c.append_source_to_target(pose_from_c(r.T))
 c.thin_target(0.5, 2)
 c.crop_target((0.0, 0.0, 0.0), 30.0, len(tgt))
