@@ -353,7 +353,7 @@ __global__ void __launch_bounds__(kGridWarps * 32, 1) k_grid_centroids(const uns
 
 struct vgicp_prep_context {
   int device = 0;
-  cudaStream_t stream = nullptr;
+  Stream stream;
   std::string err;
   DevBuf<unsigned char> staging;  // host input copied here
   DevBuf<float4> pts4;
@@ -362,9 +362,9 @@ struct vgicp_prep_context {
   DevBuf<float> out;
   DevBuf<unsigned long long> chunk_state;
   unsigned chunk_epoch = 0;
-  float4* tail = nullptr;  // [kHist]
-  int* d_counts = nullptr;  // [0] flushed total, [1] n_out
-  int* h_counts = nullptr;  // pinned
+  DevPtr<float4[]> tail;    // [kHist]
+  DevPtr<int[]> d_counts;   // [0] flushed total, [1] n_out
+  HostPtr<int[]> h_counts;  // pinned
   DevBuf<float> fflushed;  // per-point fields: flushed field centroids [n][F]
   DevBuf<float> ftail;     // ... and those of the entries still holding a voxel [kHist][F]
   // exact grid: sort keys and values (two buffers each), the sorted float4 payload, the sort scratch, the voxel starts
@@ -372,8 +372,8 @@ struct vgicp_prep_context {
   DevBuf<float4> gsorted4;
   DevBuf<unsigned char> gscratch;
   DevBuf<int> gvstart;
-  unsigned* d_grid = nullptr;  // [kGridState]
-  unsigned* h_grid = nullptr;  // pinned
+  DevPtr<unsigned[]> d_grid;   // [kGridState]
+  HostPtr<unsigned[]> h_grid;  // pinned
 };
 
 namespace {
@@ -400,14 +400,14 @@ int vgicp_prep_create(int device, vgicp_prep_handle* out) {
   if (!h) return 3;
   h->device = device;
   bool ok = cudaSetDevice(device) == cudaSuccess;
-  ok = ok && cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) == cudaSuccess;
-  ok = ok && cudaMalloc(&h->tail, kHist * sizeof(float4)) == cudaSuccess;
-  ok = ok && cudaMalloc(&h->d_counts, 2 * sizeof(int)) == cudaSuccess;
-  ok = ok && cudaMallocHost(&h->h_counts, 2 * sizeof(int)) == cudaSuccess;
-  ok = ok && cudaMalloc(&h->d_grid, kGridState * sizeof(unsigned)) == cudaSuccess;
-  ok = ok && cudaMallocHost(&h->h_grid, kGridState * sizeof(unsigned)) == cudaSuccess;
+  ok = ok && stream_create(h->stream, cudaStreamNonBlocking) == cudaSuccess;
+  ok = ok && device_alloc(h->tail, kHist * sizeof(float4)) == cudaSuccess;
+  ok = ok && device_alloc(h->d_counts, 2 * sizeof(int)) == cudaSuccess;
+  ok = ok && host_alloc(h->h_counts, 2 * sizeof(int), cudaHostAllocDefault) == cudaSuccess;
+  ok = ok && device_alloc(h->d_grid, kGridState * sizeof(unsigned)) == cudaSuccess;
+  ok = ok && host_alloc(h->h_grid, kGridState * sizeof(unsigned), cudaHostAllocDefault) == cudaSuccess;
   if (!ok) {
-    vgicp_prep_destroy(h);
+    delete h;
     return 3;
   }
   *out = h;
@@ -417,19 +417,7 @@ int vgicp_prep_create(int device, vgicp_prep_handle* out) {
 void vgicp_prep_destroy(vgicp_prep_handle h) {
   if (!h) return;
   cudaSetDevice(h->device);
-  if (h->stream) {
-    cudaStreamSynchronize(h->stream);
-    cudaStreamDestroy(h->stream);
-  }
-  h->staging.release(); h->pts4.release(); h->entry.release(); h->flushed.release(); h->out.release(); h->chunk_state.release();
-  h->fflushed.release(); h->ftail.release();
-  for (int k = 0; k < 2; k++) { h->gkeys[k].release(); h->gvals[k].release(); }
-  h->gsorted4.release(); h->gscratch.release(); h->gvstart.release();
-  if (h->d_grid) cudaFree(h->d_grid);
-  if (h->h_grid) cudaFreeHost(h->h_grid);
-  if (h->tail) cudaFree(h->tail);
-  if (h->d_counts) cudaFree(h->d_counts);
-  if (h->h_counts) cudaFreeHost(h->h_counts);
+  if (h->stream) cudaStreamSynchronize(h->stream.get());
   delete h;
 }
 
@@ -447,12 +435,12 @@ cudaError_t launch_filter(vgicp_prep_handle h, const float* d_in, size_t stride_
   for (int j = 0; j < F; j++) fa.off[j] = off[j];
   fa.flushed = h->fflushed.p;
   fa.tail = h->ftail.p;
-  k_prep_keys<<<(ni + 255) / 256, 256, 0, h->stream>>>(d_in, stride_f, ni, inv_leaf, filter, h->pts4.p, h->entry.p);
-  const cudaError_t e = cudaMemsetAsync(h->flushed.p, 0, (size_t)ni * sizeof(float4), h->stream);
+  k_prep_keys<<<(ni + 255) / 256, 256, 0, h->stream.get()>>>(d_in, stride_f, ni, inv_leaf, filter, h->pts4.p, h->entry.p);
+  const cudaError_t e = cudaMemsetAsync(h->flushed.p, 0, (size_t)ni * sizeof(float4), h->stream.get());
   if (e != cudaSuccess) return e;
-  k_prep_walk<F><<<1, kHist, 0, h->stream>>>(h->pts4.p, h->entry.p, ni, inv_leaf, h->flushed.p, h->tail, fa);
-  k_prep_scatter<F><<<chunks, kRankThreads, 0, h->stream>>>(h->flushed.p, ni, d_out, out_cap, h->chunk_state.p, h->chunk_epoch, h->d_counts, h->fflushed.p);
-  k_prep_tail<F><<<1, kHist, 0, h->stream>>>(h->tail, h->d_counts, d_out, out_cap, h->d_counts + 1, h->ftail.p);
+  k_prep_walk<F><<<1, kHist, 0, h->stream.get()>>>(h->pts4.p, h->entry.p, ni, inv_leaf, h->flushed.p, h->tail.get(), fa);
+  k_prep_scatter<F><<<chunks, kRankThreads, 0, h->stream.get()>>>(h->flushed.p, ni, d_out, out_cap, h->chunk_state.p, h->chunk_epoch, h->d_counts.get(), h->fflushed.p);
+  k_prep_tail<F><<<1, kHist, 0, h->stream.get()>>>(h->tail.get(), h->d_counts.get(), d_out, out_cap, h->d_counts.get() + 1, h->ftail.p);
   return cudaGetLastError();
 }
 
@@ -463,7 +451,7 @@ cudaError_t stage_input(vgicp_prep_handle h, const float* points, size_t n, size
   *d_in = points;
   if (on_device) return cudaSuccess;
   cudaError_t e = h->staging.reserve(n * stride_bytes);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(h->staging.p, points, (n - 1) * stride_bytes + span, cudaMemcpyHostToDevice, h->stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(h->staging.p, points, (n - 1) * stride_bytes + span, cudaMemcpyHostToDevice, h->stream.get());
   *d_in = reinterpret_cast<const float*>(h->staging.p);
   return e;
 }
@@ -491,7 +479,7 @@ int run_filter(vgicp_prep_handle h, const char* who, const float* points, size_t
     d_out = h->out.p;
   }
   const int chunks = (ni + kRankThreads - 1) / kRankThreads;
-  PREP_TRY(h, lookback_next(h->chunk_state, h->chunk_epoch, chunks, h->stream));
+  PREP_TRY(h, lookback_next(h->chunk_state, h->chunk_epoch, chunks, h->stream.get()));
   const float inv_leaf = 1.0f / leaf;
   const size_t sf = stride_bytes / 4;
   const int flt = remove_near_origin ? 1 : 0;
@@ -507,14 +495,14 @@ int run_filter(vgicp_prep_handle h, const char* who, const float* points, size_t
     case 8: PREP_TRY(h, (launch_filter<8>(h, d_in, sf, off, ni, inv_leaf, flt, d_out, out_cap, chunks))); break;
     default: return fail(h, 1, w + ": unsupported field count");
   }
-  PREP_TRY(h, cudaMemcpyAsync(h->h_counts, h->d_counts, 2 * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  PREP_TRY(h, cudaStreamSynchronize(h->stream));
+  PREP_TRY(h, cudaMemcpyAsync(h->h_counts.get(), h->d_counts.get(), 2 * sizeof(int), cudaMemcpyDeviceToHost, h->stream.get()));
+  PREP_TRY(h, cudaStreamSynchronize(h->stream.get()));
   const size_t m = (size_t)h->h_counts[1];
   *n_out = m;
   if (m > cap) return fail(h, 1, w + ": output capacity too small (n points always suffice)");
   if (!out_on_device && m > 0) {
-    PREP_TRY(h, cudaMemcpyAsync(out, d_out, m * rec * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-    PREP_TRY(h, cudaStreamSynchronize(h->stream));
+    PREP_TRY(h, cudaMemcpyAsync(out, d_out, m * rec * sizeof(float), cudaMemcpyDeviceToHost, h->stream.get()));
+    PREP_TRY(h, cudaStreamSynchronize(h->stream.get()));
   }
   return 0;
 }
@@ -525,7 +513,7 @@ cudaError_t launch_centroids(vgicp_prep_handle h, const float* d_in, size_t stri
   fa.in = d_in;
   fa.stride_f = stride_f;
   for (int j = 0; j < F; j++) fa.off[j] = off[j];
-  k_grid_centroids<F><<<blocks, kGridWarps * 32, 0, h->stream>>>(keys, h->gsorted4.p, kept, h->gvstart.p, h->d_grid, fa, d_out, out_cap);
+  k_grid_centroids<F><<<blocks, kGridWarps * 32, 0, h->stream.get()>>>(keys, h->gsorted4.p, kept, h->gvstart.p, h->d_grid.get(), fa, d_out, out_cap);
   return cudaGetLastError();
 }
 
@@ -546,12 +534,12 @@ int run_voxel_grid(vgicp_prep_handle h, const float* points, size_t n, size_t st
   const size_t sf = stride_bytes / 4;
   const int flt = remove_near_origin ? 1 : 0;
   // 1. the box of the kept points' cells, read back: the one host decision (refusals, key width) before the sort
-  PREP_TRY(h, cudaMemsetAsync(h->d_grid, 0, kGridState * sizeof(unsigned), h->stream));
+  PREP_TRY(h, cudaMemsetAsync(h->d_grid.get(), 0, kGridState * sizeof(unsigned), h->stream.get()));
   const int bb = (ni + kGridBoxThreads - 1) / kGridBoxThreads;
-  k_grid_box<<<bb < 4 * kNumSMs ? bb : 4 * kNumSMs, kGridBoxThreads, 0, h->stream>>>(d_in, sf, ni, inv, flt, h->pts4.p, h->d_grid);
+  k_grid_box<<<bb < 4 * kNumSMs ? bb : 4 * kNumSMs, kGridBoxThreads, 0, h->stream.get()>>>(d_in, sf, ni, inv, flt, h->pts4.p, h->d_grid.get());
   PREP_TRY(h, cudaGetLastError());
-  PREP_TRY(h, cudaMemcpyAsync(h->h_grid, h->d_grid, kGridState * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
-  PREP_TRY(h, cudaStreamSynchronize(h->stream));
+  PREP_TRY(h, cudaMemcpyAsync(h->h_grid.get(), h->d_grid.get(), kGridState * sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream.get()));
+  PREP_TRY(h, cudaStreamSynchronize(h->stream.get()));
   if (h->h_grid[7]) return fail(h, 1, "voxel_grid: a kept point's cell floor(x / leaf) lies outside the int range");
   const int kept = (int)h->h_grid[6];
   if (kept == 0) return 0;
@@ -570,20 +558,20 @@ int run_voxel_grid(vgicp_prep_handle h, const float* points, size_t n, size_t st
   // 2. keys + digit histograms, the sort carrying x y z and the input index
   const size_t sb = sort_scratch_bytes(ni, passes);
   PREP_TRY(h, h->gscratch.reserve(sb));
-  PREP_TRY(h, cudaMemsetAsync(h->gscratch.p, 0, sb, h->stream));
+  PREP_TRY(h, cudaMemsetAsync(h->gscratch.p, 0, sb, h->stream.get()));
   const int hb = (ni + kSortThreads * 8 - 1) / (kSortThreads * 8);
-  k_grid_keys<<<hb < 4 * kNumSMs ? hb : 4 * kNumSMs, kSortThreads, 0, h->stream>>>(h->pts4.p, ni, inv, flt, make_int3(lo[0], lo[1], lo[2]), (unsigned)div[0],
+  k_grid_keys<<<hb < 4 * kNumSMs ? hb : 4 * kNumSMs, kSortThreads, 0, h->stream.get()>>>(h->pts4.p, ni, inv, flt, make_int3(lo[0], lo[1], lo[2]), (unsigned)div[0],
                                                                                    (unsigned)(div[0] * div[1]), V, passes, h->gkeys[0].p,
                                                                                    reinterpret_cast<unsigned*>(h->gscratch.p));
   PREP_TRY(h, cudaGetLastError());
   PREP_TRY(h, launch_sort_pairs<unsigned>(h->gkeys[0].p, h->gvals[0].p, h->gkeys[1].p, h->gvals[1].p, ni, key_bits, h->gscratch.p, true, h->pts4.p, h->gsorted4.p, nullptr,
-                                          h->stream));
+                                          h->stream.get()));
   const unsigned* keys = h->gkeys[passes & 1].p;
   // 3. the voxels that reach the minimum, ranked; 4. their centroids
   const int chunks = (kept + kRankThreads - 1) / kRankThreads;
-  PREP_TRY(h, lookback_next(h->chunk_state, h->chunk_epoch, chunks, h->stream));
+  PREP_TRY(h, lookback_next(h->chunk_state, h->chunk_epoch, chunks, h->stream.get()));
   PREP_TRY(h, h->gvstart.reserve((size_t)kept));
-  k_grid_heads<<<chunks, kRankThreads, 0, h->stream>>>(keys, kept, min_points, h->chunk_state.p, h->chunk_epoch, h->gvstart.p, h->d_grid);
+  k_grid_heads<<<chunks, kRankThreads, 0, h->stream.get()>>>(keys, kept, min_points, h->chunk_state.p, h->chunk_epoch, h->gvstart.p, h->d_grid.get());
   PREP_TRY(h, cudaGetLastError());
   float* d_out = out;
   size_t out_cap = cap;
@@ -607,14 +595,14 @@ int run_voxel_grid(vgicp_prep_handle h, const float* points, size_t n, size_t st
     case 8: PREP_TRY(h, (launch_centroids<8>(h, d_in, sf, off, keys, kept, cblocks, d_out, out_cap))); break;
     default: return fail(h, 1, "voxel_grid: unsupported field count");
   }
-  PREP_TRY(h, cudaMemcpyAsync(h->h_grid + 8, h->d_grid + 8, sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream));
-  PREP_TRY(h, cudaStreamSynchronize(h->stream));
+  PREP_TRY(h, cudaMemcpyAsync(h->h_grid.get() + 8, h->d_grid.get() + 8, sizeof(unsigned), cudaMemcpyDeviceToHost, h->stream.get()));
+  PREP_TRY(h, cudaStreamSynchronize(h->stream.get()));
   const size_t m = h->h_grid[8];
   *n_out = m;
   if (m > cap) return fail(h, 1, "voxel_grid: output capacity too small (n points always suffice)");
   if (!out_on_device && m > 0) {
-    PREP_TRY(h, cudaMemcpyAsync(out, d_out, m * rec * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-    PREP_TRY(h, cudaStreamSynchronize(h->stream));
+    PREP_TRY(h, cudaMemcpyAsync(out, d_out, m * rec * sizeof(float), cudaMemcpyDeviceToHost, h->stream.get()));
+    PREP_TRY(h, cudaStreamSynchronize(h->stream.get()));
   }
   return 0;
 }

@@ -39,14 +39,13 @@ struct Cloud {
   // each cloud has its own stream: the stage-1 work of target and source overlaps on the GPU; `ready` marks the end of the
   // last operation enqueued for this cloud
   cudaStream_t st = nullptr;
-  cudaEvent_t ready = nullptr;
+  Event ready;
   DevBuf<unsigned char> staging;
   DevBuf<unsigned char> knn_scratch;
   const float4* knn_sorted = nullptr;  // the cloud in the k-NN grid's Morton order (inside knn_scratch), original index in .w
   int knn_q_begin = 0, knn_q_end = 0;  // sorted positions whose neighbour rows the last find_neighbors computed
   int arena_slot = 0;                  // which half of the exchange arena holds this cloud's covariances (stage-1 sharding)
   unsigned long long arena_seq = 0;    // slices delivered for this cloud so far
-  void release() { pts.release(); nbr.release(); covA.release(); covB.release(); staging.release(); knn_scratch.release(); }
 };
 
 constexpr long long kDenseMaxCells = 16ll << 20;  // 64 MB of cell ids per map at most
@@ -57,10 +56,10 @@ struct VoxelMap {
   bool pending = false;    // first insertion attempt enqueued, outcome not yet read (voxelmap_finish completes the build)
   int pending_B = 0;
   bool v_pending = false;  // num_voxels still in flight
-  cudaEvent_t ev_attempt = nullptr, ev_done = nullptr;
+  Event ev_attempt, ev_done;
   int ndt = 0;             // 1: built from the points alone + MIN_EIG (NDT), 0: from points + covariances (VGICP)
-  int* d_counters = nullptr;  // [0] fail count, [1] num_voxels, [2..4] / [5..7] min / max voxel coordinate, [8] set_neighbors verdict
-  int* h_counters = nullptr;  // pinned
+  DevPtr<int[]> d_counters;   // [0] fail count, [1] num_voxels, [2..4] / [5..7] min / max voxel coordinate, [8] set_neighbors verdict
+  HostPtr<int[]> h_counters;  // pinned
   DevBuf<unsigned long long> chunk_state;  // k_table_assign_ids look-back (epoch-tagged block totals)
   unsigned chunk_epoch = 0;
   DevBuf<int> dense_cells;    // direct-mapped voxel index over the bounding box (evaluation kernels), when it fits
@@ -80,11 +79,6 @@ struct VoxelMap {
   DevBuf<unsigned> sort_keys[2], sort_vals[2];
   DevBuf<unsigned char> sort_scratch;
   DevBuf<int2> segments;
-  void release() {
-    buckets.release(); vox.release(); coords.release(); slots.release(); slot_of_point.release(); dense_cells.release(); chunk_state.release();
-    for (int j = 0; j < 2; j++) { sort_keys[j].release(); sort_vals[j].release(); }
-    sort_scratch.release(); segments.release();
-  }
 };
 
 // Where the evaluation kernels leave their results: `rows` records of `len` doubles, with the partial sums and tickets of their
@@ -94,10 +88,10 @@ struct EvalChannel {
   int rows = 0;
   size_t len = 0;
   DevBuf<double> partials;
-  unsigned int* tickets = nullptr;           // [rows]: zero before the first launch; reset by each row's last block
-  double* d_out = nullptr;                   // [rows][len] (throughput hint)
-  double* h_out = nullptr;                   // pinned + mapped, same shape (latency hint)
-  unsigned long long* h_done = nullptr;      // pinned + mapped per-row completion words
+  DevPtr<unsigned int[]> tickets;              // [rows]: zero before the first launch; reset by each row's last block
+  DevPtr<double[]> d_out;                      // [rows][len] (throughput hint)
+  HostPtr<double[]> h_out;                     // pinned + mapped, same shape (latency hint)
+  HostPtr<unsigned long long[]> h_done;        // pinned + mapped per-row completion words
   unsigned long long seq = 0;                // the current launch's (or round's) sequence number
   struct Dest {
     double* out;
@@ -105,32 +99,30 @@ struct EvalChannel {
     unsigned long long seq;
   };
 
-  // fixed-size buffers at the first call; the partial sums grow
+  // fixed-size buffers at the first call (each one a failed call left missing at the next); the partial sums grow.  The shape is
+  // the same at every call on a channel.
   cudaError_t open(int n_rows, size_t rec_len, size_t n_partials, cudaStream_t st) {
-    if (!h_out) {
-      rows = n_rows;
-      len = rec_len;
-      cudaError_t e = cudaMalloc(&tickets, rows * sizeof(unsigned int));
-      if (e == cudaSuccess) e = cudaMemsetAsync(tickets, 0, rows * sizeof(unsigned int), st);
-      if (e == cudaSuccess) e = cudaMalloc(&d_out, rows * len * sizeof(double));
-      if (e == cudaSuccess) e = cudaHostAlloc(&h_done, rows * sizeof(unsigned long long), cudaHostAllocMapped);
-      if (e == cudaSuccess) memset(h_done, 0, rows * sizeof(unsigned long long));
-      if (e == cudaSuccess) e = cudaHostAlloc(&h_out, rows * len * sizeof(double), cudaHostAllocMapped);  // (last: it marks the set as complete)
-      if (e != cudaSuccess) return e;
+    rows = n_rows;
+    len = rec_len;
+    cudaError_t e = cudaSuccess;
+    if (!tickets) {
+      if ((e = device_alloc(tickets, rows * sizeof(unsigned int))) != cudaSuccess) return e;
+      if ((e = cudaMemsetAsync(tickets.get(), 0, rows * sizeof(unsigned int), st)) != cudaSuccess) {
+        tickets.reset();
+        return e;
+      }
     }
+    if (!d_out && (e = device_alloc(d_out, rows * len * sizeof(double))) != cudaSuccess) return e;
+    if (!h_done) {
+      if ((e = host_alloc(h_done, rows * sizeof(unsigned long long), cudaHostAllocMapped)) != cudaSuccess) return e;
+      memset(h_done.get(), 0, rows * sizeof(unsigned long long));
+    }
+    if (!h_out && (e = host_alloc(h_out, rows * len * sizeof(double), cudaHostAllocMapped)) != cudaSuccess) return e;
     return partials.reserve(n_partials);
-  }
-  void release() {
-    partials.release();
-    if (tickets) cudaFree(tickets);
-    if (d_out) cudaFree(d_out);
-    if (h_out) cudaFreeHost(h_out);
-    if (h_done) cudaFreeHost(h_done);
-    *this = EvalChannel();
   }
   // where a launch writes rows [row0, ...) under the execution hint
   Dest dest(bool direct, int row0 = 0) const {
-    return {(direct ? h_out : d_out) + (size_t)row0 * len, direct ? h_done + row0 : nullptr, seq};
+    return {(direct ? h_out.get() : d_out.get()) + (size_t)row0 * len, direct ? h_done.get() + row0 : nullptr, seq};
   }
   int wait(vgicp_handle h, int n, size_t count);
 };
@@ -139,7 +131,7 @@ struct EvalChannel {
 
 struct vgicp_context {
   int device = 0;
-  cudaStream_t stream = nullptr;
+  Stream stream;
   std::string err;
   uint64_t launches = 0;
 
@@ -160,17 +152,18 @@ struct vgicp_context {
   Pose lin;  // linearized_x (float)
 
   DevBuf<unsigned char> staging;    // main-stream scratch (transform_source, fitness score)
-  cudaStream_t stream_b = nullptr;  // second cloud stream
-  cudaEvent_t ev_copy = nullptr;    // "host buffer consumed" marker of set_cloud
+  Stream stream_b;                  // second cloud stream
+  Event ev_copy;                    // "host buffer consumed" marker of set_cloud
   // multi-GPU source sharding
-  CommMailbox* comm_box = nullptr;               // this rank's mailbox (device memory, IPC-exported)
-  CommMailbox* comm_peers[kCommMaxRanks] = {};   // mapped peer mailboxes (own included)
+  DevPtr<CommMailbox> comm_box;                  // this rank's mailbox (device memory, IPC-exported)
+  IpcPtr<CommMailbox> comm_peers[kCommMaxRanks];  // mapped peer mailboxes (empty at comm_rank: that one is comm_box)
   int comm_rank = 0, comm_ranks = 0;
   unsigned long long comm_seq = 0;
   int shard_begin = 0, shard_end = -1;           // evaluations cover source points [begin, end)
   // stage-1 sharding: exchange arena (covariances of both clouds + delivery flags), own and peers' (IPC-mapped)
-  unsigned char* arena = nullptr;
-  unsigned char* arena_peers[kCommMaxRanks] = {};
+  DevPtr<unsigned char[]> arena;
+  IpcPtr<unsigned char[]> arena_peers[kCommMaxRanks];  // (empty at comm_rank: that one is arena)
+  bool arena_mapped = false;                         // vgicp_comm_init_arena has mapped every rank's arena
   size_t arena_points = 0;
   int stage1_sharding = 0;
   int speculate = 1;  // LM trial evaluations also linearise at the trial pose (vgicp_set_speculation)
@@ -181,8 +174,8 @@ struct vgicp_context {
   // of single-pose state (lin, eval) as it was; opened at the first multi-pose call: [kMultiMaxHyp][kMultiOut], partials
   // [rows][grid][kLinStride]
   EvalChannel multi;
-  unsigned char* d_multi_in = nullptr;      // per-launch input: poses [hypotheses][2], then the row -> hypothesis list
-  unsigned char* h_multi_in = nullptr;      // pinned staging of d_multi_in
+  DevPtr<unsigned char[]> d_multi_in;   // per-launch input: poses [hypotheses][2], then the row -> hypothesis list
+  HostPtr<unsigned char[]> h_multi_in;  // pinned staging of d_multi_in
 
   // NDT (NDTCudaCore, ndt_cuda.cu): 0 = VGICP problem, 1 = NDT point-to-distribution, 2 = NDT distribution-to-distribution
   int problem = 0;
@@ -194,7 +187,7 @@ struct vgicp_context {
   bool ndt_ready = false;
 
   // local map (vgicp_append_source_to_target / vgicp_crop_target)
-  cudaEvent_t ev_append = nullptr;  // end of the last append: the source's stream waits for it before the source is overwritten
+  Event ev_append;                  // end of the last append: the source's stream waits for it before the source is overwritten
   DevBuf<int> crop_rank;            // per target point: rank among the points that pass the radius test, or -1
   DevBuf<unsigned long long> crop_state;  // k_crop_rank look-back (epoch-tagged block totals)
   unsigned crop_epoch = 0;
@@ -203,15 +196,15 @@ struct vgicp_context {
 
   // optional per-kernel timing (vgicp_set_profiling): CUDA events on the handle's stream around every launch
   bool prof_on = false;
-  struct ProfRec { int cat; cudaEvent_t a, b; };
+  struct ProfRec { int cat; Event a, b; };
   std::vector<ProfRec> prof_pending;
-  std::vector<cudaEvent_t> prof_pool;
+  std::vector<Event> prof_pool;
   double prof_ms[VGICP_PROF_NUM_CATEGORIES] = {0};
   uint64_t prof_launches[VGICP_PROF_NUM_CATEGORIES] = {0};
 
   // motion compensation (vgicp_deskew_source); last, so that no other member moves, and created at the first call, so that a handle
   // that never deskews does no extra work
-  cudaEvent_t ev_deskew = nullptr;  // end of the work enqueued on the main stream: the in-place deskew must not overtake its reads
+  Event ev_deskew;                  // end of the work enqueued on the main stream: the in-place deskew must not overtake its reads
   std::vector<float> deskew_times;  // the caller's timestamps, packed contiguously
 
   // vgicp_register with resident clouds: the k-NN search and covariances of both clouds and the first voxel-map insertion attempt
@@ -219,7 +212,7 @@ struct vgicp_context {
   struct Stage1Graph {
     std::vector<uintptr_t> seen;  // key of the last eager stage 1 (a second call with the same key captures)
     std::vector<uintptr_t> key;   // key of `exec`
-    cudaGraphExec_t exec = nullptr;
+    GraphExec exec;
     const float4* sorted[2] = {nullptr, nullptr};  // target / source k-NN order (host state the enqueue code leaves behind)
     int pending_B = 0;
     uint64_t launches = 0;  // kernel nodes, counted as launches on every replay
@@ -271,26 +264,26 @@ int fail(vgicp_handle h, int code, const std::string& msg) {
   return code;
 }
 
-cudaEvent_t prof_event(vgicp_handle h) {
-  if (!h->prof_pool.empty()) {
-    cudaEvent_t e = h->prof_pool.back();
+Event prof_event(vgicp_handle h) {
+  Event e;
+  if (h->prof_pool.empty()) {
+    event_create(e, cudaEventDefault);
+  } else {
+    e = std::move(h->prof_pool.back());
     h->prof_pool.pop_back();
-    return e;
   }
-  cudaEvent_t e = nullptr;
-  cudaEventCreate(&e);
   return e;
 }
 inline void prof_begin(vgicp_handle h, int cat, cudaStream_t st) {
   h->prof_launches[cat]++;
   if (!h->prof_on) return;
   vgicp_context::ProfRec r{cat, prof_event(h), prof_event(h)};
-  cudaEventRecord(r.a, st);
-  h->prof_pending.push_back(r);
+  cudaEventRecord(r.a.get(), st);
+  h->prof_pending.push_back(std::move(r));
 }
 inline void prof_end(vgicp_handle h, cudaStream_t st) {
   if (!h->prof_on) return;
-  cudaEventRecord(h->prof_pending.back().b, st);
+  cudaEventRecord(h->prof_pending.back().b.get(), st);
 }
 // every kernel launch of the library goes through here: counts it, optionally brackets it with events on its stream
 #define KLAUNCH_ST(h, st, cat, ...) \
@@ -300,7 +293,7 @@ inline void prof_end(vgicp_handle h, cudaStream_t st) {
     prof_end(h, st);                \
     (h)->launches++;                \
   } while (0)
-#define KLAUNCH(h, cat, ...) KLAUNCH_ST(h, (h)->stream, cat, __VA_ARGS__)
+#define KLAUNCH(h, cat, ...) KLAUNCH_ST(h, (h)->stream.get(), cat, __VA_ARGS__)
 
 #define CU_TRY(h, expr)                                                                                       \
   do {                                                                                                        \
@@ -454,18 +447,18 @@ int set_cloud(vgicp_handle h, Cloud& c, const float* xyz, size_t n, size_t strid
   if (on_device) {  // caller's buffer already lives in this GPU's memory: read it in place (stream-ordered)
     KLAUNCH_ST(h, c.st, VGICP_PROF_UNPACK, k_unpack_points<<<blocks_for(n, 256), 256, 0, c.st>>>(reinterpret_cast<const unsigned char*>(xyz), stride, (int)n, c.pts.p));
     CU_TRY(h, cudaGetLastError());
-    CU_TRY(h, cudaEventRecord(c.ready, c.st));
+    CU_TRY(h, cudaEventRecord(c.ready.get(), c.st));
     return VGICP_OK;
   }
   CU_TRY(h, c.staging.reserve(n * stride));
   CU_TRY(h, cudaMemcpyAsync(c.staging.p, xyz, n * stride, cudaMemcpyHostToDevice, c.st));
   // the caller may free/modify xyz after return: pageable copies are staged synchronously by the driver, pinned ones are
   // not -> wait for the copy itself (an event right behind it), not for the kernels that follow
-  CU_TRY(h, cudaEventRecord(h->ev_copy, c.st));
+  CU_TRY(h, cudaEventRecord(h->ev_copy.get(), c.st));
   KLAUNCH_ST(h, c.st, VGICP_PROF_UNPACK, k_unpack_points<<<blocks_for(n, 256), 256, 0, c.st>>>(c.staging.p, stride, (int)n, c.pts.p));
   CU_TRY(h, cudaGetLastError());
-  CU_TRY(h, cudaEventRecord(c.ready, c.st));
-  CU_TRY(h, cudaEventSynchronize(h->ev_copy));
+  CU_TRY(h, cudaEventRecord(c.ready.get(), c.st));
+  CU_TRY(h, cudaEventSynchronize(h->ev_copy.get()));
   return VGICP_OK;
 }
 
@@ -476,11 +469,11 @@ int set_neighbors(vgicp_handle h, Cloud& c, int k, const int* idx, size_t nk) {
   CU_TRY(h, cudaMemcpyAsync(c.nbr.p, idx, nk * sizeof(int), cudaMemcpyHostToDevice, c.st));
   // an index outside [0, n) would be an illegal address in k_covariance_knn and poison the context of every handle of the process:
   // one pass over the table, the verdict comes back with the synchronisation the copy needs anyway
-  int* bad = h->map.d_counters + 8;
+  int* bad = h->map.d_counters.get() + 8;
   CU_TRY(h, cudaMemsetAsync(bad, 0, sizeof(int), c.st));
   KLAUNCH_ST(h, c.st, VGICP_PROF_OTHER, k_validate_indices<<<blocks_for(nk, 256) < 8 * kNumSMs ? blocks_for(nk, 256) : 8 * kNumSMs, 256, 0, c.st>>>(c.nbr.p, nk, c.n, bad));
   CU_TRY(h, cudaGetLastError());
-  CU_TRY(h, cudaMemcpyAsync(h->map.h_counters + 8, bad, sizeof(int), cudaMemcpyDeviceToHost, c.st));
+  CU_TRY(h, cudaMemcpyAsync(h->map.h_counters.get() + 8, bad, sizeof(int), cudaMemcpyDeviceToHost, c.st));
   CU_TRY(h, cudaStreamSynchronize(c.st));
   neighbors_set(c, h->map.h_counters[8] != 0 ? 0 : k);
   if (c.k == 0) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "set_neighbors: neighbour index outside [0, num_points)");
@@ -493,7 +486,7 @@ int find_neighbors(vgicp_handle h, Cloud& c, int k) {
   CU_TRY(h, c.nbr.reserve((size_t)c.n * k));
   CU_TRY(h, c.knn_scratch.reserve(knn_grid_scratch_bytes(c.n, nullptr, nullptr)));
   int q_begin = 0, q_end = c.n;
-  if (h->stage1_sharding && h->comm_ranks > 1 && h->arena_peers[h->comm_rank]) {  // this rank's slice of the queries (sorted positions)
+  if (h->stage1_sharding && h->comm_ranks > 1 && h->arena_mapped) {  // this rank's slice of the queries (sorted positions)
     const long long base = c.n / h->comm_ranks, rem = c.n % h->comm_ranks, r = h->comm_rank;
     q_begin = (int)(r * base + (r < rem ? r : rem));
     q_end = q_begin + (int)base + (r < rem ? 1 : 0);
@@ -504,7 +497,7 @@ int find_neighbors(vgicp_handle h, Cloud& c, int k) {
   KLAUNCH_ST(h, c.st, VGICP_PROF_KNN, ke = launch_knn_grid(c.pts.p, c.n, k, c.nbr.p, c.knn_scratch.p, c.knn_scratch.cap, q_begin, q_end, &nl, &sorted, c.st));
   h->launches += nl > 0 ? nl - 1 : 0;
   CU_TRY(h, ke);
-  CU_TRY(h, cudaEventRecord(c.ready, c.st));
+  CU_TRY(h, cudaEventRecord(c.ready.get(), c.st));
   neighbors_set(c, k, sorted, q_begin, q_end);
   return VGICP_OK;
 }
@@ -514,7 +507,7 @@ int calc_covariances(vgicp_handle h, Cloud& c, int method) {
   if (method < 0 || method > 4) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "calculate_covariances: bad regularization method");
   CU_TRY(h, c.covA.reserve(c.n));
   CU_TRY(h, c.covB.reserve(c.n));
-  const bool sharded = h->stage1_sharding && h->comm_ranks > 1 && h->arena_peers[h->comm_rank] && c.knn_sorted && (c.knn_q_begin > 0 || c.knn_q_end < c.n);
+  const bool sharded = h->stage1_sharding && h->comm_ranks > 1 && h->arena_mapped && c.knn_sorted && (c.knn_q_begin > 0 || c.knn_q_end < c.n);
   if (c.n > 0 && sharded) {
     // this rank computed the neighbour rows of a slice only: covariances of that slice go straight into every rank's arena
     // (peer stores), then the ranks tell each other and wait -- all in stream order, the host does not block
@@ -523,7 +516,7 @@ int calc_covariances(vgicp_handle h, Cloud& c, int method) {
     float2* pb[kCommMaxRanks];
     ArenaPeers ap;
     for (int r = 0; r < kCommMaxRanks; r++) {
-      unsigned char* base = r < h->comm_ranks ? h->arena_peers[r] : nullptr;
+      unsigned char* base = r >= h->comm_ranks ? nullptr : r == h->comm_rank ? h->arena.get() : h->arena_peers[r].get();
       ap.hdr[r] = reinterpret_cast<CommArenaHeader*>(base);
       pa[r] = base ? reinterpret_cast<float4*>(base + kCommArenaHeaderBytes + (size_t)c.arena_slot * h->arena_points * 24) : nullptr;
       pb[r] = base ? reinterpret_cast<float2*>(reinterpret_cast<unsigned char*>(pa[r]) + h->arena_points * 16) : nullptr;
@@ -540,7 +533,7 @@ int calc_covariances(vgicp_handle h, Cloud& c, int method) {
     CU_TRY(h, ke);
   }
   covariances_set(c);
-  CU_TRY(h, cudaEventRecord(c.ready, c.st));
+  CU_TRY(h, cudaEventRecord(c.ready.get(), c.st));
   if (method == VGICP_REG_NORMALIZED_MIN_EIG)
     return fail(h, VGICP_ERR_UNSUPPORTED, "unimplemented covariance regularization method was selected (NORMALIZED_MIN_EIG has no GPU path in the reference either); raw covariances kept");
   return VGICP_OK;
@@ -561,7 +554,7 @@ int calc_covariances_rbf(vgicp_handle h, Cloud& c, int method) {
     CU_TRY(h, ke);
   }
   covariances_set(c);
-  CU_TRY(h, cudaEventRecord(c.ready, c.st));
+  CU_TRY(h, cudaEventRecord(c.ready.get(), c.st));
   if (method == VGICP_REG_NORMALIZED_MIN_EIG) return fail(h, VGICP_ERR_UNSUPPORTED, "unimplemented covariance regularization method was selected; raw covariances kept");
   return VGICP_OK;
 }
@@ -603,7 +596,7 @@ int set_covariances(vgicp_handle h, Cloud& c, const float* in9, size_t n) {
     CU_TRY(h, cudaStreamSynchronize(c.st));
   }
   covariances_set(c);
-  CU_TRY(h, cudaEventRecord(c.ready, c.st));
+  CU_TRY(h, cudaEventRecord(c.ready.get(), c.st));
   return VGICP_OK;
 }
 
@@ -632,20 +625,20 @@ int voxelmap_attempt(vgicp_handle h, Cloud& t, VoxelMap& m, int B, int count) {
   int B_last = B;
   for (int j = 1; j < count && B_last < (1 << 28); j++) B_last *= 2;
   CU_TRY(h, m.slots.reserve(B_last));
-  int* skip = m.d_counters + 9;
+  int* skip = m.d_counters.get() + 9;
   CU_TRY(h, cudaMemsetAsync(skip, 0, sizeof(int), t.st));
   int Bj = B;
   for (int j = 0; j < count && Bj <= B_last; j++, Bj *= 2) {
-    CU_TRY(h, cudaMemsetAsync(m.d_counters, 0, sizeof(int), t.st));
+    CU_TRY(h, cudaMemsetAsync(m.d_counters.get(), 0, sizeof(int), t.st));
     KLAUNCH_ST(h, t.st, VGICP_PROF_VOXELMAP, k_fill_i32<<<blocks_for(Bj, 256), 256, 0, t.st>>>(m.slots.p, -1, (size_t)Bj, skip));
     KLAUNCH_ST(h, t.st, VGICP_PROF_VOXELMAP, k_table_insert<<<blocks_for(n, 256), 256, 0, t.st>>>(m.coords.p, n, m.slots.p, (unsigned)(Bj - 1), m.max_scan, skip));
     KLAUNCH_ST(h, t.st, VGICP_PROF_VOXELMAP,
-               k_table_lookup_points<<<blocks_for(n, 256), 256, 0, t.st>>>(m.coords.p, n, m.slots.p, (unsigned)(Bj - 1), m.max_scan, m.slot_of_point.p, m.d_counters, skip));
-    KLAUNCH_ST(h, t.st, VGICP_PROF_VOXELMAP, k_table_verdict<<<1, 1, 0, t.st>>>(m.d_counters, n, Bj));
+               k_table_lookup_points<<<blocks_for(n, 256), 256, 0, t.st>>>(m.coords.p, n, m.slots.p, (unsigned)(Bj - 1), m.max_scan, m.slot_of_point.p, m.d_counters.get(), skip));
+    KLAUNCH_ST(h, t.st, VGICP_PROF_VOXELMAP, k_table_verdict<<<1, 1, 0, t.st>>>(m.d_counters.get(), n, Bj));
   }
   CU_TRY(h, cudaGetLastError());
-  CU_TRY(h, cudaMemcpyAsync(m.h_counters + 9, m.d_counters + 9, sizeof(int), cudaMemcpyDeviceToHost, t.st));
-  CU_TRY(h, cudaEventRecord(m.ev_attempt, t.st));
+  CU_TRY(h, cudaMemcpyAsync(m.h_counters.get() + 9, m.d_counters.get() + 9, sizeof(int), cudaMemcpyDeviceToHost, t.st));
+  CU_TRY(h, cudaEventRecord(m.ev_attempt.get(), t.st));
   m.pending_B = B_last;
   return VGICP_OK;
 }
@@ -661,10 +654,10 @@ int voxelmap_begin(vgicp_handle h, Cloud& t, VoxelMap& m) {
   const int n = t.n;
   CU_TRY(h, m.coords.reserve(n));
   CU_TRY(h, m.slot_of_point.reserve(n));
-  CU_TRY(h, cudaMemsetAsync(m.d_counters + 2, 0x7f, 3 * sizeof(int), t.st));  // running minimum: starts at 0x7f7f7f7f
-  CU_TRY(h, cudaMemsetAsync(m.d_counters + 5, 0x80, 3 * sizeof(int), t.st));  // running maximum: starts at 0x80808080
-  KLAUNCH_ST(h, t.st, VGICP_PROF_VOXELMAP, k_voxel_coords<<<blocks_for(n, 256), 256, 0, t.st>>>(t.pts.p, n, m.res, m.coords.p, m.d_counters + 2));
-  CU_TRY(h, cudaMemcpyAsync(m.h_counters + 2, m.d_counters + 2, 6 * sizeof(int), cudaMemcpyDeviceToHost, t.st));
+  CU_TRY(h, cudaMemsetAsync(m.d_counters.get() + 2, 0x7f, 3 * sizeof(int), t.st));  // running minimum: starts at 0x7f7f7f7f
+  CU_TRY(h, cudaMemsetAsync(m.d_counters.get() + 5, 0x80, 3 * sizeof(int), t.st));  // running maximum: starts at 0x80808080
+  KLAUNCH_ST(h, t.st, VGICP_PROF_VOXELMAP, k_voxel_coords<<<blocks_for(n, 256), 256, 0, t.st>>>(t.pts.p, n, m.res, m.coords.p, m.d_counters.get() + 2));
+  CU_TRY(h, cudaMemcpyAsync(m.h_counters.get() + 2, m.d_counters.get() + 2, 6 * sizeof(int), cudaMemcpyDeviceToHost, t.st));
   // small clouds pass with the initial 8192 buckets (1082 voxels at 17 k points); large ones are given three sizes to try at once
   int rc = voxelmap_attempt(h, t, m, m.init_num_buckets, n > 200000 ? 3 : 1);
   if (rc) return rc;
@@ -677,7 +670,7 @@ int voxelmap_finish(vgicp_handle h, Cloud& t, VoxelMap& m) {
   const int n = t.n;
   int B = 0;
   for (;;) {  // :265 (no upper bound in the reference; bounded here)
-    CU_TRY(h, cudaEventSynchronize(m.ev_attempt));
+    CU_TRY(h, cudaEventSynchronize(m.ev_attempt.get()));
     if (m.h_counters[9] != 0) { B = m.h_counters[9]; break; }  // :280, decided on the device
     B = m.pending_B * 2;
     if (B > (1 << 28)) { m.pending = false; return fail(h, VGICP_ERR_INVALID_ARGUMENT, "create_target_voxelmap: hash table would exceed 2^28 buckets"); }
@@ -694,7 +687,7 @@ int voxelmap_finish(vgicp_handle h, Cloud& t, VoxelMap& m) {
   // are: 84 x 84 x 10 cells for the 17k fixture, 300 x 300 x 40 at 1M points / 0.5 m); otherwise they probe the hash table
   m.dense.cells = nullptr;
   if (h->voxel_index_mode == 0) {
-    const int* hc = m.h_counters;
+    const int* hc = m.h_counters.get();
     const long long nx = (long long)hc[5] - hc[2] + 1, ny = (long long)hc[6] - hc[3] + 1, nz = (long long)hc[7] - hc[4] + 1;
     if (nx > 0 && ny > 0 && nz > 0 && nx <= kDenseMaxCells && ny <= kDenseMaxCells && nz <= kDenseMaxCells && nx * ny <= kDenseMaxCells && nx * ny * nz <= kDenseMaxCells) {
       const size_t cells = (size_t)(nx * ny * nz);
@@ -707,7 +700,7 @@ int voxelmap_finish(vgicp_handle h, Cloud& t, VoxelMap& m) {
     const int chunks = blocks_for(B, kRankThreads);
     CU_TRY(h, lookback_next(m.chunk_state, m.chunk_epoch, chunks, t.st));
     KLAUNCH_ST(h, t.st, VGICP_PROF_VOXELMAP,
-               k_table_assign_ids<<<chunks, kRankThreads, 0, t.st>>>(m.coords.p, m.slots.p, B, m.buckets.p, m.d_counters + 1, m.dense, m.chunk_state.p, m.chunk_epoch));
+               k_table_assign_ids<<<chunks, kRankThreads, 0, t.st>>>(m.coords.p, m.slots.p, B, m.buckets.p, m.d_counters.get() + 1, m.dense, m.chunk_state.p, m.chunk_epoch));
   }
   // voxel Gaussians: stable sort of the points by voxel id, then one warp per voxel adds its points in index order
   {
@@ -737,18 +730,18 @@ int voxelmap_finish(vgicp_handle h, Cloud& t, VoxelMap& m) {
     const unsigned* order = m.sort_vals[passes & 1].p;
     KLAUNCH_ST(h, t.st, VGICP_PROF_VOXELMAP, k_voxel_segments<<<blocks_for(n, 256), 256, 0, t.st>>>(skeys, n, invalid, m.segments.p));
     if (m.ndt) {
-      KLAUNCH_ST(h, t.st, VGICP_PROF_VOXELMAP, k_voxel_reduce<true><<<blocks_for(vmax, 4), 128, 0, t.st>>>(t.pts.p, nullptr, nullptr, order, m.segments.p, m.d_counters + 1, m.vox.p));
+      KLAUNCH_ST(h, t.st, VGICP_PROF_VOXELMAP, k_voxel_reduce<true><<<blocks_for(vmax, 4), 128, 0, t.st>>>(t.pts.p, nullptr, nullptr, order, m.segments.p, m.d_counters.get() + 1, m.vox.p));
       cudaError_t ke = cudaSuccess;
-      KLAUNCH_ST(h, t.st, VGICP_PROF_VOXELMAP, ke = launch_regularize_voxels(m.vox.p, m.d_counters + 1, vmax, VGICP_REG_MIN_EIG, t.st));  // ndt_cuda.cu:129,140
+      KLAUNCH_ST(h, t.st, VGICP_PROF_VOXELMAP, ke = launch_regularize_voxels(m.vox.p, m.d_counters.get() + 1, vmax, VGICP_REG_MIN_EIG, t.st));  // ndt_cuda.cu:129,140
       CU_TRY(h, ke);
     } else {
-      KLAUNCH_ST(h, t.st, VGICP_PROF_VOXELMAP, k_voxel_reduce<false><<<blocks_for(vmax, 4), 128, 0, t.st>>>(t.pts.p, t.covA.p, t.covB.p, order, m.segments.p, m.d_counters + 1, m.vox.p));
+      KLAUNCH_ST(h, t.st, VGICP_PROF_VOXELMAP, k_voxel_reduce<false><<<blocks_for(vmax, 4), 128, 0, t.st>>>(t.pts.p, t.covA.p, t.covB.p, order, m.segments.p, m.d_counters.get() + 1, m.vox.p));
     }
   }
   CU_TRY(h, cudaGetLastError());
-  CU_TRY(h, cudaMemcpyAsync(m.h_counters + 1, m.d_counters + 1, sizeof(int), cudaMemcpyDeviceToHost, t.st));
-  CU_TRY(h, cudaEventRecord(m.ev_done, t.st));
-  CU_TRY(h, cudaEventRecord(t.ready, t.st));
+  CU_TRY(h, cudaMemcpyAsync(m.h_counters.get() + 1, m.d_counters.get() + 1, sizeof(int), cudaMemcpyDeviceToHost, t.st));
+  CU_TRY(h, cudaEventRecord(m.ev_done.get(), t.st));
+  CU_TRY(h, cudaEventRecord(t.ready.get(), t.st));
   m.v_pending = true;
   m.built = true;
   return VGICP_OK;
@@ -758,7 +751,7 @@ int voxelmap_num_voxels(vgicp_handle h, Cloud& t, VoxelMap& m, int* nv) {
   int rc = voxelmap_finish(h, t, m);
   if (rc) return rc;
   if (m.v_pending) {
-    CU_TRY(h, cudaEventSynchronize(m.ev_done));
+    CU_TRY(h, cudaEventSynchronize(m.ev_done.get()));
     m.num_voxels = m.h_counters[1];
     m.v_pending = false;
   }
@@ -775,8 +768,8 @@ int ndt_prepare(vgicp_handle h);
 int sync_inputs(vgicp_handle h) {
   int rc = h->problem == 0 ? voxelmap_finish(h, h->target, h->map) : ndt_prepare(h);
   if (rc) return rc;
-  if (h->target.st != h->stream && h->target.ready) CU_TRY(h, cudaStreamWaitEvent(h->stream, h->target.ready, 0));
-  if (h->source.st != h->stream && h->source.ready) CU_TRY(h, cudaStreamWaitEvent(h->stream, h->source.ready, 0));
+  if (h->target.st != h->stream.get() && h->target.ready) CU_TRY(h, cudaStreamWaitEvent(h->stream.get(), h->target.ready.get(), 0));
+  if (h->source.st != h->stream.get() && h->source.ready) CU_TRY(h, cudaStreamWaitEvent(h->stream.get(), h->source.ready.get(), 0));
   return VGICP_OK;
 }
 
@@ -800,13 +793,13 @@ LinLaunch make_lin_launch(vgicp_handle h, const float4* pts, const float4* covA,
   a.robust_d2 = a.robust ? (float)(h->robust_scale * h->robust_scale) : 0.0f;
   a.pts = pts; a.covA = covA; a.covB = covB; a.n = n;
   a.comm_ranks = h->comm_ranks; a.comm_rank = h->comm_rank; a.comm_seq = 0;
-  for (int r = 0; r < kCommMaxRanks; r++) a.comm_peers[r] = h->comm_peers[r];
+  for (int r = 0; r < kCommMaxRanks; r++) a.comm_peers[r] = r >= h->comm_ranks ? nullptr : r == h->comm_rank ? h->comm_box.get() : h->comm_peers[r].get();
   a.buckets = m.buckets.p; a.mask = (unsigned)(m.num_buckets - 1); a.max_scan = m.max_scan; a.vox = m.vox.p;
   a.dense = m.dense;
   if (h->voxel_index_mode != 0) a.dense.cells = nullptr;
   a.offsets = h->d_offsets.p; a.n_off = (int)h->h_offsets.size(); a.res = m.res;
   a.Tlin = h->lin; a.Teval = h->lin;
-  a.partials = h->eval.partials.p; a.ticket = h->eval.tickets; a.out = h->eval.d_out;
+  a.partials = h->eval.partials.p; a.ticket = h->eval.tickets.get(); a.out = h->eval.d_out.get();
   a.done_flag = nullptr; a.done_seq = 0;
   // lanes per source point in the lookup phase: split the neighbour cells of a point over G lanes while the cloud is too small to
   // fill the GPU with one thread per point (latency-bound regime); one lane per point once it is large
@@ -860,7 +853,7 @@ bool with_lin_shape(int mode, int G, F&& f) {
 // robust flag as compile-time constants, launches the kernel and returns false when none exists for the shape.
 template <class F>
 int launch_eval(vgicp_handle h, int kind, bool robust, F&& launch) {
-  prof_begin(h, kind == kEvalError ? VGICP_PROF_ERROR : VGICP_PROF_LINEARIZE, h->stream);
+  prof_begin(h, kind == kEvalError ? VGICP_PROF_ERROR : VGICP_PROF_LINEARIZE, h->stream.get());
   bool launched;
   auto with_kind = [&](auto rb) {
     if (kind == kEvalSpec) launched = launch(IntC<kEvalSpec>{}, rb);
@@ -869,7 +862,7 @@ int launch_eval(vgicp_handle h, int kind, bool robust, F&& launch) {
   };
   if (robust) with_kind(std::true_type{});
   else with_kind(std::false_type{});
-  prof_end(h, h->stream);
+  prof_end(h, h->stream.get());
   if (!launched) return fail(h, VGICP_ERR_UNSUPPORTED, "no evaluation kernel for this offset table and lane split");
   h->launches++;
   CU_TRY(h, cudaGetLastError());
@@ -890,11 +883,11 @@ int launch_linearize(vgicp_handle h, const Pose& Teval, int kind) {
     constexpr int WHAT = decltype(what)::value;
     constexpr bool RB = decltype(rb)::value;
     if (L.stream) {
-      k_linearize_stream<WHAT, RB><<<L.grid, kLinThreads, sizeof(LinStreamSmem), h->stream>>>(a);
+      k_linearize_stream<WHAT, RB><<<L.grid, kLinThreads, sizeof(LinStreamSmem), h->stream.get()>>>(a);
       return true;
     }
     return with_lin_shape(h->offset_mode, L.G, [&](auto mode, auto g) {
-      k_linearize<decltype(mode)::value, WHAT, decltype(g)::value, RB><<<L.grid, kLinThreads, 0, h->stream>>>(a);
+      k_linearize<decltype(mode)::value, WHAT, decltype(g)::value, RB><<<L.grid, kLinThreads, 0, h->stream.get()>>>(a);
     });
   });
 }
@@ -928,16 +921,16 @@ int ndt_prepare(vgicp_handle h) {
     CU_TRY(h, h->ndt_src_covB.reserve(vs > 0 ? vs : 1));
     if (vs > 0)
       KLAUNCH_ST(h, s.st, VGICP_PROF_VOXELMAP,
-                 k_vox_to_cloud<<<blocks_for(vs, 256), 256, 0, s.st>>>(h->ndt_s.vox.p, h->ndt_s.d_counters + 1, h->ndt_src_pts.p, h->ndt_src_covA.p, h->ndt_src_covB.p));
+                 k_vox_to_cloud<<<blocks_for(vs, 256), 256, 0, s.st>>>(h->ndt_s.vox.p, h->ndt_s.d_counters.get() + 1, h->ndt_src_pts.p, h->ndt_src_covA.p, h->ndt_src_covB.p));
     CU_TRY(h, cudaGetLastError());
-    CU_TRY(h, cudaEventRecord(s.ready, s.st));
+    CU_TRY(h, cudaEventRecord(s.ready.get(), s.st));
     h->ndt_src_n = vs;
   } else {
     CU_TRY(h, h->ndt_src_covA.reserve(s.n));
     CU_TRY(h, h->ndt_src_covB.reserve(s.n));
     CU_TRY(h, cudaMemsetAsync(h->ndt_src_covA.p, 0, sizeof(float4) * (size_t)s.n, s.st));
     CU_TRY(h, cudaMemsetAsync(h->ndt_src_covB.p, 0, sizeof(float2) * (size_t)s.n, s.st));
-    CU_TRY(h, cudaEventRecord(s.ready, s.st));
+    CU_TRY(h, cudaEventRecord(s.ready.get(), s.st));
     h->ndt_src_n = s.n;
   }
   h->ndt_ready = true;
@@ -948,13 +941,13 @@ int ndt_prepare(vgicp_handle h) {
 // on the completion words, under the throughput hint by copying `count` doubles back behind the launch.
 int EvalChannel::wait(vgicp_handle h, int n, size_t count) {
   if (h->exec_hint == 0) {
-    const volatile unsigned long long* done = h_done;
+    const volatile unsigned long long* done = h_done.get();
     for (int r = 0; r < n; r++) {
       long spins = 0;
       while (done[r] != seq) {
         __builtin_ia32_pause();
         if (++spins > 2000000L) {  // ~a few ms without an answer: fall back to a blocking wait (also surfaces launch errors)
-          CU_TRY(h, cudaStreamSynchronize(h->stream));
+          CU_TRY(h, cudaStreamSynchronize(h->stream.get()));
           if (done[r] != seq) return fail(h, VGICP_ERR_CUDA, "evaluation kernel finished without publishing its result");
           break;
         }
@@ -962,8 +955,8 @@ int EvalChannel::wait(vgicp_handle h, int n, size_t count) {
     }
     __sync_synchronize();
   } else {
-    CU_TRY(h, cudaMemcpyAsync(h_out, d_out, count * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-    CU_TRY(h, cudaStreamSynchronize(h->stream));
+    CU_TRY(h, cudaMemcpyAsync(h_out.get(), d_out.get(), count * sizeof(double), cudaMemcpyDeviceToHost, h->stream.get()));
+    CU_TRY(h, cudaStreamSynchronize(h->stream.get()));
   }
   return VGICP_OK;
 }
@@ -976,19 +969,17 @@ int evaluate(vgicp_handle h, const Pose& Teval, int kind, const double** rec) {
   const size_t count = (h->comm_ranks > 1 || kind == kEvalSpec) ? kLinOutCommError + 1 : (kind == kEvalLinearize ? 43 : 1);
   if ((rc = h->eval.wait(h, 1, count))) return rc;
   if (h->comm_ranks > 1 && h->eval.h_out[kLinOutCommError] != 0.0) return fail(h, VGICP_ERR_COMM, "evaluate: a peer rank did not deliver its sums in time (vgicp_comm_error)");
-  *rec = h->eval.h_out;
+  *rec = h->eval.h_out.get();
   return VGICP_OK;
 }
 
 // ---- multi-pose evaluation (vgicp_align_multi, vgicp_evaluate_poses) -------------------------------------------------------
 // fixed-size buffers on first use; the partial sums grow with rows x grid (256 bytes per block and row)
 int multi_reserve(vgicp_handle h, int rows, int grid) {
-  if (!h->h_multi_in) {
-    const size_t in_bytes = (size_t)kMultiMaxHyp * (2 * sizeof(Pose) + sizeof(int)) + 16;
-    CU_TRY(h, cudaMalloc(&h->d_multi_in, in_bytes));
-    CU_TRY(h, cudaMallocHost(&h->h_multi_in, in_bytes));  // (last: it marks the pair as complete)
-  }
-  CU_TRY(h, h->multi.open(kMultiMaxHyp, kMultiOut, (size_t)rows * grid * kLinStride, h->stream));
+  const size_t in_bytes = (size_t)kMultiMaxHyp * (2 * sizeof(Pose) + sizeof(int)) + 16;
+  if (!h->d_multi_in) CU_TRY(h, device_alloc(h->d_multi_in, in_bytes));
+  if (!h->h_multi_in) CU_TRY(h, host_alloc(h->h_multi_in, in_bytes, cudaHostAllocDefault));
+  CU_TRY(h, h->multi.open(kMultiMaxHyp, kMultiOut, (size_t)rows * grid * kLinStride, h->stream.get()));
   return VGICP_OK;
 }
 
@@ -999,8 +990,8 @@ struct MultiRound {
   vgicp_handle h;
   int n_hyp;
   int n = 0;  // rows staged
-  Pose* poses = reinterpret_cast<Pose*>(h->h_multi_in);
-  int* rows = reinterpret_cast<int*>(h->h_multi_in + multi_rows_offset(n_hyp));
+  Pose* poses = reinterpret_cast<Pose*>(h->h_multi_in.get());
+  int* rows = reinterpret_cast<int*>(h->h_multi_in.get() + multi_rows_offset(n_hyp));
   // the next row: hypothesis i, evaluated at Te over the correspondences of Tl
   void add(int i, const double* Tl, const double* Te) {
     rows[n++] = i;
@@ -1010,7 +1001,7 @@ struct MultiRound {
   // a new sequence number for the round's records, and the copy
   int upload() {
     h->multi.seq++;
-    CU_TRY(h, cudaMemcpyAsync(h->d_multi_in, h->h_multi_in, multi_rows_offset(n_hyp) + (size_t)n * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    CU_TRY(h, cudaMemcpyAsync(h->d_multi_in.get(), h->h_multi_in.get(), multi_rows_offset(n_hyp) + (size_t)n * sizeof(int), cudaMemcpyHostToDevice, h->stream.get()));
     return VGICP_OK;
   }
 };
@@ -1022,10 +1013,10 @@ int launch_multi(vgicp_handle h, const LinLaunch& L, int n_hyp, int kind, bool c
   const LinArgs& a = L.a;
   const EvalChannel::Dest d = h->multi.dest(h->exec_hint == 0, row0);
   MultiArgs m;
-  m.hyp = reinterpret_cast<const int*>(h->d_multi_in + multi_rows_offset(n_hyp)) + row0;
-  m.poses = reinterpret_cast<const Pose*>(h->d_multi_in);
+  m.hyp = reinterpret_cast<const int*>(h->d_multi_in.get() + multi_rows_offset(n_hyp)) + row0;
+  m.poses = reinterpret_cast<const Pose*>(h->d_multi_in.get());
   m.partials = h->multi.partials.p;  // (the launches of a round run one after the other on the stream: slices and tickets are reused)
-  m.tickets = h->multi.tickets;
+  m.tickets = h->multi.tickets.get();
   m.out = d.out; m.done = d.done; m.done_seq = d.seq;
   m.src = src;
   const dim3 grid(L.grid, n);
@@ -1036,11 +1027,11 @@ int launch_multi(vgicp_handle h, const LinLaunch& L, int n_hyp, int kind, bool c
       constexpr bool COUNT = decltype(cnt)::value && WHAT != kEvalSpec;  // (the speculative evaluation counts no hits)
       constexpr bool SRC = decltype(per_source)::value;
       if (L.stream) {
-        k_linearize_stream_multi<WHAT, COUNT, RB, SRC><<<grid, kLinThreads, sizeof(LinStreamSmem), h->stream>>>(a, m);
+        k_linearize_stream_multi<WHAT, COUNT, RB, SRC><<<grid, kLinThreads, sizeof(LinStreamSmem), h->stream.get()>>>(a, m);
         return true;
       }
       return with_lin_shape(h->offset_mode, L.G, [&](auto mode, auto g) {
-        k_linearize_multi<decltype(mode)::value, WHAT, decltype(g)::value, COUNT, RB, SRC><<<grid, kLinThreads, 0, h->stream>>>(a, m);
+        k_linearize_multi<decltype(mode)::value, WHAT, decltype(g)::value, COUNT, RB, SRC><<<grid, kLinThreads, 0, h->stream.get()>>>(a, m);
       });
     };
     if (m.src) return with_rows(std::false_type{}, std::true_type{});  // (the multi-source rows count no hits)
@@ -1256,17 +1247,17 @@ int ct_evaluate(vgicp_handle h, const double* Tl, const double* xl, const double
     c.xe[j] = (float)xe[j];
   }
   c.partials = h->ct.partials.p;
-  c.ticket = h->ct.tickets;
+  c.ticket = h->ct.tickets.get();
   h->ct.seq++;
   const EvalChannel::Dest d = h->ct.dest(h->exec_hint == 0);
   c.out = d.out; c.done_flag = d.done; c.done_seq = d.seq;
   int rc = launch_eval(h, want_H ? kEvalLinearize : kEvalError, a.robust, [&](auto what, auto rb) {
     return with_lin_shape(h->offset_mode, L.G, [&](auto mode, auto g) {
-      k_linearize_ct<decltype(mode)::value, decltype(what)::value == kEvalLinearize, decltype(g)::value, decltype(rb)::value><<<L.grid, kLinThreads, 0, h->stream>>>(a, c);
+      k_linearize_ct<decltype(mode)::value, decltype(what)::value == kEvalLinearize, decltype(g)::value, decltype(rb)::value><<<L.grid, kLinThreads, 0, h->stream.get()>>>(a, c);
     });
   });
   if (rc || (rc = h->ct.wait(h, 1, want_H ? kCtValues : 1))) return rc;
-  *raw = h->ct.h_out;
+  *raw = h->ct.h_out.get();
   return VGICP_OK;
 }
 
@@ -1358,27 +1349,27 @@ int vgicp_create(int device, vgicp_handle* out) {
     delete h;
     return VGICP_ERR_NO_DEVICE;
   }
-  bool ok = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) == cudaSuccess;
-  ok = ok && cudaStreamCreateWithFlags(&h->stream_b, cudaStreamNonBlocking) == cudaSuccess;
-  ok = ok && cudaEventCreateWithFlags(&h->ev_copy, cudaEventDisableTiming) == cudaSuccess;
-  ok = ok && cudaEventCreateWithFlags(&h->ev_append, cudaEventDisableTiming) == cudaSuccess;
-  ok = ok && cudaEventCreateWithFlags(&h->target.ready, cudaEventDisableTiming) == cudaSuccess;
-  ok = ok && cudaEventCreateWithFlags(&h->source.ready, cudaEventDisableTiming) == cudaSuccess;
-  h->target.st = h->stream;    // the target (and its voxel map) is built on the main stream, where the evaluations run
-  h->source.st = h->stream_b;  // the source's stage 1 overlaps with it
+  bool ok = stream_create(h->stream, cudaStreamNonBlocking) == cudaSuccess;
+  ok = ok && stream_create(h->stream_b, cudaStreamNonBlocking) == cudaSuccess;
+  ok = ok && event_create(h->ev_copy, cudaEventDisableTiming) == cudaSuccess;
+  ok = ok && event_create(h->ev_append, cudaEventDisableTiming) == cudaSuccess;
+  ok = ok && event_create(h->target.ready, cudaEventDisableTiming) == cudaSuccess;
+  ok = ok && event_create(h->source.ready, cudaEventDisableTiming) == cudaSuccess;
+  h->target.st = h->stream.get();    // the target (and its voxel map) is built on the main stream, where the evaluations run
+  h->source.st = h->stream_b.get();  // the source's stage 1 overlaps with it
   for (VoxelMap* vm : {&h->map, &h->ndt_t, &h->ndt_s}) {
-    ok = ok && cudaMalloc(&vm->d_counters, 16 * sizeof(int)) == cudaSuccess;
-    ok = ok && cudaMallocHost(&vm->h_counters, 16 * sizeof(int)) == cudaSuccess;
-    ok = ok && cudaEventCreateWithFlags(&vm->ev_attempt, cudaEventDisableTiming) == cudaSuccess;
-    ok = ok && cudaEventCreateWithFlags(&vm->ev_done, cudaEventDisableTiming) == cudaSuccess;
+    ok = ok && device_alloc(vm->d_counters, 16 * sizeof(int)) == cudaSuccess;
+    ok = ok && host_alloc(vm->h_counters, 16 * sizeof(int), cudaHostAllocDefault) == cudaSuccess;
+    ok = ok && event_create(vm->ev_attempt, cudaEventDisableTiming) == cudaSuccess;
+    ok = ok && event_create(vm->ev_done, cudaEventDisableTiming) == cudaSuccess;
   }
   h->ndt_t.ndt = h->ndt_s.ndt = 1;
-  ok = ok && h->eval.open(1, 64, (size_t)kLinStreamMaxBlocks * kLinStride, h->stream) == cudaSuccess;
-  ok = ok && cudaStreamSynchronize(h->stream) == cudaSuccess;
+  ok = ok && h->eval.open(1, 64, (size_t)kLinStreamMaxBlocks * kLinStride, h->stream.get()) == cudaSuccess;
+  ok = ok && cudaStreamSynchronize(h->stream.get()) == cudaSuccess;
   // fast_vgicp_cuda.cu:28-29, with the table on the device as well: the correspondence getter reads it under every method
   ok = ok && vgicp_set_neighbor_search_method(h, VGICP_DIRECT1, -1.0) == VGICP_OK;
   if (!ok) {
-    vgicp_destroy(h);
+    delete h;
     return VGICP_ERR_CUDA;
   }
   *out = h;
@@ -1387,48 +1378,10 @@ int vgicp_create(int device, vgicp_handle* out) {
 
 int vgicp_destroy(vgicp_handle h) {
   if (!h) return VGICP_OK;
-  DeviceGuard g(h->device);
-  if (h->stream) cudaStreamSynchronize(h->stream);
-  if (h->stream_b) cudaStreamSynchronize(h->stream_b);
-  h->source.release();
-  h->target.release();
-  h->d_offsets.release();
-  h->staging.release();
+  DeviceGuard g(h->device);  // (the members free their resources on the handle's device)
+  if (h->stream) cudaStreamSynchronize(h->stream.get());
+  if (h->stream_b) cudaStreamSynchronize(h->stream_b.get());
   if (h->comm_ranks > 1) vgicp_comm_shutdown(h);
-  if (h->comm_box) cudaFree(h->comm_box);
-  if (h->arena) cudaFree(h->arena);
-  h->corr_ids.release();
-  for (VoxelMap* vm : {&h->map, &h->ndt_t, &h->ndt_s}) {
-    if (vm->d_counters) cudaFree(vm->d_counters);
-    if (vm->h_counters) cudaFreeHost(vm->h_counters);
-    if (vm->ev_attempt) cudaEventDestroy(vm->ev_attempt);
-    if (vm->ev_done) cudaEventDestroy(vm->ev_done);
-    vm->release();
-  }
-  h->ndt_src_pts.release(); h->ndt_src_covA.release(); h->ndt_src_covB.release();
-  h->crop_rank.release(); h->crop_state.release();
-  h->spare_pts.release(); h->spare_covA.release(); h->spare_covB.release();
-  for (int j = 0; j < 2; j++) { h->thin_keys[j].release(); h->thin_vals[j].release(); }
-  h->thin_scratch.release(); h->thin_keep.release(); h->thin_box.release();
-  h->carve_img.release();
-  h->eval.release();
-  h->multi.release();
-  if (h->d_multi_in) cudaFree(h->d_multi_in);
-  if (h->h_multi_in) cudaFreeHost(h->h_multi_in);
-  h->ct_times.release();
-  h->ct_spare.release();
-  h->ct_stats.release();
-  h->ct.release();
-  h->srcs.release();  // (the views into the pool are not freed here)
-  h->src_pts.release(); h->src_covA.release(); h->src_covB.release();
-  h->src_rows.release();
-  for (auto& r : h->prof_pending) { cudaEventDestroy(r.a); cudaEventDestroy(r.b); }
-  for (auto e : h->prof_pool) cudaEventDestroy(e);
-  for (cudaEvent_t e : {h->ev_copy, h->ev_append, h->ev_deskew, h->target.ready, h->source.ready, h->srcs.ready})
-    if (e) cudaEventDestroy(e);
-  if (h->s1.exec) cudaGraphExecDestroy(h->s1.exec);
-  if (h->stream_b) cudaStreamDestroy(h->stream_b);
-  if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
   return VGICP_OK;
 }
@@ -1498,8 +1451,8 @@ int vgicp_set_neighbor_search_method(vgicp_handle h, int method, double radius) 
   }
   CU_TRY(h, h->d_offsets.reserve(off.size()));
   if (!off.empty()) {
-    CU_TRY(h, cudaMemcpyAsync(h->d_offsets.p, off.data(), off.size() * sizeof(int4), cudaMemcpyHostToDevice, h->stream));
-    CU_TRY(h, cudaStreamSynchronize(h->stream));
+    CU_TRY(h, cudaMemcpyAsync(h->d_offsets.p, off.data(), off.size() * sizeof(int4), cudaMemcpyHostToDevice, h->stream.get()));
+    CU_TRY(h, cudaStreamSynchronize(h->stream.get()));
   }
   h->h_offsets.swap(off);
   h->offset_mode = mode;
@@ -1525,8 +1478,8 @@ int vgicp_swap_source_and_target(vgicp_handle h) {  // fast_vgicp_cuda.cu:97-107
   // stream, so it does not matter which one ends up where); everything in flight (incl. a pending map build that reads the old
   // target) must land first
   if (h->map.pending) { int rc0 = voxelmap_finish(h, h->target, h->map); if (rc0) return rc0; }
-  CU_TRY(h, cudaStreamSynchronize(h->stream));
-  CU_TRY(h, cudaStreamSynchronize(h->stream_b));
+  CU_TRY(h, cudaStreamSynchronize(h->stream.get()));
+  CU_TRY(h, cudaStreamSynchronize(h->stream_b.get()));
   clouds_swapped(h);
   if (h->problem != 0) return VGICP_OK;
   if (!h->target.has_pts || !h->target.has_cov) return VGICP_OK;
@@ -1729,10 +1682,10 @@ int vgicp_get_voxel_correspondences(vgicp_handle h, int* pairs, size_t cap, size
   if (total) {
     CU_TRY(h, h->corr_ids.reserve(total));
     KLAUNCH(h, VGICP_PROF_OTHER,
-            k_correspondence_ids<<<blocks_for(n, 128), 128, 0, h->stream>>>(LL.a.pts, n, LL.a.buckets, LL.a.mask, LL.a.max_scan, h->d_offsets.p, n_off, LL.a.res, h->lin, h->corr_ids.p));
+            k_correspondence_ids<<<blocks_for(n, 128), 128, 0, h->stream.get()>>>(LL.a.pts, n, LL.a.buckets, LL.a.mask, LL.a.max_scan, h->d_offsets.p, n_off, LL.a.res, h->lin, h->corr_ids.p));
     CU_TRY(h, cudaGetLastError());
-    CU_TRY(h, cudaMemcpyAsync(ids.data(), h->corr_ids.p, total * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-    CU_TRY(h, cudaStreamSynchronize(h->stream));
+    CU_TRY(h, cudaMemcpyAsync(ids.data(), h->corr_ids.p, total * sizeof(int), cudaMemcpyDeviceToHost, h->stream.get()));
+    CU_TRY(h, cudaStreamSynchronize(h->stream.get()));
   }
   size_t cnt = 0;
   for (int o = 0; o < n_off; o++)
@@ -1839,7 +1792,7 @@ int lm_rounds(vgicp_handle h, std::vector<LmState<6>>& st, const std::vector<Lin
       if ((rc = launch_multi(h, L, B, gr.lin ? kEvalLinearize : (speculate ? kEvalSpec : kEvalError), false, gr.row0, gr.n, src))) return rc;
     }
     if ((rc = h->multi.wait(h, round.n, (size_t)round.n * kMultiOut))) return rc;
-    const double* rec = h->multi.h_out;
+    const double* rec = h->multi.h_out.get();
     for (int r = 0; r < round.n; r++) lm_consume(&st[round.rows[r]], rec + (size_t)r * kMultiOut, r >= n_lin && speculate);
   }
 }
@@ -1881,7 +1834,7 @@ int vgicp_evaluate_poses(vgicp_handle h, const double* T, int n_poses, double* e
   if ((rc = round.upload())) return rc;
   if ((rc = launch_multi(h, L, B, want_H ? kEvalLinearize : kEvalError, true, 0, B, nullptr))) return rc;
   if ((rc = h->multi.wait(h, B, (size_t)B * kMultiOut))) return rc;
-  const double* rec = h->multi.h_out;
+  const double* rec = h->multi.h_out.get();
   for (int i = 0; i < B; i++) {
     const double* o = rec + (size_t)i * kMultiOut;
     err[i] = o[0];
@@ -1934,14 +1887,14 @@ int vgicp_align_sources(vgicp_handle h, const float* const* xyz, const size_t* n
   CU_TRY(h, h->src_rows.reserve(B));
   Cloud& c = h->srcs;
   if (!c.ready) {
-    CU_TRY(h, cudaEventCreateWithFlags(&c.ready, cudaEventDisableTiming));
-    c.st = h->stream_b;
+    CU_TRY(h, event_create(c.ready, cudaEventDisableTiming));
+    c.st = h->stream_b.get();
   }
   CU_TRY(h, c.nbr.reserve(n_max * k));  // (find_neighbors reserves as well; this keeps the buffers from growing source by source)
   CU_TRY(h, c.knn_scratch.reserve(knn_grid_scratch_bytes((int)n_max, nullptr, nullptr)));
   // the pool is rewritten on the cloud stream only after everything already enqueued on the main stream (which may read it)
-  CU_TRY(h, cudaEventRecord(c.ready, h->stream));
-  CU_TRY(h, cudaStreamWaitEvent(c.st, c.ready, 0));
+  CU_TRY(h, cudaEventRecord(c.ready.get(), h->stream.get()));
+  CU_TRY(h, cudaStreamWaitEvent(c.st, c.ready.get(), 0));
 
   // stage 1, source by source, and each source's launch shape and class: sources that share a kernel share the launches
   std::vector<SourceRow> desc(B);
@@ -1963,8 +1916,8 @@ int vgicp_align_sources(vgicp_handle h, const float* const* xyz, const size_t* n
     while (cls[i] < (int)classes.size() && !(classes[cls[i]].stream == L.stream && classes[cls[i]].G == L.G)) cls[i]++;
     if (cls[i] == (int)classes.size()) classes.push_back(L);
   }
-  CU_TRY(h, cudaMemcpyAsync(h->src_rows.p, desc.data(), sizeof(SourceRow) * B, cudaMemcpyHostToDevice, h->stream));
-  CU_TRY(h, cudaStreamWaitEvent(h->stream, c.ready, 0));
+  CU_TRY(h, cudaMemcpyAsync(h->src_rows.p, desc.data(), sizeof(SourceRow) * B, cudaMemcpyHostToDevice, h->stream.get()));
+  CU_TRY(h, cudaStreamWaitEvent(h->stream.get(), c.ready.get(), 0));
 
   std::vector<LmState<6>> st(B);
   const double I[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
@@ -2018,10 +1971,10 @@ static int stage1_enqueue(vgicp_handle h, int k, int reg) {
 // after a launch of the graph: the `ready` events were recorded inside the capture and mean nothing outside it; both clouds are
 // ready once the graph has run, and later work on a cloud stream must not overtake it
 static int stage1_graph_done(vgicp_handle h) {
-  CU_TRY(h, cudaEventRecord(h->map.ev_attempt, h->stream));
+  CU_TRY(h, cudaEventRecord(h->map.ev_attempt.get(), h->stream.get()));
   for (Cloud* c : {&h->target, &h->source}) {
-    CU_TRY(h, cudaEventRecord(c->ready, h->stream));
-    if (c->st != h->stream) CU_TRY(h, cudaStreamWaitEvent(c->st, c->ready, 0));
+    CU_TRY(h, cudaEventRecord(c->ready.get(), h->stream.get()));
+    if (c->st != h->stream.get()) CU_TRY(h, cudaStreamWaitEvent(c->st, c->ready.get(), 0));
   }
   return VGICP_OK;
 }
@@ -2033,8 +1986,8 @@ static int stage1_resident(vgicp_handle h, int k, int reg) {
   stage1_key(h, k, reg, key);
   if (G.exec && key == G.key) {
     for (Cloud* c : {&h->target, &h->source})  // the unpacks (eager, on the cloud streams)
-      if (c->st != h->stream) CU_TRY(h, cudaStreamWaitEvent(h->stream, c->ready, 0));
-    CU_TRY(h, cudaGraphLaunch(G.exec, h->stream));
+      if (c->st != h->stream.get()) CU_TRY(h, cudaStreamWaitEvent(h->stream.get(), c->ready.get(), 0));
+    CU_TRY(h, cudaGraphLaunch(G.exec.get(), h->stream.get()));
     // the host state the enqueue code leaves behind, as it left it when the graph was captured
     Cloud* cl[2] = {&h->target, &h->source};
     for (int j = 0; j < 2; j++) {
@@ -2054,30 +2007,30 @@ static int stage1_resident(vgicp_handle h, int k, int reg) {
     return VGICP_OK;
   }
   // second call with this key: every reserve is a no-op now, so the enqueue code only enqueues -- capture it
-  if (G.exec) { cudaGraphExecDestroy(G.exec); G.exec = nullptr; }
+  G.exec.reset();
   G.key.clear();
   const uint64_t l0 = h->launches;
   uint64_t p0[VGICP_PROF_NUM_CATEGORIES];
   memcpy(p0, h->prof_launches, sizeof(p0));
   for (Cloud* c : {&h->target, &h->source})
-    if (c->st != h->stream) CU_TRY(h, cudaStreamWaitEvent(h->stream, c->ready, 0));
+    if (c->st != h->stream.get()) CU_TRY(h, cudaStreamWaitEvent(h->stream.get(), c->ready.get(), 0));
   // thread-local: other host threads keep issuing their own work while this one captures
-  CU_TRY(h, cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeThreadLocal));
+  CU_TRY(h, cudaStreamBeginCapture(h->stream.get(), cudaStreamCaptureModeThreadLocal));
   int rc = VGICP_OK;
   cudaError_t e = cudaSuccess;
   for (Cloud* c : {&h->target, &h->source})  // fork: the cloud streams join the capture
-    if (c->st != h->stream && e == cudaSuccess && (e = cudaEventRecord(c->ready, h->stream)) == cudaSuccess) e = cudaStreamWaitEvent(c->st, c->ready, 0);
+    if (c->st != h->stream.get() && e == cudaSuccess && (e = cudaEventRecord(c->ready.get(), h->stream.get())) == cudaSuccess) e = cudaStreamWaitEvent(c->st, c->ready.get(), 0);
   if (e == cudaSuccess) rc = stage1_enqueue(h, k, reg);
   for (Cloud* c : {&h->target, &h->source})  // join (also after a failure: the capture must end with every stream joined)
-    if (c->st != h->stream) cudaStreamWaitEvent(h->stream, c->ready, 0);
+    if (c->st != h->stream.get()) cudaStreamWaitEvent(h->stream.get(), c->ready.get(), 0);
   cudaGraph_t graph = nullptr;
-  const cudaError_t ee = cudaStreamEndCapture(h->stream, &graph);
+  const cudaError_t ee = cudaStreamEndCapture(h->stream.get(), &graph);
   if (e == cudaSuccess) e = ee;
-  if (e == cudaSuccess && rc == VGICP_OK) e = cudaGraphInstantiate(&G.exec, graph, 0);
+  cudaGraphExec_t exec = nullptr;
+  if (e == cudaSuccess && rc == VGICP_OK && (e = cudaGraphInstantiate(&exec, graph, 0)) == cudaSuccess) G.exec.reset(exec);
   if (graph) cudaGraphDestroy(graph);
   if (rc) return rc;
   if (e != cudaSuccess) {
-    G.exec = nullptr;
     cudaGetLastError();
     return fail(h, VGICP_ERR_CUDA, std::string("register: stage-1 graph capture: ") + cudaGetErrorString(e));
   }
@@ -2087,7 +2040,7 @@ static int stage1_resident(vgicp_handle h, int k, int reg) {
   G.pending_B = h->map.pending_B;
   G.launches = h->launches - l0;
   for (int i = 0; i < VGICP_PROF_NUM_CATEGORIES; i++) G.prof_launches[i] = h->prof_launches[i] - p0[i];
-  CU_TRY(h, cudaGraphLaunch(G.exec, h->stream));
+  CU_TRY(h, cudaGraphLaunch(G.exec.get(), h->stream.get()));
   return stage1_graph_done(h);
 }
 
@@ -2114,14 +2067,14 @@ int vgicp_transform_source(vgicp_handle h, const double T[16], float* out_xyz, s
   const int n = h->source.n;
   if (cap < (size_t)n || stride < 12 || stride % 4) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "transform_source: bad capacity/stride");
   if (n == 0) return VGICP_OK;
-  if (h->source.st != h->stream) CU_TRY(h, cudaStreamWaitEvent(h->stream, h->source.ready, 0));
+  if (h->source.st != h->stream.get()) CU_TRY(h, cudaStreamWaitEvent(h->stream.get(), h->source.ready.get(), 0));
   CU_TRY(h, h->staging.reserve((size_t)n * stride));
   // keep the non-xyz bytes of the caller's records untouched: copy in, overwrite xyz, copy out
-  if (stride > 12) CU_TRY(h, cudaMemcpyAsync(h->staging.p, out_xyz, (size_t)n * stride, cudaMemcpyHostToDevice, h->stream));
-  KLAUNCH(h, VGICP_PROF_OTHER, k_transform_points<<<blocks_for(n, 256), 256, 0, h->stream>>>(h->source.pts.p, n, to_pose(T), h->staging.p, stride));
+  if (stride > 12) CU_TRY(h, cudaMemcpyAsync(h->staging.p, out_xyz, (size_t)n * stride, cudaMemcpyHostToDevice, h->stream.get()));
+  KLAUNCH(h, VGICP_PROF_OTHER, k_transform_points<<<blocks_for(n, 256), 256, 0, h->stream.get()>>>(h->source.pts.p, n, to_pose(T), h->staging.p, stride));
   CU_TRY(h, cudaGetLastError());
-  CU_TRY(h, cudaMemcpyAsync(out_xyz, h->staging.p, (size_t)n * stride, cudaMemcpyDeviceToHost, h->stream));
-  CU_TRY(h, cudaStreamSynchronize(h->stream));
+  CU_TRY(h, cudaMemcpyAsync(out_xyz, h->staging.p, (size_t)n * stride, cudaMemcpyDeviceToHost, h->stream.get()));
+  CU_TRY(h, cudaStreamSynchronize(h->stream.get()));
   return VGICP_OK;
 }
 
@@ -2153,7 +2106,7 @@ static int local_map_rebuild(vgicp_handle h) {
   points_changed(h, t, Change::edited);
   int rc = voxelmap_begin(h, t, h->map);
   if (rc) return rc;
-  CU_TRY(h, cudaEventRecord(t.ready, t.st));
+  CU_TRY(h, cudaEventRecord(t.ready.get(), t.st));
   return VGICP_OK;
 }
 
@@ -2170,7 +2123,7 @@ int vgicp_append_source_to_target(vgicp_handle h, const double T[16]) {
   if (!s.has_pts || !s.has_cov) return fail(h, VGICP_ERR_BAD_STATE, "append_source_to_target: source points and covariances required");
   const size_t n = (size_t)t.n + (size_t)s.n;
   if (n > (size_t)0x7fffffff / 64) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "append_source_to_target: the merged target would exceed the points a cloud may hold");
-  if (s.st != t.st) CU_TRY(h, cudaStreamWaitEvent(t.st, s.ready, 0));
+  if (s.st != t.st) CU_TRY(h, cudaStreamWaitEvent(t.st, s.ready.get(), 0));
   CU_TRY(h, t.pts.grow(n, t.n, t.st));
   CU_TRY(h, t.covA.grow(n, t.n, t.st));
   CU_TRY(h, t.covB.grow(n, t.n, t.st));
@@ -2179,8 +2132,8 @@ int vgicp_append_source_to_target(vgicp_handle h, const double T[16]) {
                k_append_transformed<<<blocks_for(s.n, 256), 256, 0, t.st>>>(s.pts.p, s.covA.p, s.covB.p, s.n, to_pose(T), t.pts.p + t.n, t.covA.p + t.n, t.covB.p + t.n));
     CU_TRY(h, cudaGetLastError());
     // the next upload into the source's arrays (on the source's stream) must not overtake this read of them
-    CU_TRY(h, cudaEventRecord(h->ev_append, t.st));
-    if (s.st != t.st) CU_TRY(h, cudaStreamWaitEvent(s.st, h->ev_append, 0));
+    CU_TRY(h, cudaEventRecord(h->ev_append.get(), t.st));
+    if (s.st != t.st) CU_TRY(h, cudaStreamWaitEvent(s.st, h->ev_append.get(), 0));
   }
   t.n = (int)n;
   return local_map_rebuild(h);
@@ -2197,12 +2150,12 @@ static int local_map_rank(vgicp_handle h, const unsigned char* keep, float cx, f
   CU_TRY(h, h->spare_pts.reserve(n));
   CU_TRY(h, h->spare_covA.reserve(n));
   CU_TRY(h, h->spare_covB.reserve(n));
-  int* d_count = h->map.d_counters + 10;
+  int* d_count = h->map.d_counters.get() + 10;
   KLAUNCH_ST(h, t.st, VGICP_PROF_OTHER,
              k_crop_rank<<<blocks, kRankThreads, 0, t.st>>>(t.pts.p, keep, n, cx, cy, cz, r2, h->crop_rank.p, d_count, h->crop_state.p, h->crop_epoch));
   CU_TRY(h, cudaGetLastError());
   // the host needs the new size (and must refuse an empty result before anything is modified)
-  CU_TRY(h, cudaMemcpyAsync(h->map.h_counters + 10, d_count, sizeof(int), cudaMemcpyDeviceToHost, t.st));
+  CU_TRY(h, cudaMemcpyAsync(h->map.h_counters.get() + 10, d_count, sizeof(int), cudaMemcpyDeviceToHost, t.st));
   CU_TRY(h, cudaStreamSynchronize(t.st));
   *passed = (size_t)h->map.h_counters[10];
   return VGICP_OK;
@@ -2367,11 +2320,11 @@ int vgicp_carve_target(vgicp_handle h, const double T[16], const vgicp_carve_par
   CU_TRY(h, h->thin_keep.reserve(n));
   // 1. the range image, from the source on the target's stream; the next upload into the source must not overtake this read
   CU_TRY(h, cudaMemsetAsync(h->carve_img.p, 0xFF, pixels * sizeof(unsigned), t.st));
-  if (s.st != t.st) CU_TRY(h, cudaStreamWaitEvent(t.st, s.ready, 0));
+  if (s.st != t.st) CU_TRY(h, cudaStreamWaitEvent(t.st, s.ready.get(), 0));
   KLAUNCH_ST(h, t.st, VGICP_PROF_OTHER, k_carve_image<<<blocks_for(s.n, 256), 256, 0, t.st>>>(s.pts.p, s.n, im, h->carve_img.p));
   CU_TRY(h, cudaGetLastError());
-  CU_TRY(h, cudaEventRecord(h->ev_append, t.st));
-  if (s.st != t.st) CU_TRY(h, cudaStreamWaitEvent(s.st, h->ev_append, 0));
+  CU_TRY(h, cudaEventRecord(h->ev_append.get(), t.st));
+  if (s.st != t.st) CU_TRY(h, cudaStreamWaitEvent(s.st, h->ev_append.get(), 0));
   // 2. the keep mask; 3. thinning's compaction with it (the mask alone decides: a non-finite point it keeps stays)
   KLAUNCH_ST(h, t.st, VGICP_PROF_OTHER,
              k_carve_keep<<<blocks_for(n, 256), 256, 0, t.st>>>(t.pts.p, n, Ti, im, h->carve_img.p, P.window, (float)P.margin, (float)P.margin_rel, h->thin_keep.p));
@@ -2429,16 +2382,16 @@ static int deskew_enqueue(vgicp_handle h, const char* who, const float* d_t, con
   const double omega = sqrt(twist[0] * twist[0] + twist[1] * twist[1] + twist[2] * twist[2]);
   if (omega * span > 1.5707963267948966)
     return fail(h, VGICP_ERR_INVALID_ARGUMENT, std::string(who) + ": the rotation over the sweep exceeds pi/2 (|omega| * max |t_i - t_ref|), beyond the series");
-  if (s.st != h->stream) {
-    if (!h->ev_deskew) CU_TRY(h, cudaEventCreateWithFlags(&h->ev_deskew, cudaEventDisableTiming));
-    CU_TRY(h, cudaEventRecord(h->ev_deskew, h->stream));
-    CU_TRY(h, cudaStreamWaitEvent(s.st, h->ev_deskew, 0));
+  if (s.st != h->stream.get()) {
+    if (!h->ev_deskew) CU_TRY(h, event_create(h->ev_deskew, cudaEventDisableTiming));
+    CU_TRY(h, cudaEventRecord(h->ev_deskew.get(), h->stream.get()));
+    CU_TRY(h, cudaStreamWaitEvent(s.st, h->ev_deskew.get(), 0));
   }
-  if (s.st != h->target.st) CU_TRY(h, cudaStreamWaitEvent(s.st, h->ev_append, 0));
+  if (s.st != h->target.st) CU_TRY(h, cudaStreamWaitEvent(s.st, h->ev_append.get(), 0));
   KLAUNCH_ST(h, s.st, VGICP_PROF_OTHER,
              k_deskew_points<<<blocks_for(s.n, 256), 256, 0, s.st>>>(s.pts.p, d_t, s.n, (float)t_ref, xi[0], xi[1], xi[2], xi[3], xi[4], xi[5]));
   CU_TRY(h, cudaGetLastError());
-  CU_TRY(h, cudaEventRecord(s.ready, s.st));
+  CU_TRY(h, cudaEventRecord(s.ready.get(), s.st));
   points_changed(h, s, Change::moved);
   return VGICP_OK;
 }
@@ -2456,10 +2409,10 @@ int vgicp_deskew_source(vgicp_handle h, const float* t, size_t n, size_t stride_
   Cloud& s = h->source;
   CU_TRY(h, s.staging.reserve(n * sizeof(float)));
   CU_TRY(h, cudaMemcpyAsync(s.staging.p, packed.data(), n * sizeof(float), cudaMemcpyHostToDevice, s.st));
-  CU_TRY(h, cudaEventRecord(h->ev_copy, s.st));
+  CU_TRY(h, cudaEventRecord(h->ev_copy.get(), s.st));
   rc = deskew_enqueue(h, "deskew_source", reinterpret_cast<const float*>(s.staging.p), twist, lo, hi, t_ref);
   // the packed timestamps are reused by the next call: the copy out of them must have landed
-  CU_TRY(h, cudaEventSynchronize(h->ev_copy));
+  CU_TRY(h, cudaEventSynchronize(h->ev_copy.get()));
   return rc;
 }
 
@@ -2475,8 +2428,8 @@ int vgicp_set_source_timestamps(vgicp_handle h, const float* t, size_t n, size_t
   if ((rc = timestamps_pack(h, "set_source_timestamps", t, n, stride_bytes, packed, &lo, &hi))) return rc;
   return timestamps_commit(h, "set_source_timestamps", lo, hi, t_ref, [&]() -> int {
     CU_TRY(h, h->ct_times.reserve(n));
-    CU_TRY(h, cudaMemcpyAsync(h->ct_times.p, packed.data(), n * sizeof(float), cudaMemcpyHostToDevice, h->stream));
-    CU_TRY(h, cudaStreamSynchronize(h->stream));  // (`packed` goes out of scope)
+    CU_TRY(h, cudaMemcpyAsync(h->ct_times.p, packed.data(), n * sizeof(float), cudaMemcpyHostToDevice, h->stream.get()));
+    CU_TRY(h, cudaStreamSynchronize(h->stream.get()));  // (`packed` goes out of scope)
     return VGICP_OK;
   });
 }
@@ -2492,16 +2445,16 @@ int vgicp_set_source_timestamps_device(vgicp_handle h, const float* d_t, size_t 
   // after the source's pending work (a set_source_cloud_device read of the same buffer): the readback below then also tells the
   // caller that buffer is free
   const Cloud& s = h->source;
-  if (s.st != h->stream && s.ready) CU_TRY(h, cudaStreamWaitEvent(h->stream, s.ready, 0));
+  if (s.st != h->stream.get() && s.ready) CU_TRY(h, cudaStreamWaitEvent(h->stream.get(), s.ready.get(), 0));
   CU_TRY(h, h->ct_spare.reserve(n));
   CU_TRY(h, h->ct_stats.reserve(3));
-  CU_TRY(h, cudaMemsetAsync(h->ct_stats.p, 0, 3 * sizeof(unsigned), h->stream));
+  CU_TRY(h, cudaMemsetAsync(h->ct_stats.p, 0, 3 * sizeof(unsigned), h->stream.get()));
   KLAUNCH(h, VGICP_PROF_OTHER,
-          k_gather_times<<<blocks_for(n, 256), 256, 0, h->stream>>>(reinterpret_cast<const unsigned char*>(d_t), stride_bytes, (int)n, h->ct_spare.p, h->ct_stats.p));
+          k_gather_times<<<blocks_for(n, 256), 256, 0, h->stream.get()>>>(reinterpret_cast<const unsigned char*>(d_t), stride_bytes, (int)n, h->ct_spare.p, h->ct_stats.p));
   CU_TRY(h, cudaGetLastError());
   unsigned st[3];
-  CU_TRY(h, cudaMemcpyAsync(st, h->ct_stats.p, sizeof(st), cudaMemcpyDeviceToHost, h->stream));
-  CU_TRY(h, cudaStreamSynchronize(h->stream));  // (the caller may reuse d_t after return)
+  CU_TRY(h, cudaMemcpyAsync(st, h->ct_stats.p, sizeof(st), cudaMemcpyDeviceToHost, h->stream.get()));
+  CU_TRY(h, cudaStreamSynchronize(h->stream.get()));  // (the caller may reuse d_t after return)
   if (st[0]) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "set_source_timestamps_device: non-finite timestamp");
   auto from_key = [](unsigned k) {
     const unsigned b = (k & 0x80000000u) ? (k & 0x7fffffffu) : ~k;
@@ -2526,7 +2479,7 @@ int vgicp_deskew_source_stored(vgicp_handle h, const double twist[6]) {
   if (!rc) rc = deskew_enqueue(h, "deskew_source_stored", h->ct_times.p, twist, h->ct_lo, h->ct_hi, h->ct_t_ref);
   if (rc) return rc;
   // the next write of the timestamp buffers (on the main stream) must not overtake this read of ct_times
-  if (h->source.st != h->stream) CU_TRY(h, cudaStreamWaitEvent(h->stream, h->source.ready, 0));
+  if (h->source.st != h->stream.get()) CU_TRY(h, cudaStreamWaitEvent(h->stream.get(), h->source.ready.get(), 0));
   return VGICP_OK;
 }
 
@@ -2543,7 +2496,7 @@ int vgicp_compute_error_ct(vgicp_handle h, const double T_lin[16], const double 
   if (!twist_in_series(xi_lin, h->ct_span) || !twist_in_series(xi_eval, h->ct_span))
     return fail(h, VGICP_ERR_INVALID_ARGUMENT, "compute_error_ct: the rotation over the sweep (|omega| * max |s_i|) exceeds pi/2, beyond the series");
   if ((rc = sync_inputs(h))) return rc;
-  CU_TRY(h, h->ct.open(1, kCtStride, (size_t)kLinMaxBlocks * kCtStride, h->stream));
+  CU_TRY(h, h->ct.open(1, kCtStride, (size_t)kLinMaxBlocks * kCtStride, h->stream.get()));
   const bool want_H = H144 != nullptr;
   const double* raw = nullptr;
   if ((rc = ct_evaluate(h, T_lin, xi_lin, T_eval, xi_eval, want_H, &raw))) return rc;
@@ -2569,7 +2522,7 @@ int vgicp_align_ct(vgicp_handle h, const double guess[16], const double twist_gu
     return fail(h, VGICP_ERR_INVALID_ARGUMENT, "align_ct: the twist guess or prior rotates more than pi/2 over the sweep (|omega| * max |s_i|), beyond the series");
   const vgicp_lsq_params P = lsq_params(params);
   if ((rc = sync_inputs(h))) return rc;
-  CU_TRY(h, h->ct.open(1, kCtStride, (size_t)kLinMaxBlocks * kCtStride, h->stream));
+  CU_TRY(h, h->ct.open(1, kCtStride, (size_t)kLinMaxBlocks * kCtStride, h->stream.get()));
   LmState<12> st = lm_init<12>(guess, P);
   memcpy(st.tw0, twist_guess, sizeof(st.tw0));
   st.span = h->ct_span;
@@ -2604,11 +2557,11 @@ int vgicp_comm_export(vgicp_handle h, unsigned char* handle64) {
   if (!handle64) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "comm_export: null buffer");
   static_assert(sizeof(cudaIpcMemHandle_t) == 64, "cudaIpcMemHandle_t is 64 bytes");
   if (!h->comm_box) {
-    CU_TRY(h, cudaMalloc(&h->comm_box, sizeof(CommMailbox)));
-    CU_TRY(h, cudaMemset(h->comm_box, 0, sizeof(CommMailbox)));
+    CU_TRY(h, device_alloc(h->comm_box, sizeof(CommMailbox)));
+    CU_TRY(h, cudaMemset(h->comm_box.get(), 0, sizeof(CommMailbox)));
   }
   cudaIpcMemHandle_t ipc;
-  CU_TRY(h, cudaIpcGetMemHandle(&ipc, h->comm_box));
+  CU_TRY(h, cudaIpcGetMemHandle(&ipc, h->comm_box.get()));
   memcpy(handle64, &ipc, 64);
   return VGICP_OK;
 }
@@ -2618,23 +2571,25 @@ int vgicp_comm_init(vgicp_handle h, int rank, int nranks, const unsigned char* a
   DeviceGuard g(h->device);
   if (nranks < 1 || nranks > kCommMaxRanks || rank < 0 || rank >= nranks || !all_handles) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "comm_init: need 1 <= nranks <= 8 and all handles");
   if (!h->comm_box) return fail(h, VGICP_ERR_BAD_STATE, "comm_init: call vgicp_comm_export first");
+  IpcPtr<CommMailbox> peers[kCommMaxRanks];  // (closed again if a later rank fails)
   for (int r = 0; r < nranks; r++) {
-    if (r == rank) { h->comm_peers[r] = h->comm_box; continue; }
+    if (r == rank) continue;
     cudaIpcMemHandle_t ipc;
     memcpy(&ipc, all_handles + (size_t)r * 64, 64);
     void* p = nullptr;
     cudaError_t e = cudaIpcOpenMemHandle(&p, ipc, cudaIpcMemLazyEnablePeerAccess);
     if (e != cudaSuccess) return fail(h, VGICP_ERR_COMM, std::string("comm_init: cudaIpcOpenMemHandle: ") + cudaGetErrorString(e));
-    h->comm_peers[r] = reinterpret_cast<CommMailbox*>(p);
+    peers[r].reset(static_cast<CommMailbox*>(p));
   }
+  for (int r = 0; r < kCommMaxRanks; r++) h->comm_peers[r] = std::move(peers[r]);
   h->comm_rank = rank;
   h->comm_ranks = nranks;
   h->comm_seq = 0;
   // the mailbox outlives vgicp_comm_shutdown: flags left by a previous session could equal the first tags of this one.  Clear it
   // here; the caller puts a host barrier between vgicp_comm_init on all ranks and the first evaluation (see the header), so no
   // peer writes into it before the clear has landed.
-  CU_TRY(h, cudaMemsetAsync(h->comm_box, 0, sizeof(CommMailbox), h->stream));
-  CU_TRY(h, cudaStreamSynchronize(h->stream));
+  CU_TRY(h, cudaMemsetAsync(h->comm_box.get(), 0, sizeof(CommMailbox), h->stream.get()));
+  CU_TRY(h, cudaStreamSynchronize(h->stream.get()));
   return VGICP_OK;
 }
 
@@ -2646,16 +2601,16 @@ int vgicp_comm_export_arena(vgicp_handle h, size_t max_points, unsigned char* ha
   max_points = (max_points + 15) & ~(size_t)15;  // the two clouds' float4 / float2 arrays follow each other: keep every array 16-byte aligned
   if (h->arena && h->arena_points != max_points) return fail(h, VGICP_ERR_BAD_STATE, "comm_export_arena: arena already allocated with another capacity");
   if (!h->arena) {
-    CU_TRY(h, cudaStreamSynchronize(h->stream));
-    CU_TRY(h, cudaStreamSynchronize(h->stream_b));
+    CU_TRY(h, cudaStreamSynchronize(h->stream.get()));
+    CU_TRY(h, cudaStreamSynchronize(h->stream_b.get()));
     const size_t bytes = kCommArenaHeaderBytes + 2 * max_points * 24 + 64;  // (+ padding: bulk copies read covB in 16-byte units)
-    CU_TRY(h, cudaMalloc(&h->arena, bytes));
-    CU_TRY(h, cudaMemset(h->arena, 0, bytes));
+    CU_TRY(h, device_alloc(h->arena, bytes));
+    CU_TRY(h, cudaMemset(h->arena.get(), 0, bytes));
     h->arena_points = max_points;
     // the covariance arrays of both clouds now live in the arena (previous covariances are dropped)
     Cloud* cl[2] = {&h->target, &h->source};
     for (int j = 0; j < 2; j++) {
-      unsigned char* base = h->arena + kCommArenaHeaderBytes + (size_t)j * max_points * 24;
+      unsigned char* base = h->arena.get() + kCommArenaHeaderBytes + (size_t)j * max_points * 24;
       cl[j]->covA.attach(reinterpret_cast<float4*>(base), max_points);
       cl[j]->covB.attach(reinterpret_cast<float2*>(base + max_points * 16), max_points);
       cl[j]->arena_slot = j;
@@ -2664,7 +2619,7 @@ int vgicp_comm_export_arena(vgicp_handle h, size_t max_points, unsigned char* ha
     covariances_dropped(h);
   }
   cudaIpcMemHandle_t ipc;
-  CU_TRY(h, cudaIpcGetMemHandle(&ipc, h->arena));
+  CU_TRY(h, cudaIpcGetMemHandle(&ipc, h->arena.get()));
   memcpy(handle64, &ipc, 64);
   return VGICP_OK;
 }
@@ -2674,15 +2629,18 @@ int vgicp_comm_init_arena(vgicp_handle h, const unsigned char* all_handles) {
   DeviceGuard g(h->device);
   if (!all_handles) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "comm_init_arena: null handles");
   if (h->comm_ranks < 1 || !h->arena) return fail(h, VGICP_ERR_BAD_STATE, "comm_init_arena: call vgicp_comm_init and vgicp_comm_export_arena first");
+  IpcPtr<unsigned char[]> peers[kCommMaxRanks];  // (closed again if a later rank fails)
   for (int r = 0; r < h->comm_ranks; r++) {
-    if (r == h->comm_rank) { h->arena_peers[r] = h->arena; continue; }
+    if (r == h->comm_rank) continue;
     cudaIpcMemHandle_t ipc;
     memcpy(&ipc, all_handles + (size_t)r * 64, 64);
     void* p = nullptr;
     cudaError_t e = cudaIpcOpenMemHandle(&p, ipc, cudaIpcMemLazyEnablePeerAccess);
     if (e != cudaSuccess) return fail(h, VGICP_ERR_COMM, std::string("comm_init_arena: cudaIpcOpenMemHandle: ") + cudaGetErrorString(e));
-    h->arena_peers[r] = reinterpret_cast<unsigned char*>(p);
+    peers[r].reset(static_cast<unsigned char*>(p));
   }
+  for (int r = 0; r < kCommMaxRanks; r++) h->arena_peers[r] = std::move(peers[r]);
+  h->arena_mapped = true;
   return VGICP_OK;
 }
 
@@ -2695,14 +2653,11 @@ int vgicp_set_stage1_sharding(vgicp_handle h, int enable) {
 int vgicp_comm_shutdown(vgicp_handle h) {
   CHECK_HANDLE(h);
   DeviceGuard g(h->device);
-  if (h->stream) cudaStreamSynchronize(h->stream);
-  if (h->stream_b) cudaStreamSynchronize(h->stream_b);
-  for (int r = 0; r < h->comm_ranks; r++)
-    if (r != h->comm_rank && h->arena_peers[r]) cudaIpcCloseMemHandle(h->arena_peers[r]);
-  for (int r = 0; r < kCommMaxRanks; r++) h->arena_peers[r] = nullptr;
-  for (int r = 0; r < h->comm_ranks; r++)
-    if (r != h->comm_rank && h->comm_peers[r]) cudaIpcCloseMemHandle(h->comm_peers[r]);
-  for (int r = 0; r < kCommMaxRanks; r++) h->comm_peers[r] = nullptr;
+  if (h->stream) cudaStreamSynchronize(h->stream.get());
+  if (h->stream_b) cudaStreamSynchronize(h->stream_b.get());
+  for (auto& p : h->arena_peers) p.reset();
+  for (auto& p : h->comm_peers) p.reset();
+  h->arena_mapped = false;
   h->comm_ranks = 0;
   h->comm_rank = 0;
   return VGICP_OK;
@@ -2715,12 +2670,12 @@ int vgicp_comm_error(vgicp_handle h, int* error) {
   *error = 0;
   if (h->comm_box) {
     CommMailbox tmp;
-    CU_TRY(h, cudaMemcpy(&tmp, h->comm_box, sizeof(CommMailbox), cudaMemcpyDeviceToHost));
+    CU_TRY(h, cudaMemcpy(&tmp, h->comm_box.get(), sizeof(CommMailbox), cudaMemcpyDeviceToHost));
     *error = tmp.error;
   }
   if (h->arena) {
     CommArenaHeader hdr;
-    CU_TRY(h, cudaMemcpy(&hdr, h->arena, sizeof(hdr), cudaMemcpyDeviceToHost));
+    CU_TRY(h, cudaMemcpy(&hdr, h->arena.get(), sizeof(hdr), cudaMemcpyDeviceToHost));
     *error |= hdr.error;
   }
   return VGICP_OK;
@@ -2779,9 +2734,9 @@ int vgicp_set_voxel_index(vgicp_handle h, int mode) {
 int vgicp_set_profiling(vgicp_handle h, int enable) {
   CHECK_HANDLE(h);
   DeviceGuard g(h->device);
-  CU_TRY(h, cudaStreamSynchronize(h->stream_b));
-  CU_TRY(h, cudaStreamSynchronize(h->stream));
-  for (auto& r : h->prof_pending) { h->prof_pool.push_back(r.a); h->prof_pool.push_back(r.b); }
+  CU_TRY(h, cudaStreamSynchronize(h->stream_b.get()));
+  CU_TRY(h, cudaStreamSynchronize(h->stream.get()));
+  for (auto& r : h->prof_pending) { h->prof_pool.push_back(std::move(r.a)); h->prof_pool.push_back(std::move(r.b)); }
   h->prof_pending.clear();
   for (int i = 0; i < VGICP_PROF_NUM_CATEGORIES; i++) { h->prof_ms[i] = 0.0; h->prof_launches[i] = 0; }
   h->prof_on = enable != 0;
@@ -2792,13 +2747,13 @@ int vgicp_get_profile(vgicp_handle h, double* ms, uint64_t* launches, int capaci
   CHECK_HANDLE(h);
   DeviceGuard g(h->device);
   if (!ms || !launches || capacity < VGICP_PROF_NUM_CATEGORIES) return fail(h, VGICP_ERR_INVALID_ARGUMENT, "get_profile: need VGICP_PROF_NUM_CATEGORIES entries");
-  CU_TRY(h, cudaStreamSynchronize(h->stream_b));
-  CU_TRY(h, cudaStreamSynchronize(h->stream));
+  CU_TRY(h, cudaStreamSynchronize(h->stream_b.get()));
+  CU_TRY(h, cudaStreamSynchronize(h->stream.get()));
   for (auto& r : h->prof_pending) {
     float t = 0.f;
-    if (cudaEventElapsedTime(&t, r.a, r.b) == cudaSuccess) h->prof_ms[r.cat] += (double)t;
-    h->prof_pool.push_back(r.a);
-    h->prof_pool.push_back(r.b);
+    if (cudaEventElapsedTime(&t, r.a.get(), r.b.get()) == cudaSuccess) h->prof_ms[r.cat] += (double)t;
+    h->prof_pool.push_back(std::move(r.a));
+    h->prof_pool.push_back(std::move(r.b));
   }
   h->prof_pending.clear();
   for (int i = 0; i < VGICP_PROF_NUM_CATEGORIES; i++) { ms[i] = h->prof_ms[i]; launches[i] = h->prof_launches[i]; }
@@ -2820,15 +2775,15 @@ int vgicp_get_fitness_score(vgicp_handle h, const double T[16], double max_range
   const int n = h->source.n;
   *score = std::numeric_limits<double>::max();
   if (n == 0 || h->target.n == 0) return VGICP_OK;
-  if (h->source.st != h->stream) CU_TRY(h, cudaStreamWaitEvent(h->stream, h->source.ready, 0));
-  if (h->target.st != h->stream) CU_TRY(h, cudaStreamWaitEvent(h->stream, h->target.ready, 0));
+  if (h->source.st != h->stream.get()) CU_TRY(h, cudaStreamWaitEvent(h->stream.get(), h->source.ready.get(), 0));
+  if (h->target.st != h->stream.get()) CU_TRY(h, cudaStreamWaitEvent(h->stream.get(), h->target.ready.get(), 0));
   CU_TRY(h, h->staging.reserve((size_t)n * sizeof(float)));
   float* d_out = reinterpret_cast<float*>(h->staging.p);
-  KLAUNCH(h, VGICP_PROF_OTHER, k_nn1_sqdist<<<blocks_for(n, 256), 256, 0, h->stream>>>(h->source.pts.p, n, h->target.pts.p, h->target.n, to_pose(T), d_out));
+  KLAUNCH(h, VGICP_PROF_OTHER, k_nn1_sqdist<<<blocks_for(n, 256), 256, 0, h->stream.get()>>>(h->source.pts.p, n, h->target.pts.p, h->target.n, to_pose(T), d_out));
   CU_TRY(h, cudaGetLastError());
   std::vector<float> d2(n);
-  CU_TRY(h, cudaMemcpyAsync(d2.data(), d_out, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
-  CU_TRY(h, cudaStreamSynchronize(h->stream));
+  CU_TRY(h, cudaMemcpyAsync(d2.data(), d_out, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, h->stream.get()));
+  CU_TRY(h, cudaStreamSynchronize(h->stream.get()));
   double sum = 0.0;
   long cnt = 0;
   for (int i = 0; i < n; i++)
@@ -2848,15 +2803,15 @@ int vgicp_synchronize(vgicp_handle h) {
   CHECK_HANDLE(h);
   DeviceGuard g(h->device);
   if (h->map.pending) { int rc = voxelmap_finish(h, h->target, h->map); if (rc) return rc; }
-  CU_TRY(h, cudaStreamSynchronize(h->stream_b));
-  CU_TRY(h, cudaStreamSynchronize(h->stream));
+  CU_TRY(h, cudaStreamSynchronize(h->stream_b.get()));
+  CU_TRY(h, cudaStreamSynchronize(h->stream.get()));
   return VGICP_OK;
 }
 
 int vgicp_get_stream(vgicp_handle h, uint64_t* stream) {
   CHECK_HANDLE(h);
   if (!stream) return VGICP_ERR_INVALID_ARGUMENT;
-  *stream = (uint64_t)(uintptr_t)h->stream;
+  *stream = (uint64_t)(uintptr_t)h->stream.get();
   return VGICP_OK;
 }
 

@@ -1,7 +1,9 @@
 #!/bin/bash
 # compute-sanitizer passes over the hot path: memcheck + racecheck + synccheck on one full registration per neighbour mode,
 # on both k-NN search paths, and on all four users of the shared block rank (voxel ids, crop and thinning, both voxel grids).
-# One log per tool, written by the loop at the end.
+# memcheck also reports every allocation left at exit and every failing CUDA call; the driver ends by destroying a handle in each
+# state that holds a lazily created resource, and empties torch's cache so that only the libraries' own allocations remain.
+# One log per tool, written by the loop at the end into the directory given as the first argument.
 set -u
 cat > /tmp/san_driver.py <<'PY'
 import sys, numpy as np
@@ -107,8 +109,22 @@ for n in (1, 513, 4097):
     c.set_source_cloud(np.ascontiguousarray(d["target"][:n])); c.calculate_source_covariances_rbf(3)
     print("rbf", n, "finite", bool(np.isfinite(c.get_source_covariances()).all()))
 c.close()
+# handle lifetime: every state with a lazily created resource (multi-pose, multi-source, deskew, CT, profiling, stage-1 graph,
+# pending voxel map, thin and carve, the exact grid), destroyed there
+sys.path.insert(0, "tests")
+from test_gpu_handle_lifetime import STATES
+t32, s32 = np.ascontiguousarray(tgt[:, :3], np.float32), np.ascontiguousarray(src[:, :3], np.float32)
+for state in STATES:
+    state(torch, t32, s32).close()
+    print("lifetime", state.__name__, "closed")
+torch.cuda.empty_cache()
 PY
+out=${1:-/tmp/vgicp_sanitizer}  # the directory the logs go to (first argument)
+mkdir -p "$out"
 for tool in memcheck racecheck synccheck; do
-  timeout 900 compute-sanitizer --tool $tool --print-limit 20 python /tmp/san_driver.py > gpurun_out/r02_sanitizer_$tool.log 2>&1
-  echo "== $tool: $(grep -E 'ERROR SUMMARY|RACECHECK SUMMARY' gpurun_out/r02_sanitizer_$tool.log | tail -1)"
+  extra=""
+  [ $tool = memcheck ] && extra="--leak-check full --report-api-errors all"
+  log="$out/sanitizer_$tool.log"
+  timeout 900 compute-sanitizer --tool $tool $extra --print-limit 20 python /tmp/san_driver.py > "$log" 2>&1
+  echo "== $tool: $(grep -E 'ERROR SUMMARY|RACECHECK SUMMARY' "$log" | tail -1)"
 done
